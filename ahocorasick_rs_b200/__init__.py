@@ -1,8 +1,8 @@
-"""B200-native multi-pattern matcher with the ``ahocorasick_rs`` Python API.
+"""H100-native multi-pattern matcher with the ``ahocorasick_rs`` Python API.
 
-Mirrors /root/reference/pysrc/ahocorasick_rs/__init__.py:1-23 (same exported
+Mirrors the reference's pysrc/ahocorasick_rs/__init__.py:1-23 (same exported
 names, including the deprecated MATCHKIND_* constants); the scan runs in
-hand-written sm_100a CUDA kernels behind the C ABI in include/acb200.h."""
+hand-written sm_90a CUDA kernels behind the C ABI in include/acb200.h."""
 from .matcher import AhoCorasick, BytesAhoCorasick, MatchKind, Implementation
 
 # Backwards compatibility (reference: pysrc/ahocorasick_rs/__init__.py:10-12)

@@ -54,7 +54,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). ahocorasick_rs_b200 has no CPU fallback.")
+                "(nvcc, sm_90a). ahocorasick_rs_b200 has no CPU fallback.")
         L = C.CDLL(LIB_PATH)
         L.acb_last_error.restype = C.c_char_p
         L.acb_version.restype = C.c_char_p

@@ -677,7 +677,7 @@ static int fail(int code, const std::string &msg) {
 extern "C" {
 
 const char *acb_last_error(void) { return g_err.c_str(); }
-const char *acb_version(void) { return "acb200 0.2 (sm_100a)"; }
+const char *acb_version(void) { return "acb200 0.2 (sm_90a)"; }
 uint64_t acb_launch_count(void) { return g_launches.load(); }
 
 int acb_timing_enable(int on) {
@@ -940,7 +940,7 @@ int launch_staged(const DevImage &im, const DevHot &hot, const Batch &B, const S
     int warps = (int)((tasks + ctas - 1) / ctas);
     if (warps < 4) warps = 4;
     // as many warps as fit: the scan is a chain of dependent shared-memory loads per lane, more warps hide more of
-    // it (measured 26 -> 32 warps: 170 -> 164 us); balancing the last round of tasks instead was not better
+    // it; balancing the last round of tasks instead was not better
     if (warps > kWarpsMax) warps = kWarpsMax;
     const uint32_t row_bytes = COLMODE == kColAscii ? kAsciiCols * 2 : im.n_cols * 2;
     const uint32_t stage_bytes = (uint32_t)warps * V * (2 * kStageBytes + kMetaBytes);
@@ -1004,7 +1004,7 @@ inline int epilogue_blocks_per_sm(int max_bps, uint64_t n_units) {
         return e ? std::atoi(e) : 0;
     }();
     (void)n_units;
-    int b = forced > 0 ? forced : max_bps;  // (one block per SM was measured: 214 vs 197 us per config-2 step -- more blocks win)
+    int b = forced > 0 ? forced : max_bps;  // (more blocks per SM beat one: the phases are short and latency bound)
     return b > max_bps ? max_bps : (b < 1 ? 1 : b);
 }
 
@@ -1150,8 +1150,10 @@ int acb_select_non_overlapping(const acb_automaton *a, const int64_t *dev_rows, 
 int acb_pack_gather_block(const uint64_t *dev_total, const acb_match *dev_out, uint32_t hay_base, uint64_t cap, void *dev_block, void *stream) {
     if (!dev_total || !dev_out || !dev_block) return fail(ACB_EINVAL, "null argument");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
     unsigned blocks = (unsigned)((cap + 255) / 256);
-    if (blocks > 296) blocks = 296;
+    if (blocks > 2u * (unsigned)d.sms) blocks = 2u * (unsigned)d.sms;  // two blocks per SM, grid-stride beyond that
     if (blocks < 1) blocks = 1;
     pack_gather_block_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const unsigned long long *>(dev_total), dev_out, hay_base, cap,
                                                      reinterpret_cast<uint4 *>(dev_block));
@@ -1340,7 +1342,7 @@ int acb_scan_batch(const acb_automaton *a, const void *dev_image, const void *de
         if (g_tuning.hot_rows > 0 && (uint32_t)g_tuning.hot_rows < fit128) fit128 = (uint32_t)g_tuning.hot_rows;
         // Byte-indexed (128-wide) rows make the transition two instructions per byte (IDP4A + LDS) instead of four,
         // but they are 256 bytes each (only ~230 fit below 64 KB) and on the config-2 text the kernel is bound by
-        // the shared-memory pipe, not by instruction issue: measured equal to the compact table (162 vs 160 us).
+        // the shared-memory pipe, not by instruction issue, so it is no faster than the compact table.
         // Opt-in (tuning.table = 2), one segment per lane only (two per lane leave too little room for the rows).
         const bool ascii = g_tuning.table == 2 && fit128 > 0 && per_lane == 1;
         rc = ACB_DISPATCH(launch_staged_cols, h, im, hot, B, P, out, seg_info, d, task_counter, acc + kAccGroups, st, ascii, per_lane);

@@ -1,5 +1,5 @@
 // scan_global.cuh -- segment-parallel scan straight from the automaton image in
-// global memory (which an L2 of 126 MB holds for any realistic pattern set).
+// global memory (the H100's 50 MB L2 holds the hot part of the table).
 //
 // The staged kernel (scan_staged.cuh) lives off a few hundred "hot" table rows in
 // shared memory; that is the right tool when the scan spends its time near the
@@ -14,9 +14,7 @@
 // kernel (speculated segment starts after a warm-up, SegInfo, unit counts), so
 // the epilogue does not know the difference.
 //
-// Measured on config 3-5 shapes: 90-130 GB/s, 3-6x the staged kernel there, and the same with 2048 instead
-// of 1536 threads per SM: the limit is L2 throughput for random 32-byte sectors (one per transition), not
-// latency.
+// The limit is L2 throughput for random 32-byte sectors (one per transition), not latency.
 #pragma once
 #include "scan_staged.cuh"
 

@@ -29,8 +29,8 @@
 //        different bank groups (conflict free), and a warp-wide cp.async
 //        instruction (8 rows) fills four whole 128-byte lines of shared
 //        memory.  (An 80-byte pitch without a swizzle reads just as well, but
-//        every copy instruction then straddles 12-14 lines: ncu showed 14
-//        shared-memory wavefronts per LDGSTS instead of 8, the floor.)
+//        every copy instruction then straddles 12-14 lines instead of 8, the
+//        floor.)
 //   V = segments per lane (template parameter): 1, or 2 whose chains interleave.
 //
 // All shared-memory traffic of the scan loop goes through explicit 32-bit

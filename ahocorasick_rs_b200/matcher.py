@@ -3,7 +3,7 @@
 Reference being mirrored: /root/reference/src/lib.rs (PyO3 classes
 ``AhoCorasick`` 29-33/134-273, ``BytesAhoCorasick`` 360-435, enums 91-128) and
 pysrc/ahocorasick_rs/ahocorasick_rs.pyi.  Same names, argument meaning and
-error behaviour; the scan itself runs in the sm_100a kernels behind
+error behaviour; the scan itself runs in the sm_90a kernels behind
 include/acb200.h.  There is no CPU fallback: without the CUDA library or a
 CUDA device every search raises.
 

@@ -54,7 +54,7 @@ def gather_match_lists(local, hay_base: int, group=None, dst: Optional[int] = No
     kmax = max(max(counts), 1)
     # Send and receive buffers are kept (grow-only) per device and dtype: a fresh multi-hundred-megabyte tensor per call
     # is handed to NCCL's stream and cannot be reused by the allocator until that stream has passed it, so every call
-    # would cudaMalloc anew (measured on 8 GPUs: 65-120 ms per gather of 76 MB per rank; 1.4 ms with kept buffers).
+    # would cudaMalloc anew.
     key = (str(dev), local.dtype)
     bufs = _GATHER_BUFS.get(key)
     if bufs is None or bufs[0].numel() < kmax * 4 or bufs[1].numel() < world * kmax * 4:

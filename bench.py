@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- haystack GB/s scanned (+ matches/s) for find_matches_as_indexes on the BASELINE.json workloads.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config 2|3|4|5]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config 2|3|4|5] [--dump-outputs DIR]
 
 --config (default 2, the configuration BASELINE.json's metric is quoted on at one GPU):
   2  benchmarks/names.txt patterns (4 244), Implementation.DFA, 100k x 4 KiB synthetic UTF-8 haystacks, AhoCorasick
@@ -58,7 +58,38 @@ def measured_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3), not measured"
+
+
+def gpu_identity(gpu_index):
+    """The card a number was measured on: its name and power limit (nvidia-smi), None where unavailable."""
+    try:
+        row = subprocess.run(["nvidia-smi", "-i", str(gpu_index), "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+        return {"name": row[0].strip(), "power_limit_w": float(row[1])}
+    except Exception:
+        return {"name": None, "power_limit_w": None}
+
+
+def dump_outputs(path, matches, match_offsets, total, budget=64 << 20, seed=0):
+    """What the timed path returned in its last step, as float64 .npy files under `path`: matches (k, 4) = (haystack,
+    pattern, start, end), match_offsets (n + 1), total.  Above `budget` bytes in all, a fixed seeded sample of rows is
+    written instead of the whole array, with the indexes of the sampled rows (<name>_index.npy)."""
+    os.makedirs(path, exist_ok=True)
+    m = matches.cpu().numpy()
+    m = (m.view(np.uint32) if m.dtype == np.int32 else m).astype(np.float64).reshape(-1, 4)
+    arrays = {"matches": m, "match_offsets": match_offsets.cpu().numpy().astype(np.float64),
+              "total": np.array([total], dtype=np.float64)}
+    share = (budget - 4096) // 2   # each of the two large arrays gets at most half (index arrays included; 4 KB for the rest)
+    for name in ("match_offsets", "matches"):
+        a = arrays[name]
+        if a.nbytes > share:
+            row_bytes = a.nbytes // len(a) + 8
+            idx = np.sort(np.random.default_rng(seed).choice(len(a), size=share // row_bytes, replace=False))
+            arrays[name] = a[idx]
+            arrays[name + "_index"] = idx.astype(np.float64)
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), a)
 
 
 class ClockSampler:
@@ -260,7 +291,11 @@ def main():
     ap.add_argument("--kernel", type=int, default=0, help=argparse.SUPPRESS)
     ap.add_argument("--hot-rows", type=int, default=0, help=argparse.SUPPRESS)
     ap.add_argument("--table", type=int, default=0, help=argparse.SUPPRESS)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one returned (rank 0) to DIR/<name>.npy, float64, at most 64 MB")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     claim_stdout()
 
@@ -374,26 +409,32 @@ def main():
     launches0 = L.acb_launch_count()
     sampler = ClockSampler(local_rank)
     sampler.start()
-    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    ev0.record()
-    host_t0 = time.perf_counter()
-    gathered = None
-    for i in range(args.steps):
-        out, moffs, tot = step(i)
+    try:
+        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        ev0.record()
+        host_t0 = time.perf_counter()
+        gathered = None
+        for i in range(args.steps):
+            out, moffs, tot = step(i)
+            if world > 1:
+                # the only exchange of the path: gather the per-shard match lists
+                if gather is not None:
+                    gathered = gather(out, tot, (rank * 2 + (i & 1)) * n_hay, slot=i % SLOTS)   # fixed-size blocks, side stream, no host round trip
+                else:
+                    gathered = big_gather(out)
+        if gather is not None:
+            gather.finish()  # the exchanges ran on a side stream: the timed region ends when the last one has
+        ev1.record()
+        host_enqueue_ms = (time.perf_counter() - host_t0) * 1e3 / args.steps
+        torch.cuda.synchronize()
         if world > 1:
-            # the only exchange of the path: gather the per-shard match lists
-            if gather is not None:
-                gathered = gather(out, tot, (rank * 2 + (i & 1)) * n_hay, slot=i % SLOTS)   # fixed-size blocks, side stream, no host round trip
-            else:
-                gathered = big_gather(out)
-    if gather is not None:
-        gather.finish()  # the exchanges ran on a side stream: the timed region ends when the last one has
-    ev1.record()
-    host_enqueue_ms = (time.perf_counter() - host_t0) * 1e3 / max(args.steps, 1)
-    torch.cuda.synchronize()
-    if world > 1:
-        dist.barrier()
-    clocks = sampler.stop()
+            dist.barrier()
+    finally:
+        clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        # the last step's buffers are those of workspace slot (steps - 1) % SLOTS, untouched until the e2e leg below
+        total_last = int(tot) if big else int(tot[0].item())
+        dump_outputs(args.dump_outputs, out[:total_last], moffs, total_last)
     ms = ev0.elapsed_time(ev1)
     launches = int(L.acb_launch_count() - launches0)
     kms, kn = ctypes.c_double(0), ctypes.c_uint64(0)
@@ -506,13 +547,6 @@ def main():
     achieved = alg_bytes / (k_ms * 1e-3) / 1e9 if k_ms > 0 else 0.0
     engine = scan_stats.get("engine")
     kernel_name = "sieve_scan_kernel" if engine == "sieve" else ("scan_global_kernel" if scan_stats.get("global_table") else "scan_staged_kernel")
-    traffic, traffic_src = None, None
-    tj = os.path.join(ROOT, "profiles", f"r02_{C['name']}_scan_kernel.json")
-    if os.path.exists(tj) and args.scale == 1.0 and not args.haystacks:
-        with open(tj) as f:
-            tjv = json.load(f)
-        if tjv.get("kernel") == kernel_name:
-            traffic, traffic_src = tjv["dram_traffic_bytes_per_launch"], f"profiles/r02_{C['name']}_scan_kernel.json (ncu --set full, dram__bytes_read.sum + dram__bytes_write.sum)"
     line = {
         "metric": METRIC, "value": value, "unit": "GB/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": ms_max / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -523,7 +557,7 @@ def main():
         "matches_per_s": matches_per_step * args.steps * world / (ms_max * 1e-3),
         "matches_per_step_per_gpu": matches_per_step,
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src, "kernel": kernel_name,
+                     "peak_source": peak_src, "kernel": kernel_name,
                      "kernel_ms": k_ms / lps, "kernel_ms_per_step": k_ms, "kernel_launches_per_step": lps,
                      "algorithmic_bytes_per_launch": alg_bytes / lps},
         "e2e": {"value": e2e_bytes * e2e_steps * world / e2e_s / 1e9, "unit": "GB/s",
@@ -534,6 +568,7 @@ def main():
         "scan_stats": scan_stats,
         "verified": verified,
         "host_enqueue_ms_per_step": host_enqueue_ms,
+        "gpu": gpu_identity(local_rank),
         "clocks": clocks,
     }
     if not args.no_cpu_baseline:

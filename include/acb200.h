@@ -1,5 +1,5 @@
 /*
- * acb200.h -- C ABI of the B200-native multi-pattern matcher (libacb200.so).
+ * acb200.h -- C ABI of the H100-native multi-pattern matcher (libacb200.so).
  *
  * This is the drop-in boundary for the reference's hot path.  The reference
  * (G-Research/ahocorasick_rs) has no C ABI of its own: its PyO3 shim

@@ -1,7 +1,7 @@
 // Microbenchmark: staging 64-byte pieces (one per lane, 4 KiB apart in global memory) into shared memory,
 // double buffered per warp, with (a) cp.async 16 B (LDGSTS: 4 instructions per warp and chunk) and (b) one
 // cp.async.bulk (TMA, UBLKCP) of 64 B per lane completing on a per-warp mbarrier.  Nothing consumes the data:
-// this measures what the copy path alone sustains per SM.   nvcc -arch=sm_100a -O3 stage_copy.cu
+// this measures what the copy path alone sustains per SM.   nvcc -arch=sm_90a -O3 stage_copy.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>

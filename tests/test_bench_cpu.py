@@ -35,6 +35,33 @@ def test_reference_arm_line():
     assert d["e2e"] == {"value": d["value"], "unit": "GB/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}
 
 
+def test_dump_outputs_float64_within_budget(tmp_path):
+    """--dump-outputs: float64 arrays; above the budget, the same seeded sample of rows every time."""
+    import numpy as np
+    import torch
+
+    import bench
+
+    rows = np.arange(4 * 5000, dtype=np.uint32).reshape(5000, 4)
+    rows[:, 3] = 0xFFFFFFF0   # uint32 values above 2^31 survive the int32 view the scan returns
+    m = torch.from_numpy(rows.view(np.int32))
+    mo = torch.arange(101, dtype=torch.int64) * 50
+    bench.dump_outputs(str(tmp_path / "a"), m, mo, 5000, budget=1 << 30)
+    got = np.load(tmp_path / "a" / "matches.npy")
+    assert got.dtype == np.float64 and np.array_equal(got, rows.astype(np.float64))
+    assert np.array_equal(np.load(tmp_path / "a" / "match_offsets.npy"), mo.numpy().astype(np.float64))
+    assert np.load(tmp_path / "a" / "total.npy").tolist() == [5000.0]
+    for d in ("b", "c"):
+        bench.dump_outputs(str(tmp_path / d), m, mo, 5000, budget=64 << 10)
+    files = sorted(os.listdir(tmp_path / "b"))
+    assert files == ["match_offsets.npy", "matches.npy", "matches_index.npy", "total.npy"]
+    assert sum(os.path.getsize(tmp_path / "b" / f) for f in files) <= 64 << 10
+    idx = np.load(tmp_path / "b" / "matches_index.npy").astype(np.int64)
+    assert np.array_equal(np.load(tmp_path / "b" / "matches.npy"), rows[idx].astype(np.float64))
+    for f in files:
+        assert np.array_equal(np.load(tmp_path / "b" / f), np.load(tmp_path / "c" / f))
+
+
 def test_reference_arm_other_ranks_stay_silent():
     env = dict(os.environ, RANK="1", WORLD_SIZE="2", LOCAL_RANK="1")
     p = subprocess.run([sys.executable, "bench.py", "--impl", "reference", "--gpus", "2", "--steps", "1", "--warmup", "0"],
