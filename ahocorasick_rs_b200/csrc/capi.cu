@@ -174,6 +174,12 @@ constexpr int kAccTraps = 4;    // times a lane left the hot table
 constexpr int kAccRepairs = 5;  // segment boundaries repaired
 constexpr int kAccWords = 8;
 
+// totals[6] after a table walker's epilogue: which of its branches the scan took (the sieve epilogue uses
+// totals[6..7] for its own sizes).  Results never depend on these; tests read them to know they reached a path.
+constexpr unsigned kPathFarCp = 1u;     // code points: the prefix sum over all segments' continuation bytes
+constexpr unsigned kPathSearch = 2u;    // per-haystack offsets by binary search (else the warp run-fill)
+constexpr unsigned kPathRepaired = 4u;  // some speculated segment start was wrong: the repair pass ran
+
 // ---------------------------------------------------------------------------
 // everything after the table walkers in ONE cooperative kernel (grid-wide
 // barriers between the phases):
@@ -317,13 +323,14 @@ __device__ __forceinline__ void order_body(const EpilogueArgs &E, unsigned long 
 
 // phase 4: per-haystack CSR offsets into the ordered output + the totals
 // (raw_total: read before the barrier in front of this phase, which resets the counter)
-__device__ __forceinline__ void match_offsets_body(const EpilogueArgs &E, unsigned long long raw_total) {
+__device__ __forceinline__ void match_offsets_body(const EpilogueArgs &E, unsigned long long raw_total, unsigned paths) {
     const unsigned long long total = E.unit_offsets[E.n_items];
     const bool complete = raw_total <= E.raw_cap && total <= E.out_cap;
     const unsigned long long avail = total < E.out_cap ? total : E.out_cap;
     const int64_t nh = E.B.n_haystacks;
     const acb_match *out = E.out_buf;
-    if (complete && avail <= 4 * (unsigned long long)(nh + 1)) {
+    const bool run_fill = complete && avail <= 4 * (unsigned long long)(nh + 1);
+    if (run_fill) {
         // Few matches per haystack: one pass over the records.  Record i is the first of every haystack in
         // (haystack of record i - 1, haystack of record i]; i == avail closes the list (haystacks up to nh).  The warp
         // fills those runs together, so a long run of haystacks without matches does not hold up one thread.
@@ -369,7 +376,8 @@ __device__ __forceinline__ void match_offsets_body(const EpilogueArgs &E, unsign
         totals[3] = acc[kAccTraps];
         totals[4] = raw_total;
         totals[5] = acc[kAccRepairs];
-        totals[6] = totals[7] = 0;
+        totals[6] = paths | (run_fill ? 0u : kPathSearch);
+        totals[7] = 0;
         acc[kAccRaw] = acc[kAccGroups] = acc[kAccTraps] = acc[kAccRepairs] = 0;
         acc[kAccQueue] = 0;    // the scan kernel's task queue (low word) and the repair flag (high word)
         acc[kAccContFar] = 0;
@@ -419,7 +427,7 @@ __global__ void __launch_bounds__(kScanThreads) epilogue_kernel(EpilogueArgs E) 
     const unsigned long long raw_total = *reinterpret_cast<volatile unsigned long long *>(E.acc + kAccRaw);
     order_body(E, raw_total, CP, repaired, far);
     grid.sync();
-    match_offsets_body(E, raw_total);
+    match_offsets_body(E, raw_total, (far ? kPathFarCp : 0u) | (repaired ? kPathRepaired : 0u));
 }
 
 

@@ -110,6 +110,13 @@ def scan_in_windows(scan_window, hay, window_bytes: int, halo: int, codepoints: 
     return parts
 
 
+# last_stats["paths"] of a table-walker scan: the branches its epilogue took (kPath* in csrc/capi.cu).  They never
+# change results; tests check them to know that an input reached the path it was made for.
+PATH_FAR_CP = 1      # code points: prefix sum of every segment's continuation bytes (a haystack spans > 8 segments)
+PATH_SEARCH = 2      # per-haystack offsets by binary search (more than 4 records per haystack, or an incomplete list)
+PATH_REPAIRED = 4    # some speculated segment start was wrong and the repair pass ran
+
+
 class _Automaton:
     """Owns the host automaton handle, its device image and a growable device
     workspace.  Shared by both public classes."""
@@ -391,6 +398,7 @@ class _Automaton:
                 if hot:
                     self._note_trap_stats(hot, tot[2], tot[3])
                     self.last_stats = {"engine": "table", "groups": tot[2], "traps": tot[3], "repairs": tot[5], "segments": plan.n_segments,
+                                       "paths": tot[6],
                                        "hot_rows": hot["rows"].rows, "hot_rows128": hot["rows"].rows128,
                                        "hot_visited": hot["rows"].visited, "hot_coverage": round(hot.get("coverage", 1.0), 5),
                                        "global_table": bool(hot["rows"].reserved & 1),

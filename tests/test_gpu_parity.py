@@ -2,7 +2,6 @@
 (include/acb200.h) by the package, against the CPU oracle on the same seeded
 inputs, against the reference's golden vectors, and -- at larger sizes --
 through size-independent properties.  Bit-exact: integer/index work."""
-import ctypes as C
 import json
 import os
 
@@ -13,74 +12,15 @@ pytestmark = pytest.mark.gpu
 
 torch = pytest.importorskip("torch")
 
-from ahocorasick_rs_b200 import (AhoCorasick, BytesAhoCorasick, Implementation, MatchKind, _capi, workloads as W)
+from ahocorasick_rs_b200 import AhoCorasick, BytesAhoCorasick, Implementation, MatchKind, workloads as W
 from oracle import Oracle
 
+from .gpu_helpers import KINDS, check_batch, dev, gpu_batch, kernel, set_kernel  # noqa: F401 (kernel: the fixture)
+
 HERE = os.path.dirname(os.path.abspath(__file__))
-KINDS = [MatchKind.Standard, MatchKind.LeftmostFirst, MatchKind.LeftmostLongest]
 
 with open(os.path.join(HERE, "golden", "reference_vectors.json"), encoding="utf-8") as f:
     VECTORS = json.load(f)["vectors"]
-
-
-def set_kernel(kernel=0, hot_rows=0, segment_bytes=0, table=0):
-    _capi.set_tuning(kernel, hot_rows, segment_bytes, table)
-
-
-@pytest.fixture(params=["sieve", "sieve-small-tasks", "staged", "plain", "staged-tiny-hot", "staged-small-segments", "staged-compact-table",
-                        "staged-byte-table", "staged-byte-table-tiny", "staged-two-per-lane", "staged-two-per-lane-tiny", "global-segments", "global-small-segments"])
-def kernel(request):
-    if request.param == "sieve":
-        set_kernel(5)                 # the default engine: position-parallel filter + exact verification (scan_sieve.cuh)
-    elif request.param == "sieve-small-tasks":
-        set_kernel(5, 0, 512)         # one 512-byte window per task: every boundary case at every task start
-    elif request.param == "plain":
-        set_kernel(1)
-    elif request.param == "staged":
-        set_kernel(2)                 # the default: compact (column-indexed) table, one segment per lane
-    elif request.param == "staged-tiny-hot":
-        set_kernel(2, 5, 0, 1)        # 5 hot rows, compact table: nearly every group leaves the hot set
-    elif request.param == "staged-compact-table":
-        set_kernel(2, 0, 0, 1)        # column-indexed table even where the byte-indexed one would do
-    elif request.param == "staged-byte-table":
-        set_kernel(2, 0, 0, 2)        # byte-indexed table (IDP4A transitions) wherever the patterns are ASCII
-    elif request.param == "staged-byte-table-tiny":
-        set_kernel(2, 7, 256, 2)      # byte-indexed table forced, 7 rows, 256-byte segments
-    elif request.param == "global-segments":
-        set_kernel(4)                 # segment-parallel, tables in global memory / L2 (what dense automata get)
-    elif request.param == "global-small-segments":
-        set_kernel(4, 0, 128)         # ... with 128-byte segments: speculation and repair everywhere
-    elif request.param == "staged-two-per-lane":
-        set_kernel(3)                 # two segments per lane (two interleaved chains)
-    elif request.param == "staged-two-per-lane-tiny":
-        set_kernel(3, 6, 128, 1)      # ... with 6 hot rows and 128-byte segments: careful path and repair everywhere
-    else:
-        set_kernel(2, 0, 128)  # 128-byte segments: speculative starts and the repair pass everywhere
-    yield request.param
-    set_kernel(0)
-
-
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-def gpu_batch(ac, data, offs, overlapping=False):
-    m, moffs, total = ac.scan_device(dev(data), dev(offs), overlapping)
-    return m.cpu().numpy().view(np.uint32), moffs.cpu().numpy(), total
-
-
-def check_batch(pats_bytes, kind, data, offs, overlapping=False, codepoints=False, implementation=None):
-    orc = Oracle(pats_bytes, kind.name)
-    total, counts, rec = orc.scan_batch(data, offs, overlapping=overlapping, codepoints=codepoints)
-    if codepoints:
-        ac = AhoCorasick([p.decode() for p in pats_bytes], kind, implementation=implementation)
-    else:
-        ac = BytesAhoCorasick(pats_bytes, kind, implementation=implementation)
-    m, moffs, gtotal = gpu_batch(ac, data, offs, overlapping)
-    assert gtotal == total
-    assert np.array_equal(np.diff(moffs), counts.astype(np.int64))
-    assert np.array_equal(m, rec)
-    return total
 
 
 # ---------------------------------------------------------------- golden vectors, through the drop-in classes
