@@ -1434,8 +1434,9 @@ int acb_scan_batch(const acb_automaton *a, const void *dev_image, const void *de
         if (fit128 > hot.n_rows128) fit128 = hot.n_rows128;
         if (g_tuning.hot_rows > 0 && (uint32_t)g_tuning.hot_rows < fit128) fit128 = (uint32_t)g_tuning.hot_rows;
         // Byte-indexed (128-wide) rows make the transition two instructions per byte (IDP4A + LDS) instead of four,
-        // but they are 256 bytes each (only ~230 fit below 64 KB) and on the config-2 text the kernel is bound by
-        // the shared-memory pipe, not by instruction issue, so it is no faster than the compact table.
+        // but they are 256 bytes each (only ~230 fit below 64 KB), and on the config-2 text the kernel is bound by
+        // the arrival of its staged bytes, not by the chain (on an H100 the warps wait for their next chunk ~60 % of
+        // the time; DESIGN.md §6), so it is no faster than the compact table.
         // Opt-in (tuning.table = 2), one segment per lane only (two per lane leave too little room for the rows).
         const bool ascii = g_tuning.table == 2 && fit128 > 0 && per_lane == 1;
         rc = ACB_DISPATCH(launch_staged_cols, h, im, hot, B, P, out, seg_out, d, task_counter, acc + kAccGroups, st, ascii, per_lane);

@@ -52,7 +52,9 @@
 // Each lane reads its bytes in 64-byte chunks of the ABSOLUTE address grid,
 // so every cp.async is 16-byte aligned and a warp-wide copy instruction
 // touches 8 x 64 contiguous bytes.  Chunk k+1 is in flight while chunk k is
-// scanned (the scan of a chunk takes longer than an HBM round trip).
+// scanned.  The copies ask the L2 for whole 128-byte lines: a lane's rows are
+// 4 KiB apart, and fetching two chunks of a row per DRAM access instead of one
+// is what keeps the warps fed (DESIGN.md §6; a third staging buffer was slower).
 #pragma once
 #include <type_traits>
 
@@ -171,8 +173,11 @@ __device__ __forceinline__ uint32_t fstep4(uint32_t s, uint32_t w, const FastTab
 // continuation bytes (10xxxxxx) in a word
 __device__ __forceinline__ uint32_t cont_bytes(uint32_t w) { return __popc(w & ~(w << 1) & 0x80808080u); }
 
+// .L2::128B: the L2 fetches the whole 128-byte line, not just the 64 bytes a lane's chunk needs, so the next chunk of
+// the row is usually in L2 by the time it is copied (DESIGN.md §6).  src must be a valid address even when
+// src_bytes is 0.
 __device__ __forceinline__ void cp_async16(uint32_t dst_smem, const void *src, uint32_t src_bytes) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst_smem), "l"(src), "r"(src_bytes) : "memory");
+    asm volatile("cp.async.cg.shared.global.L2::128B [%0], [%1], 16, %2;\n" ::"r"(dst_smem), "l"(src), "r"(src_bytes) : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;\n" ::: "memory"); }
@@ -530,8 +535,9 @@ scan_staged_kernel(DevImage im, DevHot hot_img, Batch B, SegPlan P, Sink out, Se
 #pragma unroll
             for (int i = 0; i < 4 * V; i++) {
                 const uint2 m = V == 1 ? mrow[i & 3] : lds64(cp_meta + i * 64);
-                const uint8_t *src = reinterpret_cast<const uint8_t *>(gbase) + ((size_t)(m.x + k * 4 + (lane & 3)) << 4);
-                cp_async16(dst + i * 8 * kRow, src, k < m.y ? 16u : 0u);
+                const bool live = k < m.y;  // else the unit is zero-filled, from the grid origin (a valid address)
+                const uint8_t *src = reinterpret_cast<const uint8_t *>(gbase) + (live ? (size_t)(m.x + k * 4 + (lane & 3)) << 4 : 0);
+                cp_async16(dst + i * 8 * kRow, src, live ? 16u : 0u);
             }
             cp_async_commit();
         };

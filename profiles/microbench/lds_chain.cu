@@ -1,4 +1,4 @@
-// Microbenchmark behind DESIGN.md section 5: cycles per step of the scan kernel's dependent chain
+// Microbenchmark behind DESIGN.md section 6: cycles per step of the scan kernel's dependent chain
 //   LDS.U16 -> (IMAD | IDP4A) -> LDS.U16
 // for 1..32 warps per SM and 1 or 2 independent chains per thread.  One CTA per SM, table of 40 KB of u16
 // "row addresses" in shared memory, bytes from registers.  Build: nvcc -arch=sm_90a -O3 lds_chain.cu
