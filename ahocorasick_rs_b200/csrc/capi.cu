@@ -173,6 +173,8 @@ constexpr int kAccGroups = 3;   // 16-byte groups in the stream
 constexpr int kAccTraps = 4;    // times a lane left the hot table
 constexpr int kAccRepairs = 5;  // segment boundaries repaired
 constexpr int kAccWords = 8;
+// acb_any_match's dev_scratch: [0] task counter (low u32), [1] tasks skipped whole, [2] windows not scanned
+constexpr int kAnyScratchWords = 3;
 
 // totals[6] after a table walker's epilogue: which of its branches the scan took (the sieve epilogue uses
 // totals[6..7] for its own sizes).  Results never depend on these; tests read them to know they reached a path.
@@ -1133,7 +1135,8 @@ DevSieve make_sieve_view(const SieveHeader &h, const void *dev_sieve) {
     return v;
 }
 
-template <bool CP>
+// ANY: the any-match mode (acb_any_match): hay_cont carries its flags and task_cont its two skip counters, out goes unused
+template <bool CP, bool ANY = false>
 int launch_sieve(const DevSieve &sv, const Batch &B, SievePlan &P, const Sink &out, uint32_t *task_cont, uint32_t *hay_cont,
                  unsigned int *task_counter, const DeviceInfo &d, cudaStream_t st) {
     // as many windows of text per warp as fit next to the filters (a power of two): the more, the fuller the rounds of
@@ -1146,7 +1149,7 @@ int launch_sieve(const DevSieve &sv, const Batch &B, SievePlan &P, const Sink &o
     P.ring = ring;
 #define ACB_SIEVE_GO(WC)                                                                                  \
     do {                                                                                                  \
-        auto kern = sieve_scan_kernel<CP, WC>;                                                            \
+        auto kern = sieve_scan_kernel<CP, WC, ANY>;                                                       \
         CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, d.max_smem_optin)); \
         kern<<<d.sms, kSieveThreads, smem, st>>>(sv, B, P, out, task_cont, hay_cont, task_counter);       \
     } while (0)
@@ -1226,6 +1229,41 @@ int acb_select_non_overlapping(const acb_automaton *a, const int64_t *dev_rows, 
                                          kind == ACB_LEFTMOST_LONGEST ? 1 : 0, (long long)h.max_pat_len, reinterpret_cast<long long *>(dev_out),
                                          reinterpret_cast<unsigned long long *>(dev_count));
     g_launches++;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+int acb_any_match(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                  int64_t n_haystacks, uint64_t total_bytes, uint8_t *dev_flags, uint64_t *dev_scratch, void *stream) {
+    if (!a || !dev_sieve || !dev_offsets || !dev_flags || !dev_scratch || (total_bytes && !dev_bytes)) return fail(ACB_EINVAL, "null argument");
+    if (n_haystacks < 0 || n_haystacks > 0xfffffffell) return fail(ACB_EINVAL, "n_haystacks out of range (0 .. 2^32 - 2)");
+    if (total_bytes >= (1ull << 31)) return fail(ACB_EINVAL, "total_bytes must be below 2^31 (scan larger inputs in windows)");
+    SieveHeader sh;
+    {
+        std::lock_guard<std::mutex> lock(a->impl->sieve_mutex);
+        if (a->impl->sieve.size() < sizeof(SieveHeader)) return fail(ACB_EINVAL, "acb_sieve_build has not been called");
+        std::memcpy(&sh, a->impl->sieve.data(), sizeof(sh));
+    }
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CUDA_OK(cudaMemsetAsync(dev_scratch, 0, kAnyScratchWords * sizeof(uint64_t), st));
+    if (n_haystacks == 0 || total_bytes == 0) return ACB_OK;
+    acb_plan plan;
+    acb_plan_scan(a, dev_bytes, total_bytes, (uint64_t)n_haystacks, &plan);
+    SievePlan SP;
+    SP.origin = -(int64_t)(reinterpret_cast<uintptr_t>(dev_bytes) & 511u);
+    SP.task_bytes = plan.task_bytes;
+    SP.n_tasks = (int64_t)((total_bytes + (uint64_t)(-SP.origin) + plan.task_bytes - 1) / plan.task_bytes);
+    SP.buf_bytes = total_bytes;
+    SP.avg_len = total_bytes / (uint64_t)n_haystacks;
+    if (SP.avg_len < 1) SP.avg_len = 1;
+    const Batch B{dev_bytes, dev_offsets, n_haystacks};
+    unsigned long long *scr = reinterpret_cast<unsigned long long *>(dev_scratch);
+    // (the kernel's code-point pointers carry the skip counters and the flags in this mode)
+    const int rc = launch_sieve<false, true>(make_sieve_view(sh, dev_sieve), B, SP, Sink{}, reinterpret_cast<uint32_t *>(scr + 1),
+                                             reinterpret_cast<uint32_t *>(dev_flags), reinterpret_cast<unsigned int *>(scr), d, st);
+    if (rc) return rc;
     CUDA_OK(cudaGetLastError());
     return ACB_OK;
 }

@@ -33,6 +33,15 @@
 //
 // Output of this kernel = the OVERLAPPING match list.  sieve_epilogue_kernel (capi.cu) orders it and, for the
 // non-overlapping searches, selects from it per haystack.
+//
+// ANY (acb_any_match): the answer is one flag per haystack, "some pattern occurs in it", and the kernel writes no list.
+// Stage 2 stores 1 to the flag of every haystack in which it finds a terminal node (a plain byte store: every writer
+// stores the same value).  A position is only ever skipped when its haystack's flag is already set:
+//   task skip     a task whose part of the stream lies inside one flagged haystack is not scanned at all;
+//   window exit   while a warp walks a task, the flag of the haystack that holds the rest of the task is loaded together
+//                 with the next window's bytes (only once that window lies inside it); when it is set, the warp stops
+//                 scanning, verifies what it had queued from earlier windows and moves on.
+// Flags set by other CTAs during the launch are read with ld.relaxed.gpu (never through the non-coherent cache).
 #pragma once
 #include "scan_staged.cuh"
 #include "sieve.h"
@@ -104,6 +113,13 @@ __device__ __forceinline__ uint4 load_chunk(const uint8_t *bytes, int64_t q, int
     return make_uint4(w[0], w[1], w[2], w[3]);
 }
 
+// a haystack flag, coherent at device scope (other CTAs set flags during the launch)
+__device__ __forceinline__ uint32_t ld_flag(const uint8_t *p) {
+    uint32_t v;
+    asm volatile("ld.relaxed.gpu.global.u8 %0, [%1];\n" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+
 // continuation bytes among the first nbytes (0..16) of the 16-byte chunk at shared address a
 __device__ __forceinline__ uint32_t cont_prefix(uint32_t a, uint32_t nbytes) {
     uint32_t n = 0;
@@ -131,9 +147,16 @@ __device__ __forceinline__ uint32_t warp_excl_scan(uint32_t v, uint32_t lane, ui
 // WC: 0 = W < 4 (the window word is shifted down), 1 = W == 4, 2 = W in 6..8 (two words), 3 = W == 5 (a word and a byte)
 //
 // Positions inside a task are 32-bit offsets from the task's start (`rel`); the 64-bit stream position is t_lo + rel.
-template <bool CP, int WC>
+//
+// ANY (CP = false only): `out` is unused, and the two code-point pointers carry the any-match outputs instead (so the
+// list-mode instantiations keep their parameter block): hay_cont -> flags = u8[n_haystacks], task_cont -> skipped =
+// u64[2] = [tasks skipped whole, windows not scanned] (see acb_any_match).
+template <bool CP, int WC, bool ANY = false>
 __global__ void __launch_bounds__(kSieveThreads, 1)
 sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_cont, uint32_t *hay_cont, unsigned int *task_counter) {
+    static_assert(!(ANY && CP), "the any-match mode has no positions to count");
+    uint8_t *const flags = reinterpret_cast<uint8_t *>(hay_cont);
+    unsigned long long *const skipped = reinterpret_cast<unsigned long long *>(task_cont);
     extern __shared__ __align__(128) uint8_t smem[];
     const uint32_t bloom_s = (uint32_t)__cvta_generic_to_shared(smem);
     const uint32_t bloom_bytes = sv.bloom_words * 4;
@@ -199,6 +222,7 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
     };
 
     unsigned int claimed = 0;
+    uint32_t tasks_skipped = 0, windows_skipped = 0;  // (ANY)
     if (lane == 0) claimed = atomicAdd(task_counter, 1u);
     for (;;) {
         const unsigned int task = __shfl_sync(0xffffffffu, claimed, 0);
@@ -206,7 +230,7 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
         if (lane == 0) claimed = atomicAdd(task_counter, 1u);  // the next one: its round trip overlaps this task
         const int64_t t_lo = P.origin + (int64_t)task * T;
         if (t_lo >= vhi || t_lo + (int64_t)T <= vlo) {
-            if (lane == 0) {
+            if (lane == 0 && !ANY) {
                 out.unit_counts[task] = 0;
                 if (CP) task_cont[task] = 0;
             }
@@ -240,6 +264,29 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
         };
         int32_t offc = load_offc(hb);
         int32_t next_start = __shfl_sync(0xffffffffu, offc, 1);  // start of haystack hb + 1
+        // ANY: the haystack that holds the task's last stream byte, and its start (relative); from that start on the rest
+        // of the task lies inside it.  A task that lies inside it whole, with its flag set, is skipped.
+        int64_t tail_h = 0;
+        int32_t tail_s = 0x7fffffff;
+        uint32_t tail_flag = 0;  // lane 0: its flag, loaded with the next window's bytes (nonzero: stop before that window)
+        if (ANY) {
+            const uint32_t k = __popc(__ballot_sync(0xffffffffu, offc <= (int32_t)hi_r - 1));  // >= 1: lane 0 holds hb's start
+            if (k < 32) {
+                tail_h = hb + k - 1;
+                tail_s = __shfl_sync(0xffffffffu, offc, k - 1);
+            } else {
+                tail_h = find_haystack(B, t_lo + hi_r - 1);
+                tail_s = (int32_t)max(__ldg(B.offsets + tail_h) - t_lo, (int64_t)-0x7fffffff);
+            }
+            if (tail_s <= (int32_t)lo_r) {
+                uint32_t f = 0;
+                if (lane == 0) f = ld_flag(flags + tail_h);
+                if (__shfl_sync(0xffffffffu, f, 0)) {
+                    tasks_skipped++;
+                    continue;
+                }
+            }
+        }
         // Haystack containing the byte at rel, and its start (relative).  The shuffles are executed by the whole warp (rel
         // may differ per lane).  Positions before the cached range (queued in an earlier window) walk back from it; a
         // window with more than 31 haystack starts (haystacks of a few bytes) falls back to a search.
@@ -345,9 +392,13 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
                     na = nc;
                     d++;
                 }
-                if (best != kSieveNoNode) cnt = __ldg(&sv.nb[best].chain_cnt);
+                if (ANY) {
+                    if (best != kSieveNoNode) flags[h] = 1;  // a pattern ends here, inside haystack h
+                } else if (best != kSieveNoNode) {
+                    cnt = __ldg(&sv.nb[best].chain_cnt);
+                }
             }
-            const uint32_t hits = __ballot_sync(0xffffffffu, cnt != 0);
+            const uint32_t hits = ANY ? 0u : __ballot_sync(0xffffffffu, cnt != 0);
             if (hits) {
                 uint32_t total;
                 const uint32_t exc = warp_excl_scan(cnt, lane, &total);
@@ -443,6 +494,20 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
         uint32_t cur_slot = slot_s(wrel);  // the ring slot of the current window
 
         for (;; wrel += kWin) {
+            if (ANY && (int32_t)wrel >= tail_s && __shfl_sync(0xffffffffu, tail_flag, 0)) {
+                // the rest of the task lies inside a flagged haystack: verify what earlier windows queued (it may belong
+                // to other haystacks), then stop
+                windows_skipped += (wlast - wrel) / kWin + 1;
+                for (;;) {
+                    if (q2n > 32 || (q1n == 0 && q2n != 0))
+                        round2();
+                    else if (q1n != 0)
+                        round1();
+                    else
+                        break;
+                }
+                break;
+            }
             if (wrel + kWin <= wlast) {
                 // the next window (a window takes a warp a few microseconds: one load in flight per lane covers the latency);
                 // whole windows inside the stream (all but a task's edges) take the direct load
@@ -450,6 +515,8 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
                     nxt = __ldg(reinterpret_cast<const uint4 *>(tptr + (wrel + kWin + 16 * lane)));
                 else
                     nxt = load16(wrel + kWin + 16 * lane);
+                // ANY: the flag that may end the task, in flight with the bytes it would save
+                if (ANY && lane == 0 && (int32_t)(wrel + kWin) >= tail_s) tail_flag = ld_flag(flags + tail_h);
             }
             // ---- fast path: first filter probe for the 16 positions of this lane ----
             uint32_t pz = __shfl_up_sync(0xffffffffu, cur.z, 1), pw = __shfl_up_sync(0xffffffffu, cur.w, 1);
@@ -584,9 +651,13 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
             carry_w = __shfl_sync(0xffffffffu, cur.w, 31);
             cur = nxt;
         }
-        if (lane == 0) out.unit_counts[task] = n_emitted;
+        if (lane == 0 && !ANY) out.unit_counts[task] = n_emitted;
         if (CP && lane == 0) task_cont[task] = cp_before;
         __syncwarp();
+    }
+    if (ANY && lane == 0) {
+        if (tasks_skipped) atomicAdd(skipped, (unsigned long long)tasks_skipped);
+        if (windows_skipped) atomicAdd(skipped + 1, (unsigned long long)windows_skipped);
     }
 }
 

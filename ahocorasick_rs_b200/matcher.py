@@ -9,7 +9,8 @@ CUDA device every search raises.
 
 Additions next to the drop-in methods (the reference API is one haystack per
 call): ``find_matches_as_indexes_batch`` and ``scan_device`` for batches that
-are already device resident.
+are already device resident; ``is_match`` / ``is_match_batch`` /
+``is_match_device``, the crate's ``AhoCorasick::is_match`` per haystack.
 """
 from __future__ import annotations
 
@@ -147,7 +148,7 @@ class _Automaton:
         self._ws = {}          # (device index, slot) -> dict of tensors
         self._small = {}       # device index -> the small-call context
         self.last_stats = {}
-        self._lock = threading.Lock()
+        self._lock = threading.RLock()   # (re-entered: any_device's table-walker path scans with scan_device under it)
         self._host_lock = threading.RLock()   # host-buffer calls: staging buffer + workspaces until the results are on the host
 
     def __del__(self):
@@ -282,6 +283,8 @@ class _Automaton:
         need = (ws is None or ws["n_units"] < plan.n_units or ws["n_segments"] < plan.n_segments or
                 ws["scratch"].numel() < plan.scratch_words or ws["n_haystacks"] < n_haystacks or ws["capacity"] < capacity)
         if need:
+            if ws is not None and ws.get("reader") is not None:
+                ws["reader"].synchronize()   # an any_device comparison still reading the buffers about to be freed
             n_units = max(plan.n_units, ws["n_units"] if ws else 0, 1)
             n_seg = max(plan.n_segments, ws["n_segments"] if ws else 0, 1)
             n_hay = max(n_haystacks, ws["n_haystacks"] if ws else 0, 1)
@@ -328,6 +331,150 @@ class _Automaton:
             raise ValueError(f"match kind {self.matchkind.name} does not support overlapping searches")
 
     # ---- scans ------------------------------------------------------------------
+    def _pick_engine(self, dev, data, offsets, overlapping):
+        """Which kernel family scans (data, offsets): None = the sieve, else the hot image the table walkers use.
+        Called under self._lock.  Results are identical; only speed and the device images a scan needs differ.
+          table  the automaton walkers: best when the scan lives in a few hundred states that fit in shared memory
+                 (sparse matches in text) -- the profile of the data says so (hot-row coverage);
+          sieve  the position-parallel filter + exact verification: everything else (dense pattern sets, whose
+                 states live in L2), and small inputs, where the profiling pass would cost more than the scan.
+        The tuning knob's forced kernel and ENGINE override the profile."""
+        torch = _torch()
+        forced = _capi.current_kernel()
+        if overlapping == 2 or forced == 5 or (forced == 0 and self.ENGINE == "sieve"):
+            return None
+        if forced in (1, 2, 3, 4) or self.ENGINE == "table":
+            return self.hot(dev, data, offsets, overlapping)
+        if self.implementation in (Implementation.ContiguousNFA, Implementation.NoncontiguousNFA):
+            return None   # the caller asked for a compact (non-DFA) table format: that is the sieve image
+        if data.numel() < self.AUTO_PROFILE_BYTES and self._hot.get(dev.index if dev.index is not None else torch.cuda.current_device()) is None:
+            return None
+        hot = self.hot(dev, data, offsets, overlapping)
+        return None if hot["rows"].reserved & 1 else hot
+
+    def any_device(self, data, offsets, out=None, sync: bool = True):
+        """Which haystacks of a device-resident batch contain an occurrence of any pattern -> bool CUDA tensor (n,).
+        The answer does not depend on the match kind.  `out` (bool, (n,), contiguous, on the data's device): the
+        answer is OR-ed into it, and haystacks already True there are not scanned.  With sync=False a call that runs
+        the sieve returns right after enqueueing (and last_stats are not updated).
+
+        Where the engine rule of scan_device picks the sieve, its kernel runs in the any-match mode (acb_any_match:
+        no match list, work stops per haystack at its first match); where it picks a table walker (text whose scan
+        stays in a few hot states), the walker's full scan is faster than the sieve's and its per-haystack counts give
+        the answer.  That path always waits for its scan, whatever `sync` says: a match list that did not fit the
+        workspace is only known on the host, and is scanned again with room for all of it (a truncated list would
+        report haystacks with matches as False).  The next scan that reuses the workspace waits, on the device, for
+        the comparison that reads it, so the returned tensor is the caller's own on either path, whatever stream or
+        thread scans next."""
+        torch = _require_cuda()
+        dev = data.device
+        n = offsets.numel() - 1
+        if out is not None and (out.dtype != torch.bool or out.dim() != 1 or out.numel() != max(n, 0) or out.device != dev or
+                                not out.is_contiguous()):
+            raise ValueError(f"out must be a contiguous bool tensor of shape ({max(n, 0)},) on {dev}")
+        if n <= 0 or data.numel() == 0:
+            return out if out is not None else torch.zeros(max(n, 0), dtype=torch.bool, device=dev)
+        if data.numel() > self.WINDOW_BYTES:
+            if not sync:
+                raise ValueError(f"buffers above {self.WINDOW_BYTES} bytes are scanned in windows: sync=False is not available")
+            return self._any_device_windows(data, offsets, out if out is not None else torch.zeros(n, dtype=torch.bool, device=dev))
+        with self._lock, torch.cuda.device(dev):
+            use_sieve = self._pick_engine(dev, data, offsets, False) is None
+            if use_sieve:
+                if out is None:
+                    out = torch.zeros(n, dtype=torch.bool, device=dev)
+                sieve_t, _ = self.sieve(dev)
+                plan = self._plan(data, n)
+                scratch = torch.empty(3, dtype=torch.int64, device=dev)
+                rc = self._L.acb_any_match(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
+                                           out.data_ptr(), scratch.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+                if rc != _capi.ACB_OK:
+                    raise RuntimeError(_capi.last_error())
+            else:
+                # scan_device (it takes the lock again and makes the same choice) with sync=True: it retries until the
+                # list is complete.  Its match_offsets are a view of workspace slot 0, which every scan of this
+                # automaton shares: the next scan that uses the slot waits for the event recorded after the comparison
+                # (on whatever stream it runs), and a slot that grows first waits for it on the host.
+                _, mo, _ = self.scan_device(data, offsets, False, False)
+                hit = mo[1:] > mo[:-1]
+                if out is None:
+                    out = hit
+                else:
+                    out |= hit
+                reader = torch.cuda.Event()
+                reader.record(torch.cuda.current_stream(dev))
+                self._ws[(dev.index if dev.index is not None else torch.cuda.current_device(), 0)]["reader"] = reader
+                self.last_stats = {"engine": self.last_stats.get("engine", "table"), "mode": "any"}
+                return out
+        if sync:
+            _, skipped, windows = scratch.tolist()
+            task_bytes = int(plan.task_bytes)
+            tasks = (data.numel() + (data.data_ptr() & 511) + task_bytes - 1) // task_bytes
+            self.last_stats = {"engine": "sieve", "mode": "any", "task_bytes": task_bytes, "tasks": tasks,
+                               "tasks_skipped": skipped, "windows_skipped": windows}
+        return out
+
+    def _any_device_windows(self, data, offsets, out):
+        """any_device for buffers above WINDOW_BYTES: runs of whole haystacks that fit one call each get their slice
+        of `out`; one haystack above the limit is scanned in windows that share max_pattern_len - 1 bytes (an
+        occurrence lies inside one of them whole) and share its flag, stopping at the first window that sets it."""
+        torch = _require_cuda()
+        dev = data.device
+        n = offsets.numel() - 1
+        limit = self.WINDOW_BYTES
+        lens = offsets[1:] - offsets[:-1]
+        oversized = bool((lens > limit).any().item())
+        h = 0
+        while h < n:
+            start = int(offsets[h].item())
+            if oversized and int(lens[h].item()) > limit:
+                hay, flag = data[start:start + int(lens[h].item())], out[h:h + 1]
+                step = limit - max(self.max_pattern_len - 1, 0)
+                w0 = 0
+                while not bool(flag.item()):
+                    w1 = min(w0 + limit, hay.numel())
+                    self.any_device(hay[w0:w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=dev), flag)
+                    if w1 == hay.numel():
+                        break
+                    w0 += step
+                h += 1
+                continue
+            # the longest run of whole haystacks that fits one call (and stops before an oversized one)
+            h1 = int(torch.searchsorted(offsets, torch.tensor([start + limit], dtype=torch.int64, device=dev), right=True).item()) - 1
+            h1 = max(h + 1, min(h1, n))
+            if oversized:
+                big = torch.nonzero(lens[h:h1] > limit)
+                if big.numel():
+                    h1 = h + int(big[0].item())
+            end = int(offsets[h1].item())
+            self.any_device(data[start:end], offsets[h:h1 + 1] - start, out[h:h1])
+            h = h1
+        return out
+
+    def any_host_batch(self, chunks: Sequence[bytes]):
+        """Host buffers (bytes-like objects, one per haystack) -> list of bool: does each contain any pattern.  The
+        offsets and the haystacks are gathered into the pinned staging buffer and go to the device in one copy."""
+        torch = _require_cuda()
+        n = len(chunks)
+        if n == 0:
+            return []
+        offs = np.zeros(n + 1, dtype=np.int64)
+        np.cumsum(np.fromiter((len(c) for c in chunks), dtype=np.int64, count=n), out=offs[1:])
+        total_bytes = int(offs[-1])
+        head = (8 * (n + 1) + 511) & ~511   # the offsets, then the bytes at a 512-byte boundary of the buffer
+        dev = torch.device("cuda", torch.cuda.current_device())
+        with self._host_lock:
+            host = self._pinned(head + total_bytes)
+            hv = host.numpy()
+            hv[:8 * (n + 1)].view(np.int64)[:] = offs
+            if n == 1:
+                hv[head:head + total_bytes] = np.frombuffer(chunks[0], dtype=np.uint8)
+            elif total_bytes:
+                hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
+            d = host[:head + total_bytes].to(dev, non_blocking=True)
+            mask = self.any_device(d[head:], d[:8 * (n + 1)].view(torch.int64))
+            return mask.cpu().tolist()
+
     def scan_device(self, data, offsets, overlapping=False, codepoints=False, capacity: Optional[int] = None,
                     sync: bool = True, ws_slot: int = 0):
         """Scan a device-resident batch.  data: uint8 CUDA tensor, offsets: int64
@@ -352,35 +499,17 @@ class _Automaton:
         img = self.image(dev)
         cap = capacity or max(1024, n * 2)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        # which kernel family: the position-parallel sieve (default) or the table walkers (forced by the tuning knob,
-        # or ENGINE = "table").  Results are identical; only the device images a scan needs differ.
-        forced = _capi.current_kernel()
         with self._lock, torch.cuda.device(dev):
-            # Which kernel family.  Results are identical; only speed and the device images a scan needs differ.
-            #   table  the automaton walkers: best when the scan lives in a few hundred states that fit in shared memory
-            #          (sparse matches in text) -- the profile of the data says so (hot-row coverage);
-            #   sieve  the position-parallel filter + exact verification: everything else (dense pattern sets, whose
-            #          states live in L2), and small inputs, where the profiling pass would cost more than the scan.
-            hot = None
-            if overlapping == 2 or forced == 5 or (forced == 0 and self.ENGINE == "sieve"):
-                use_sieve = True
-            elif forced in (1, 2, 3, 4) or self.ENGINE == "table":
-                use_sieve = False
-            elif self.implementation in (Implementation.ContiguousNFA, Implementation.NoncontiguousNFA):
-                use_sieve = True   # the caller asked for a compact (non-DFA) table format: that is the sieve image
-            else:
-                use_sieve = data.numel() < self.AUTO_PROFILE_BYTES and self._hot.get(dev.index if dev.index is not None else torch.cuda.current_device()) is None
-                if not use_sieve:
-                    hot = self.hot(dev, data, offsets, overlapping)
-                    use_sieve = bool(hot["rows"].reserved & 1)
+            hot = self._pick_engine(dev, data, offsets, overlapping)
+            use_sieve = hot is None
             if use_sieve:
                 sieve_t, sieve_d = self.sieve(dev)
-                hot = None
-            elif hot is None:
-                hot = self.hot(dev, data, offsets, overlapping)
             plan = self._plan(data, n)
             while True:
                 ws = self._workspace(dev, plan, n, cap, ws_slot)
+                reader = ws.pop("reader", None)
+                if reader is not None:   # any_device's comparison (maybe on another stream) reads this workspace first
+                    torch.cuda.current_stream(dev).wait_event(reader)
                 st = self._ws_struct(ws)
                 rc = self._L.acb_scan_batch(self._h, img.data_ptr(),
                                             hot["tensor"].data_ptr() if hot else None, C.byref(hot["rows"]) if hot else None,
@@ -814,6 +943,25 @@ class AhoCorasick:
         """Device-resident UTF-8 batch -> (matches, match_offsets, total); code point indexes."""
         return self._ac.scan_device(data, offsets, overlapping, codepoints=True, **kw)
 
+    # ---- additions: yes / no per haystack (the crate's AhoCorasick::is_match) ------------------------------
+    def is_match(self, haystack: str) -> bool:
+        """Does any pattern occur in `haystack`?  The same for every match kind, so there is no `overlapping`."""
+        if not isinstance(haystack, str):
+            raise TypeError("argument 'haystack': 'str' expected")
+        return self._ac.any_host_batch([haystack.encode("utf-8")])[0]
+
+    def is_match_batch(self, haystacks: Sequence[str]) -> list:
+        """``is_match`` for each haystack, in one transfer and one scan."""
+        hays = list(haystacks)
+        for h in hays:
+            if not isinstance(h, str):
+                raise TypeError("argument 'haystack': 'str' expected")
+        return self._ac.any_host_batch([h.encode("utf-8") for h in hays])
+
+    def is_match_device(self, data, offsets, out=None, sync: bool = True):
+        """Device-resident UTF-8 batch -> bool tensor (n,) on its device (see _Automaton.any_device)."""
+        return self._ac.any_device(data, offsets, out, sync)
+
     def scan_host(self, data, offsets, overlapping: bool = False, **kw):
         """Host-resident UTF-8 batch (uint8 array + int64 offsets) -> host arrays (matches (k, 4), match_offsets (n + 1));
         code point indexes.  Copies and scans are pipelined (see _Automaton.scan_host)."""
@@ -854,6 +1002,19 @@ class BytesAhoCorasick:
     def scan_device(self, data, offsets, overlapping: bool = False, **kw):
         """Device-resident batch -> (matches, match_offsets, total); byte offsets."""
         return self._ac.scan_device(data, offsets, overlapping, codepoints=False, **kw)
+
+    # ---- additions: yes / no per haystack (the crate's AhoCorasick::is_match) ------------------------------
+    def is_match(self, haystack) -> bool:
+        """Does any pattern occur in `haystack` (a bytes-like object)?  The same for every match kind."""
+        return self._ac.any_host_batch([_as_buffer_bytes(haystack)])[0]
+
+    def is_match_batch(self, haystacks: Sequence) -> list:
+        """``is_match`` for each haystack, in one transfer and one scan."""
+        return self._ac.any_host_batch([_as_buffer_bytes(h) for h in haystacks])
+
+    def is_match_device(self, data, offsets, out=None, sync: bool = True):
+        """Device-resident batch -> bool tensor (n,) on its device (see _Automaton.any_device)."""
+        return self._ac.any_device(data, offsets, out, sync)
 
     def scan_host(self, data, offsets, overlapping: bool = False, **kw):
         """Host-resident batch (uint8 array + int64 offsets) -> host arrays (matches (k, 4), match_offsets (n + 1));

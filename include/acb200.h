@@ -234,6 +234,32 @@ int acb_select_non_overlapping(const acb_automaton *a, const int64_t *dev_rows, 
                                 void *stream);
 
 /*
+ * Which haystacks contain an occurrence of any pattern.  Stands in for the crate's AhoCorasick::is_match, once per
+ * haystack of a device-resident batch (haystack h = dev_bytes[dev_offsets[h] .. dev_offsets[h+1]); total_bytes =
+ * length of the dev_bytes buffer, below 2^31).  The answer does not depend on the match kind (a haystack has a
+ * non-overlapping match of any kind iff some pattern occurs in it), so every automaton is accepted.  It needs the sieve
+ * image (acb_sieve_build / acb_sieve_write) and runs the sieve kernel in its any-match mode: one launch, no match list,
+ * no epilogue; the task size comes from acb_plan_scan (acb_tuning.segment_bytes applies when tuning.kernel = 5).
+ *
+ * dev_flags = u8[n_haystacks], read and written: a haystack whose flag is nonzero on entry is not scanned and keeps its
+ * flag; the call sets flag h to 1 when haystack h contains a pattern, and never clears one (zero the array for a fresh
+ * answer; OR-accumulating lets several calls -- windows of one haystack, several automata -- share one array).
+ * dev_scratch = u64[3], any contents: the call clears it (cudaMemsetAsync) and leaves
+ *   [0] its task counter (low 32 bits: tasks claimed, one more per warp than there are tasks);
+ *   [1] tasks skipped whole: tasks of task_bytes (a grid anchored at the 512-byte aligned address at or before dev_bytes)
+ *       whose part of the stream [dev_offsets[0], dev_offsets[n]) lies inside one haystack whose flag was set when a
+ *       warp claimed the task;
+ *   [2] windows not scanned: in the other tasks, the 512-byte windows of the grid from the first one, past the task's
+ *       first, that lies inside the haystack holding the rest of the task, if that haystack's flag was set when the
+ *       previous window was loaded, through the task's last window.
+ * Skipping changes speed only, never the flags.  Returns ACB_EINVAL, before any CUDA call, for a null pointer (a null
+ * dev_bytes is accepted when total_bytes == 0: an empty buffer), n_haystacks outside [0, 2^32 - 2],
+ * total_bytes >= 2^31 or an automaton without a sieve image.  n_haystacks == 0 or total_bytes == 0 launches nothing.
+ */
+int acb_any_match(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                  int64_t n_haystacks, uint64_t total_bytes, uint8_t *dev_flags, uint64_t *dev_scratch, void *stream);
+
+/*
  * Multi-GPU: the fixed-size block a rank contributes to the gather of the per-shard match lists (the only exchange
  * of the sharded path; NCCL all-gather over NVLink).  dev_block holds (cap + 1) records of 16 bytes: record 0 =
  * (match count, hay_base, complete flag, 0), then the first `cap` matches of a finished scan (dev_total / dev_out of
