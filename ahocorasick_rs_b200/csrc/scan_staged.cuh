@@ -54,7 +54,9 @@
 // touches 8 x 64 contiguous bytes.  Chunk k+1 is in flight while chunk k is
 // scanned.  The copies ask the L2 for whole 128-byte lines: a lane's rows are
 // 4 KiB apart, and fetching two chunks of a row per DRAM access instead of one
-// is what keeps the warps fed (DESIGN.md §6; a third staging buffer was slower).
+// is what keeps the warps fed.  The copy of the chunk that completes a line
+// marks it evict_first, so the spent stream leaves the L2 first (DESIGN.md §6;
+// a third staging buffer and L2 prefetches of a lane's later bytes were slower).
 #pragma once
 #include <type_traits>
 
@@ -178,6 +180,18 @@ __device__ __forceinline__ uint32_t cont_bytes(uint32_t w) { return __popc(w & ~
 // src_bytes is 0.
 __device__ __forceinline__ void cp_async16(uint32_t dst_smem, const void *src, uint32_t src_bytes) {
     asm volatile("cp.async.cg.shared.global.L2::128B [%0], [%1], 16, %2;\n" ::"r"(dst_smem), "l"(src), "r"(src_bytes) : "memory");
+}
+// The same with an evict_first L2 policy, for the copy of the chunk that completes its 128-byte line: that line is
+// spent, so the L2 gives it up before anything else.  (evict_first on every copy is much slower: the first half's
+// copy would evict the line before the second half is read.  DESIGN.md §6.)
+__device__ __forceinline__ void cp_async16_last(uint32_t dst_smem, const void *src, uint32_t src_bytes) {
+    asm volatile(
+        "{\n"
+        ".reg .b64 pol;\n"
+        "createpolicy.fractional.L2::evict_first.b64 pol, 1.0;\n"
+        "cp.async.cg.shared.global.L2::cache_hint.L2::128B [%0], [%1], 16, %2, pol;\n"
+        "}\n" ::"r"(dst_smem), "l"(src), "r"(src_bytes)
+        : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;\n" ::: "memory"); }
@@ -537,7 +551,10 @@ scan_staged_kernel(DevImage im, DevHot hot_img, Batch B, SegPlan P, Sink out, Se
                 const uint2 m = V == 1 ? mrow[i & 3] : lds64(cp_meta + i * 64);
                 const bool live = k < m.y;  // else the unit is zero-filled, from the grid origin (a valid address)
                 const uint8_t *src = reinterpret_cast<const uint8_t *>(gbase) + (live ? (size_t)(m.x + k * 4 + (lane & 3)) << 4 : 0);
-                cp_async16(dst + i * 8 * kRow, src, live ? 16u : 0u);
+                if (reinterpret_cast<uintptr_t>(src) & 64)
+                    cp_async16_last(dst + i * 8 * kRow, src, live ? 16u : 0u);
+                else
+                    cp_async16(dst + i * 8 * kRow, src, live ? 16u : 0u);
             }
             cp_async_commit();
         };
