@@ -88,6 +88,10 @@ def lib():
         L.acb_select_non_overlapping.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
         L.acb_any_match.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64, C.c_void_p, C.c_void_p,
                                     C.c_void_p]
+        L.acb_find_first.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64, C.c_void_p, C.c_void_p,
+                                     C.c_void_p]
+        L.acb_first_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.acb_rows_to_codepoints.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
         L.acb_pack_gather_block.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p, C.c_void_p]
         L.acb_scan_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(HotDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                      C.c_uint64, C.c_int, C.c_int, C.POINTER(Plan), C.POINTER(Workspace), C.c_void_p]
@@ -122,5 +126,5 @@ EXPORTS = [
     "acb_launch_count", "acb_set_tuning", "acb_timing_enable", "acb_timing_read",
     "acb_profile", "acb_hot_bytes", "acb_hot_build", "acb_hot_rows", "acb_hot_describe",
     "acb_sieve_build", "acb_sieve_write", "acb_sieve_describe", "acb_pack_gather_block", "acb_select_non_overlapping",
-    "acb_any_match",
+    "acb_any_match", "acb_find_first", "acb_first_rows", "acb_rows_to_codepoints",
 ]

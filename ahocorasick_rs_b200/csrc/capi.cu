@@ -173,7 +173,7 @@ constexpr int kAccGroups = 3;   // 16-byte groups in the stream
 constexpr int kAccTraps = 4;    // times a lane left the hot table
 constexpr int kAccRepairs = 5;  // segment boundaries repaired
 constexpr int kAccWords = 8;
-// acb_any_match's dev_scratch: [0] task counter (low u32), [1] tasks skipped whole, [2] windows not scanned
+// acb_any_match's and acb_find_first's dev_scratch: [0] task counter (low u32), [1] tasks skipped whole, [2] windows not scanned
 constexpr int kAnyScratchWords = 3;
 
 // totals[6] after a table walker's epilogue: which of its branches the scan took (the sieve epilogue uses
@@ -718,6 +718,133 @@ __global__ void select_rows_kernel(const long long *rows, unsigned long long n, 
     *count = w;
 }
 
+// ---------------------------------------------------------------------------
+// acb_first_rows: first-match keys (scan_sieve.cuh, FIRST) -> int64 rows (pattern, start, end), one thread per
+// haystack.  LeftmostFirst keys name (start, pattern): the end is start + the pattern's length.  The other two kinds
+// name (start, end): the pattern is the lowest pid of the reverse-trie node of those bytes -- the node stage 2 found --
+// reached by the same walk (hash of the W bytes before the end, then one child per byte towards the start).
+// ---------------------------------------------------------------------------
+__device__ uint32_t sieve_pid_of(const DevSieve &sv, const uint8_t *hay, uint32_t start, uint32_t end) {
+    uint32_t lo = 0, hi = 0;  // the 8 bytes ending at end, little endian (the byte at end - 1 is the top byte of lo)
+    for (uint32_t k = 1; k <= 8 && k <= end - start; k++) {
+        const uint32_t b = hay[end - k];
+        if (k <= 4)
+            lo |= b << (8 * (4 - k));
+        else
+            hi |= b << (8 * (8 - k));
+    }
+    const uint32_t klo = sv.W <= 4 ? lo >> (8u * (4u - sv.W)) : lo, khi = sv.W <= 4 ? 0u : hi >> (8u * (8u - sv.W));
+    const uint32_t x = klo + khi * kMixHi;
+    uint32_t s = __umulhi(x * kMulSlot, sv.ht_size), v = kSieveNoNode;
+    for (;;) {
+        const SieveSlot e = sv.ht[s];
+        if (e.node == kSieveNoNode) break;
+        if (e.key_lo == klo && e.key_hi == khi) {
+            v = e.node;
+            break;
+        }
+        s = (s + 1) & (sv.ht_size - 1);
+    }
+    for (uint32_t d = sv.W; v != kSieveNoNode && d < end - start; d++) {
+        const uint32_t b = hay[end - 1 - d];  // the byte before the d-byte suffix
+        const uint32_t first = sv.na[v].first_kid, nk = (sv.na[v].meta >> 8) & 0x1ffu;
+        uint32_t l0 = 0, l1 = nk;  // first child with byte >= b
+        while (l0 < l1) {
+            const uint32_t mid = (l0 + l1) >> 1;
+            if ((sv.na[first + mid].meta & 0xffu) < b)
+                l0 = mid + 1;
+            else
+                l1 = mid;
+        }
+        v = l0 < nk && (sv.na[first + l0].meta & 0xffu) == b ? first + l0 : kSieveNoNode;
+    }
+    if (v == kSieveNoNode || sv.nb[v].own_cnt == 0) return 0xffffffffu;  // (a key always names a pattern)
+    return sv.pids[sv.nb[v].own_off];  // ascending: the lowest index among patterns with these bytes
+}
+
+__global__ void first_rows_kernel(DevSieve sv, const uint32_t *pat_len, Batch B, const unsigned long long *keys, long long *rows, int kind) {
+    for (int64_t h = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; h < B.n_haystacks; h += (int64_t)gridDim.x * blockDim.x) {
+        const unsigned long long key = keys[h];
+        long long pid = -1, start = -1, end = -1;
+        if (key != ~0ull) {
+            const uint32_t hi = (uint32_t)(key >> 32), lo = (uint32_t)key;
+            if (kind == ACB_LEFTMOST_FIRST) {
+                start = hi;
+                pid = lo;
+                end = start + pat_len[lo];
+            } else {
+                end = kind == ACB_STANDARD ? hi : 0xffffffffu - lo;
+                start = kind == ACB_STANDARD ? end - (0xffffffffu - lo) : hi;
+                const uint32_t p = sieve_pid_of(sv, B.bytes + B.offsets[h], (uint32_t)start, (uint32_t)end);
+                pid = p == 0xffffffffu ? -1 : (long long)p;
+            }
+        }
+        rows[3 * h] = pid;
+        rows[3 * h + 1] = start;
+        rows[3 * h + 2] = end;
+    }
+}
+
+// ---------------------------------------------------------------------------
+// acb_rows_to_codepoints: byte rows -> code point rows.  The stream is cut into tiles of kCpTile bytes; a warp takes
+// tiles grid-stride and, for every haystack with a row that overlaps the tile before the row's end, counts the UTF-8
+// continuation bytes of that overlap before the row's start and before its end, and subtracts them from the output row
+// with one atomic each.  Work is the bytes before each row's end, spread over the whole grid whatever the haystacks'
+// sizes.  The input rows are only read (the output starts as their copy), so no warp sees another's subtraction.
+// ---------------------------------------------------------------------------
+constexpr int64_t kCpTile = 16384;
+
+__global__ void __launch_bounds__(256) rows_to_codepoints_kernel(Batch B, int64_t buf_bytes, const long long *rows, long long *cp) {
+    const uint32_t lane = threadIdx.x & 31;
+    // tiles cover the buffer; the stream [offsets[0], offsets[n]) is the part of it that is counted
+    const int64_t stream_lo = max(__ldg(B.offsets), (int64_t)0), stream_hi = min(__ldg(B.offsets + B.n_haystacks), buf_bytes);
+    const int64_t n_tiles = (buf_bytes + kCpTile - 1) / kCpTile;
+    const int64_t n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t t = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; t < n_tiles; t += n_warps) {
+        const int64_t lo = max(t * kCpTile, stream_lo), hi = min((t + 1) * kCpTile, stream_hi);
+        if (lo >= hi) continue;
+        for (int64_t h = find_haystack(B, lo); h < B.n_haystacks; h++) {
+            const int64_t hs = __ldg(B.offsets + h);
+            if (hs >= hi) break;
+            const int64_t start = __ldg(rows + 3 * h + 1), end = __ldg(rows + 3 * h + 2);
+            if (end < 0) continue;
+            const int64_t a = max(lo, hs), be = min(hi, hs + end), bs = min(hi, hs + start);
+            if (be <= a) continue;
+            // 16-byte chunks at aligned addresses; bytes outside [a, be) read as zero (not a continuation byte)
+            const int64_t p0 = a - (int64_t)(reinterpret_cast<uintptr_t>(B.bytes + a) & 15u);
+            unsigned long long ce = 0, cs = 0;
+            for (int64_t p = p0 + 16 * (int64_t)lane; p < be; p += 512) {
+                uint32_t w[4] = {0, 0, 0, 0};
+                if (p >= a && p + 16 <= be) {
+                    const uint4 v = __ldg(reinterpret_cast<const uint4 *>(B.bytes + p));
+                    w[0] = v.x, w[1] = v.y, w[2] = v.z, w[3] = v.w;
+                } else {
+                    for (int k = 0; k < 16; k++)
+                        if (p + k >= a && p + k < be) w[k >> 2] |= (uint32_t)__ldg(B.bytes + p + k) << (8 * (k & 3));
+                }
+                uint32_t m = 0;  // bit k: byte k of the chunk is a continuation byte (10xxxxxx)
+#pragma unroll
+                for (int j = 0; j < 4; j++) {
+                    const uint32_t f = w[j] & ~(w[j] << 1) & 0x80808080u;
+                    m |= (((f >> 7) & 1u) | ((f >> 14) & 2u) | ((f >> 21) & 4u) | ((f >> 28) & 8u)) << (4 * j);
+                }
+                const int64_t ks = min(max(bs - p, (int64_t)0), (int64_t)16);  // bytes of the chunk before the start
+                ce += __popc(m);
+                cs += __popc(m & ((1u << ks) - 1u));
+            }
+#pragma unroll
+            for (int d = 16; d >= 1; d >>= 1) {
+                ce += __shfl_xor_sync(0xffffffffu, ce, d);
+                cs += __shfl_xor_sync(0xffffffffu, cs, d);
+            }
+            if (lane == 0) {
+                if (cs) atomicAdd(reinterpret_cast<unsigned long long *>(cp + 3 * h + 1), 0ull - cs);
+                if (ce) atomicAdd(reinterpret_cast<unsigned long long *>(cp + 3 * h + 2), 0ull - ce);
+            }
+        }
+    }
+}
+
 // when the input is empty: nothing ran, publish zeros
 __global__ void zero_outputs_kernel(unsigned long long *unit_offsets, unsigned long long *match_offsets, int64_t n_haystacks,
                                     unsigned long long *totals) {
@@ -1135,8 +1262,9 @@ DevSieve make_sieve_view(const SieveHeader &h, const void *dev_sieve) {
     return v;
 }
 
-// ANY: the any-match mode (acb_any_match): hay_cont carries its flags and task_cont its two skip counters, out goes unused
-template <bool CP, bool ANY = false>
+// MODE kSieveAny (acb_any_match) / kSieveFirst + kind (acb_find_first): hay_cont carries the flags / keys and task_cont
+// the two skip counters, out goes unused
+template <bool CP, int MODE = kSieveList>
 int launch_sieve(const DevSieve &sv, const Batch &B, SievePlan &P, const Sink &out, uint32_t *task_cont, uint32_t *hay_cont,
                  unsigned int *task_counter, const DeviceInfo &d, cudaStream_t st) {
     // as many windows of text per warp as fit next to the filters (a power of two): the more, the fuller the rounds of
@@ -1149,7 +1277,7 @@ int launch_sieve(const DevSieve &sv, const Batch &B, SievePlan &P, const Sink &o
     P.ring = ring;
 #define ACB_SIEVE_GO(WC)                                                                                  \
     do {                                                                                                  \
-        auto kern = sieve_scan_kernel<CP, WC, ANY>;                                                       \
+        auto kern = sieve_scan_kernel<CP, WC, MODE>;                                                      \
         CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, d.max_smem_optin)); \
         kern<<<d.sms, kSieveThreads, smem, st>>>(sv, B, P, out, task_cont, hay_cont, task_counter);       \
     } while (0)
@@ -1186,6 +1314,55 @@ int launch_sieve_epilogue(SieveEpiArgs &E, const DeviceInfo &d, cudaStream_t st)
     const int use_bps = epilogue_blocks_per_sm(bps, n_work);
     CUDA_OK(cudaLaunchCooperativeKernel(reinterpret_cast<void *>(kern), dim3(d.sms * use_bps), dim3(kScanThreads), args, 0, st));
     g_launches++;
+    return ACB_OK;
+}
+
+int sieve_header(const acb_automaton *a, SieveHeader &sh) {
+    std::lock_guard<std::mutex> lock(a->impl->sieve_mutex);
+    if (a->impl->sieve.size() < sizeof(SieveHeader)) return fail(ACB_EINVAL, "acb_sieve_build has not been called");
+    std::memcpy(&sh, a->impl->sieve.data(), sizeof(sh));
+    return ACB_OK;
+}
+
+// acb_any_match (mode kSieveAny, out = u8 flags) and acb_find_first (kSieveFirst + kind, out = u64 keys): one launch of
+// the sieve kernel in a mode that writes no list and stops early
+int sieve_early_scan(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                     int64_t n_haystacks, uint64_t total_bytes, void *dev_out, uint64_t *dev_scratch, void *stream, int mode) {
+    if (!a || !dev_sieve || !dev_offsets || !dev_out || !dev_scratch || (total_bytes && !dev_bytes)) return fail(ACB_EINVAL, "null argument");
+    if (n_haystacks < 0 || n_haystacks > 0xfffffffell) return fail(ACB_EINVAL, "n_haystacks out of range (0 .. 2^32 - 2)");
+    if (total_bytes >= (1ull << 31)) return fail(ACB_EINVAL, "total_bytes must be below 2^31 (scan larger inputs in windows)");
+    SieveHeader sh;
+    if (int rc = sieve_header(a, sh)) return rc;
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CUDA_OK(cudaMemsetAsync(dev_scratch, 0, kAnyScratchWords * sizeof(uint64_t), st));
+    if (n_haystacks == 0 || total_bytes == 0) return ACB_OK;
+    acb_plan plan;
+    acb_plan_scan(a, dev_bytes, total_bytes, (uint64_t)n_haystacks, &plan);
+    SievePlan SP;
+    SP.origin = -(int64_t)(reinterpret_cast<uintptr_t>(dev_bytes) & 511u);
+    SP.task_bytes = plan.task_bytes;
+    SP.n_tasks = (int64_t)((total_bytes + (uint64_t)(-SP.origin) + plan.task_bytes - 1) / plan.task_bytes);
+    SP.buf_bytes = total_bytes;
+    SP.avg_len = total_bytes / (uint64_t)n_haystacks;
+    if (SP.avg_len < 1) SP.avg_len = 1;
+    const Batch B{dev_bytes, dev_offsets, n_haystacks};
+    const DevSieve sv = make_sieve_view(sh, dev_sieve);
+    unsigned long long *scr = reinterpret_cast<unsigned long long *>(dev_scratch);
+    // (the kernel's code-point pointers carry the skip counters and the flags / keys in these modes)
+    uint32_t *skipped = reinterpret_cast<uint32_t *>(scr + 1), *out = static_cast<uint32_t *>(dev_out);
+    unsigned int *counter = reinterpret_cast<unsigned int *>(scr);
+    int rc;
+    switch (mode) {
+        case kSieveAny: rc = launch_sieve<false, kSieveAny>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
+        case kSieveFirst + ACB_STANDARD: rc = launch_sieve<false, kSieveFirst + ACB_STANDARD>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
+        case kSieveFirst + ACB_LEFTMOST_FIRST: rc = launch_sieve<false, kSieveFirst + ACB_LEFTMOST_FIRST>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
+        case kSieveFirst + ACB_LEFTMOST_LONGEST: rc = launch_sieve<false, kSieveFirst + ACB_LEFTMOST_LONGEST>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
+        default: return fail(ACB_EINVAL, "unknown match kind");
+    }
+    if (rc) return rc;
+    CUDA_OK(cudaGetLastError());
     return ACB_OK;
 }
 
@@ -1235,35 +1412,57 @@ int acb_select_non_overlapping(const acb_automaton *a, const int64_t *dev_rows, 
 
 int acb_any_match(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
                   int64_t n_haystacks, uint64_t total_bytes, uint8_t *dev_flags, uint64_t *dev_scratch, void *stream) {
-    if (!a || !dev_sieve || !dev_offsets || !dev_flags || !dev_scratch || (total_bytes && !dev_bytes)) return fail(ACB_EINVAL, "null argument");
+    if (!dev_flags) return fail(ACB_EINVAL, "null argument");
+    return sieve_early_scan(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, dev_flags, dev_scratch, stream, kSieveAny);
+}
+
+int acb_find_first(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                   int64_t n_haystacks, uint64_t total_bytes, uint64_t *dev_keys, uint64_t *dev_scratch, void *stream) {
+    if (!dev_keys) return fail(ACB_EINVAL, "null argument");
+    if (!a) return fail(ACB_EINVAL, "null argument");
+    return sieve_early_scan(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, dev_keys, dev_scratch, stream,
+                            kSieveFirst + (int)a->impl->hdr.match_kind);
+}
+
+int acb_first_rows(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                   int64_t n_haystacks, const uint64_t *dev_keys, int64_t *dev_rows, void *stream) {
+    if (!a || !dev_sieve || !dev_offsets || !dev_keys || !dev_rows) return fail(ACB_EINVAL, "null argument");
     if (n_haystacks < 0 || n_haystacks > 0xfffffffell) return fail(ACB_EINVAL, "n_haystacks out of range (0 .. 2^32 - 2)");
-    if (total_bytes >= (1ull << 31)) return fail(ACB_EINVAL, "total_bytes must be below 2^31 (scan larger inputs in windows)");
     SieveHeader sh;
-    {
-        std::lock_guard<std::mutex> lock(a->impl->sieve_mutex);
-        if (a->impl->sieve.size() < sizeof(SieveHeader)) return fail(ACB_EINVAL, "acb_sieve_build has not been called");
-        std::memcpy(&sh, a->impl->sieve.data(), sizeof(sh));
-    }
+    if (int rc = sieve_header(a, sh)) return rc;
     DeviceInfo d;
     if (int rc = device_info(d)) return rc;
+    if (n_haystacks == 0) return ACB_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CUDA_OK(cudaMemsetAsync(dev_scratch, 0, kAnyScratchWords * sizeof(uint64_t), st));
-    if (n_haystacks == 0 || total_bytes == 0) return ACB_OK;
-    acb_plan plan;
-    acb_plan_scan(a, dev_bytes, total_bytes, (uint64_t)n_haystacks, &plan);
-    SievePlan SP;
-    SP.origin = -(int64_t)(reinterpret_cast<uintptr_t>(dev_bytes) & 511u);
-    SP.task_bytes = plan.task_bytes;
-    SP.n_tasks = (int64_t)((total_bytes + (uint64_t)(-SP.origin) + plan.task_bytes - 1) / plan.task_bytes);
-    SP.buf_bytes = total_bytes;
-    SP.avg_len = total_bytes / (uint64_t)n_haystacks;
-    if (SP.avg_len < 1) SP.avg_len = 1;
-    const Batch B{dev_bytes, dev_offsets, n_haystacks};
-    unsigned long long *scr = reinterpret_cast<unsigned long long *>(dev_scratch);
-    // (the kernel's code-point pointers carry the skip counters and the flags in this mode)
-    const int rc = launch_sieve<false, true>(make_sieve_view(sh, dev_sieve), B, SP, Sink{}, reinterpret_cast<uint32_t *>(scr + 1),
-                                             reinterpret_cast<uint32_t *>(dev_flags), reinterpret_cast<unsigned int *>(scr), d, st);
-    if (rc) return rc;
+    int64_t blocks = (n_haystacks + 127) / 128;
+    if (blocks > 16ll * d.sms) blocks = 16ll * d.sms;  // grid-stride beyond that
+    const uint32_t *pat_len = reinterpret_cast<const uint32_t *>(static_cast<const uint8_t *>(dev_sieve) + sh.off_pat_len);
+    first_rows_kernel<<<(unsigned)blocks, 128, 0, st>>>(make_sieve_view(sh, dev_sieve), pat_len, Batch{dev_bytes, dev_offsets, n_haystacks},
+                                                        reinterpret_cast<const unsigned long long *>(dev_keys),
+                                                        reinterpret_cast<long long *>(dev_rows), (int)a->impl->hdr.match_kind);
+    g_launches++;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+int acb_rows_to_codepoints(const uint8_t *dev_bytes, const int64_t *dev_offsets, int64_t n_haystacks, uint64_t total_bytes,
+                           const int64_t *dev_rows, int64_t *dev_cp_rows, void *stream) {
+    if (!dev_offsets || !dev_rows || !dev_cp_rows || (total_bytes && !dev_bytes)) return fail(ACB_EINVAL, "null argument");
+    if (dev_rows == dev_cp_rows) return fail(ACB_EINVAL, "dev_cp_rows must not be dev_rows");
+    if (n_haystacks < 0) return fail(ACB_EINVAL, "n_haystacks out of range");
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    if (n_haystacks == 0) return ACB_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CUDA_OK(cudaMemcpyAsync(dev_cp_rows, dev_rows, (uint64_t)n_haystacks * 3 * sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
+    if (total_bytes == 0) return ACB_OK;
+    const int64_t tiles = (int64_t)((total_bytes + kCpTile - 1) / kCpTile);
+    int64_t blocks = (tiles + 7) / 8;  // 8 warps per block, a tile per warp
+    if (blocks > 8ll * d.sms) blocks = 8ll * d.sms;  // grid-stride beyond that
+    rows_to_codepoints_kernel<<<(unsigned)blocks, 256, 0, st>>>(Batch{dev_bytes, dev_offsets, n_haystacks}, (int64_t)total_bytes,
+                                                                reinterpret_cast<const long long *>(dev_rows),
+                                                                reinterpret_cast<long long *>(dev_cp_rows));
+    g_launches++;
     CUDA_OK(cudaGetLastError());
     return ACB_OK;
 }

@@ -42,6 +42,19 @@
 //                 with the next window's bytes (only once that window lies inside it); when it is set, the warp stops
 //                 scanning, verifies what it had queued from earlier windows and moves on.
 // Flags set by other CTAs during the launch are read with ld.relaxed.gpu (never through the non-coherent cache).
+//
+// FIRST (acb_find_first): the answer is each haystack's first match for the automaton's match kind, as one u64 KEY per
+// haystack that stage 2 lowers with atomicMin (a smaller key is a better match; positions are haystack-relative):
+//   Standard         end << 32 | (0xffffffff - length)      earliest end, then the longest pattern
+//   LeftmostFirst    start << 32 | pattern                  leftmost start, then the lowest pattern index
+//   LeftmostLongest  start << 32 | (0xffffffff - end)       leftmost start, then the longest pattern
+// At one end position only the deepest terminal node can give the smallest key (shorter patterns ending there start
+// later; patterns with the same bytes are ranked by index, and a node's pids are ascending), so a matching position
+// yields one candidate and no walk along the match chain.  A position whose haystack-relative end is e can only give a
+// primary key (the high word) of at least e (Standard) or e - max_pattern_len (the leftmost kinds): it cannot beat a
+// key whose primary is below that bound.  The any-match skips apply with "flag set" read as "cannot beat the key"
+// (strictly: an equal primary may still win on the low word); the tail haystack's key is loaded, high word only, one
+// window ahead as its flag is.
 #pragma once
 #include "scan_staged.cuh"
 #include "sieve.h"
@@ -120,6 +133,18 @@ __device__ __forceinline__ uint32_t ld_flag(const uint8_t *p) {
     return v;
 }
 
+// the primary (high word) of a haystack's first-match key, coherent at device scope (other CTAs lower keys during the launch)
+__device__ __forceinline__ uint32_t ld_key_hi(const unsigned long long *p) {
+    uint32_t v;
+    asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];\n" : "=r"(v) : "l"(reinterpret_cast<const uint32_t *>(p) + 1) : "memory");
+    return v;
+}
+
+// what the kernel produces
+constexpr int kSieveList = 0;   // the overlapping match list (acb_scan_batch)
+constexpr int kSieveAny = 1;    // one flag per haystack (acb_any_match)
+constexpr int kSieveFirst = 2;  // one first-match key per haystack (acb_find_first): kSieveFirst + the match kind (ACB_*)
+
 // continuation bytes among the first nbytes (0..16) of the 16-byte chunk at shared address a
 __device__ __forceinline__ uint32_t cont_prefix(uint32_t a, uint32_t nbytes) {
     uint32_t n = 0;
@@ -148,14 +173,18 @@ __device__ __forceinline__ uint32_t warp_excl_scan(uint32_t v, uint32_t lane, ui
 //
 // Positions inside a task are 32-bit offsets from the task's start (`rel`); the 64-bit stream position is t_lo + rel.
 //
-// ANY (CP = false only): `out` is unused, and the two code-point pointers carry the any-match outputs instead (so the
-// list-mode instantiations keep their parameter block): hay_cont -> flags = u8[n_haystacks], task_cont -> skipped =
-// u64[2] = [tasks skipped whole, windows not scanned] (see acb_any_match).
-template <bool CP, int WC, bool ANY = false>
+// MODE kSieveAny and kSieveFirst + kind (CP = false only): `out` is unused, and the two code-point pointers carry the
+// mode's outputs instead (so the list-mode instantiations keep their parameter block): hay_cont -> flags =
+// u8[n_haystacks] (any) or keys = u64[n_haystacks] (first), task_cont -> skipped = u64[2] = [tasks skipped whole,
+// windows not scanned] (see acb_any_match, acb_find_first).
+template <bool CP, int WC, int MODE = kSieveList>
 __global__ void __launch_bounds__(kSieveThreads, 1)
 sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_cont, uint32_t *hay_cont, unsigned int *task_counter) {
-    static_assert(!(ANY && CP), "the any-match mode has no positions to count");
+    constexpr bool ANY = MODE == kSieveAny, FIRST = MODE >= kSieveFirst, EARLY = ANY || FIRST;  // EARLY: no list, work stops early
+    constexpr int KIND = MODE - kSieveFirst;  // (FIRST)
+    static_assert(!(EARLY && CP), "the any-match and first-match modes have no positions to count");
     uint8_t *const flags = reinterpret_cast<uint8_t *>(hay_cont);
+    unsigned long long *const keys = reinterpret_cast<unsigned long long *>(hay_cont);
     unsigned long long *const skipped = reinterpret_cast<unsigned long long *>(task_cont);
     extern __shared__ __align__(128) uint8_t smem[];
     const uint32_t bloom_s = (uint32_t)__cvta_generic_to_shared(smem);
@@ -222,7 +251,7 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
     };
 
     unsigned int claimed = 0;
-    uint32_t tasks_skipped = 0, windows_skipped = 0;  // (ANY)
+    uint32_t tasks_skipped = 0, windows_skipped = 0;  // (EARLY)
     if (lane == 0) claimed = atomicAdd(task_counter, 1u);
     for (;;) {
         const unsigned int task = __shfl_sync(0xffffffffu, claimed, 0);
@@ -230,7 +259,7 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
         if (lane == 0) claimed = atomicAdd(task_counter, 1u);  // the next one: its round trip overlaps this task
         const int64_t t_lo = P.origin + (int64_t)task * T;
         if (t_lo >= vhi || t_lo + (int64_t)T <= vlo) {
-            if (lane == 0 && !ANY) {
+            if (lane == 0 && !EARLY) {
                 out.unit_counts[task] = 0;
                 if (CP) task_cont[task] = 0;
             }
@@ -264,12 +293,21 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
         };
         int32_t offc = load_offc(hb);
         int32_t next_start = __shfl_sync(0xffffffffu, offc, 1);  // start of haystack hb + 1
-        // ANY: the haystack that holds the task's last stream byte, and its start (relative); from that start on the rest
-        // of the task lies inside it.  A task that lies inside it whole, with its flag set, is skipped.
+        // EARLY: the haystack that holds the task's last stream byte, and its start (relative); from that start on the rest
+        // of the task lies inside it.  A task that lies inside it whole, with its flag set (FIRST: whose first position
+        // cannot beat its key), is skipped.
         int64_t tail_h = 0;
         int32_t tail_s = 0x7fffffff;
-        uint32_t tail_flag = 0;  // lane 0: its flag, loaded with the next window's bytes (nonzero: stop before that window)
-        if (ANY) {
+        // lane 0: its flag (FIRST: its key's primary), loaded with the next window's bytes (stop before that window when
+        // the flag is nonzero; FIRST: when the window's first position cannot beat the key)
+        uint32_t tail_flag = FIRST ? 0xffffffffu : 0u;
+        // FIRST: no position of the tail haystack from rel on can beat a key whose primary is key_hi
+        auto cannot_win = [&](uint32_t rel, uint32_t key_hi) -> bool {
+            const uint32_t e = rel - (uint32_t)tail_s + 1u;  // haystack-relative end of a match whose last byte is at rel
+            const uint32_t bound = KIND == 0 ? e : e - min(e, sv.max_pat_len);
+            return bound > key_hi;
+        };
+        if (EARLY) {
             const uint32_t k = __popc(__ballot_sync(0xffffffffu, offc <= (int32_t)hi_r - 1));  // >= 1: lane 0 holds hb's start
             if (k < 32) {
                 tail_h = hb + k - 1;
@@ -280,11 +318,13 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
             }
             if (tail_s <= (int32_t)lo_r) {
                 uint32_t f = 0;
-                if (lane == 0) f = ld_flag(flags + tail_h);
-                if (__shfl_sync(0xffffffffu, f, 0)) {
+                if (lane == 0) f = FIRST ? ld_key_hi(keys + tail_h) : ld_flag(flags + tail_h);
+                f = __shfl_sync(0xffffffffu, f, 0);
+                if (FIRST ? cannot_win(lo_r, f) : f != 0) {
                     tasks_skipped++;
                     continue;
                 }
+                if (FIRST) tail_flag = f;
             }
         }
         // Haystack containing the byte at rel, and its start (relative).  The shuffles are executed by the whole warp (rel
@@ -333,7 +373,7 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
             const uint32_t rel = ent2.x, aux = ent2.w;
             int32_t hs;
             const int64_t h = hay_of(active ? rel : max(wrel, lo_r), hs);
-            uint32_t best = kSieveNoNode, cnt = 0;
+            uint32_t best = kSieveNoNode, cnt = 0, best_d = 0;  // best_d: the depth of best (FIRST)
             if (active && (int32_t)rel - (int32_t)(W - 1) >= hs) {
                 const uint32_t klo = ent2.y, khi = ent2.z;
                 const uint32_t x = klo + khi * kMixHi;
@@ -353,7 +393,10 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
                 uint2 na = make_uint2(0, 0);
                 if (v != kSieveNoNode) na = __ldg(reinterpret_cast<const uint2 *>(sv.na + v));
                 while (v != kSieveNoNode) {
-                    if (na.y & kNodeTerminal) best = v;
+                    if (na.y & kNodeTerminal) {
+                        best = v;
+                        if (FIRST) best_d = d;
+                    }
                     const uint32_t nk = (na.y >> 8) & 0x1ffu;
                     if (nk == 0 || (int32_t)rel - (int32_t)d < hs) break;  // no longer pattern, or it would start before the haystack
                     const uint32_t b = __ldg(tptr + ((int64_t)(int32_t)rel - (int64_t)d));
@@ -394,11 +437,23 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
                 }
                 if (ANY) {
                     if (best != kSieveNoNode) flags[h] = 1;  // a pattern ends here, inside haystack h
+                } else if (FIRST) {
+                    if (best != kSieveNoNode) {  // the best match ending here: the deepest terminal node, its lowest pid
+                        const uint32_t end_rel = rel + 1u - (uint32_t)hs, start_rel = end_rel - best_d;
+                        unsigned long long key;
+                        if (KIND == 0)
+                            key = (unsigned long long)end_rel << 32 | (0xffffffffu - best_d);
+                        else if (KIND == 1)
+                            key = (unsigned long long)start_rel << 32 | __ldg(sv.pids + __ldg(&sv.nb[best].own_off));
+                        else
+                            key = (unsigned long long)start_rel << 32 | (0xffffffffu - end_rel);
+                        atomicMin(keys + h, key);
+                    }
                 } else if (best != kSieveNoNode) {
                     cnt = __ldg(&sv.nb[best].chain_cnt);
                 }
             }
-            const uint32_t hits = ANY ? 0u : __ballot_sync(0xffffffffu, cnt != 0);
+            const uint32_t hits = EARLY ? 0u : __ballot_sync(0xffffffffu, cnt != 0);
             if (hits) {
                 uint32_t total;
                 const uint32_t exc = warp_excl_scan(cnt, lane, &total);
@@ -494,9 +549,10 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
         uint32_t cur_slot = slot_s(wrel);  // the ring slot of the current window
 
         for (;; wrel += kWin) {
-            if (ANY && (int32_t)wrel >= tail_s && __shfl_sync(0xffffffffu, tail_flag, 0)) {
-                // the rest of the task lies inside a flagged haystack: verify what earlier windows queued (it may belong
-                // to other haystacks), then stop
+            if (EARLY && (int32_t)wrel >= tail_s &&
+                (FIRST ? cannot_win(wrel, __shfl_sync(0xffffffffu, tail_flag, 0)) : __shfl_sync(0xffffffffu, tail_flag, 0) != 0)) {
+                // the rest of the task lies inside a flagged haystack (FIRST: none of its positions can beat its key):
+                // verify what earlier windows queued (it may belong to other haystacks), then stop
                 windows_skipped += (wlast - wrel) / kWin + 1;
                 for (;;) {
                     if (q2n > 32 || (q1n == 0 && q2n != 0))
@@ -515,8 +571,8 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
                     nxt = __ldg(reinterpret_cast<const uint4 *>(tptr + (wrel + kWin + 16 * lane)));
                 else
                     nxt = load16(wrel + kWin + 16 * lane);
-                // ANY: the flag that may end the task, in flight with the bytes it would save
-                if (ANY && lane == 0 && (int32_t)(wrel + kWin) >= tail_s) tail_flag = ld_flag(flags + tail_h);
+                // EARLY: the flag (key) that may end the task, in flight with the bytes it would save
+                if (EARLY && lane == 0 && (int32_t)(wrel + kWin) >= tail_s) tail_flag = FIRST ? ld_key_hi(keys + tail_h) : ld_flag(flags + tail_h);
             }
             // ---- fast path: first filter probe for the 16 positions of this lane ----
             uint32_t pz = __shfl_up_sync(0xffffffffu, cur.z, 1), pw = __shfl_up_sync(0xffffffffu, cur.w, 1);
@@ -651,11 +707,11 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
             carry_w = __shfl_sync(0xffffffffu, cur.w, 31);
             cur = nxt;
         }
-        if (lane == 0 && !ANY) out.unit_counts[task] = n_emitted;
+        if (lane == 0 && !EARLY) out.unit_counts[task] = n_emitted;
         if (CP && lane == 0) task_cont[task] = cp_before;
         __syncwarp();
     }
-    if (ANY && lane == 0) {
+    if (EARLY && lane == 0) {
         if (tasks_skipped) atomicAdd(skipped, (unsigned long long)tasks_skipped);
         if (windows_skipped) atomicAdd(skipped + 1, (unsigned long long)windows_skipped);
     }

@@ -299,6 +299,8 @@ uint64_t sieve_image_build(const uint8_t *blob, const uint64_t *offsets, uint64_
     off = align16(off + uint64_t(nb.size()) * sizeof(SieveNodeB));
     h.off_pids = off;
     off = align16(off + uint64_t(pids.size()) * 4 + 16);
+    h.off_pat_len = off;
+    off = align16(off + n * 4);
     h.total_bytes = off;
     out.assign(off, 0);
     uint8_t *img = out.data();
@@ -308,6 +310,10 @@ uint64_t sieve_image_build(const uint8_t *blob, const uint64_t *offsets, uint64_
     std::memcpy(img + h.off_node_a, na.data(), uint64_t(na.size()) * sizeof(SieveNodeA));
     std::memcpy(img + h.off_node_b, nb.data(), uint64_t(nb.size()) * sizeof(SieveNodeB));
     if (!pids.empty()) std::memcpy(img + h.off_pids, pids.data(), pids.size() * 4);
+    for (uint64_t i = 0; i < n; i++) {
+        const uint32_t len = (uint32_t)(offsets[i + 1] - offsets[i]);
+        std::memcpy(img + h.off_pat_len + 4 * i, &len, 4);
+    }
     return off;
 }
 

@@ -96,7 +96,7 @@ struct SieveHeader {
     uint32_t n_filter_entries;
     uint32_t prim_words;   // the primary bitmap: ONE bit per W-byte suffix, kept sparse (the fast path tests only this)
     uint32_t term_levels;  // bit d: some pattern is exactly d bytes long (d <= 16): only those levels carry end marks
-    uint32_t pad1, pad2;
+    uint64_t off_pat_len;  // u32[n_pids]: the length of pattern i (n_pids = the number of patterns; read by acb_first_rows)
     uint64_t off_bloom;    // u32[bloom_words]
     uint64_t off_ht;       // SieveSlot[ht_mask + 1]
     uint64_t off_node_a;   // SieveNodeA[n_nodes]

@@ -10,7 +10,9 @@ CUDA device every search raises.
 Additions next to the drop-in methods (the reference API is one haystack per
 call): ``find_matches_as_indexes_batch`` and ``scan_device`` for batches that
 are already device resident; ``is_match`` / ``is_match_batch`` /
-``is_match_device``, the crate's ``AhoCorasick::is_match`` per haystack.
+``is_match_device``, the crate's ``AhoCorasick::is_match`` per haystack;
+``find_first`` / ``find_first_batch`` / ``find_first_device``, the crate's
+``AhoCorasick::find`` per haystack.
 """
 from __future__ import annotations
 
@@ -450,6 +452,175 @@ class _Automaton:
             self.any_device(data[start:end], offsets[h:h1 + 1] - start, out[h:h1])
             h = h1
         return out
+
+    # ---- the first match per haystack (the crate's AhoCorasick::find) ---------------------------------------------
+    def first_order(self, row):
+        """Sort key of a (pattern, start, end) row: the first match of a haystack is the minimum over its overlapping
+        matches (select_non_overlapping in csrc/capi.cu, first iteration)."""
+        p, s, e = row
+        if self.matchkind == MatchKind.Standard:
+            return (e, s, p)
+        if self.matchkind == MatchKind.LeftmostFirst:
+            return (s, p)
+        return (s, -e, p)
+
+    def first_keys(self, data, offsets, keys):
+        """acb_find_first on the sieve: lowers the u64 keys (an int64 CUDA tensor (n,), -1 = no match yet) of a batch
+        below WINDOW_BYTES; returns the u64[3] scratch tensor (task counter, tasks skipped, windows not scanned)."""
+        torch = _require_cuda()
+        dev = data.device
+        n = offsets.numel() - 1
+        sieve_t, _ = self.sieve(dev)
+        scratch = torch.empty(3, dtype=torch.int64, device=dev)
+        rc = self._L.acb_find_first(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
+                                    keys.data_ptr(), scratch.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        if rc != _capi.ACB_OK:
+            raise RuntimeError(_capi.last_error())
+        return scratch
+
+    def first_rows(self, data, offsets, keys):
+        """acb_first_rows: keys -> int64 (n, 3) rows (pattern, start, end) in bytes, -1 rows where there is no match."""
+        torch = _require_cuda()
+        dev = data.device
+        n = offsets.numel() - 1
+        sieve_t, _ = self.sieve(dev)
+        rows = torch.empty((n, 3), dtype=torch.int64, device=dev)
+        rc = self._L.acb_first_rows(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, keys.data_ptr(),
+                                    rows.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        if rc != _capi.ACB_OK:
+            raise RuntimeError(_capi.last_error())
+        return rows
+
+    def _rows_to_codepoints(self, data, offsets, rows):
+        torch = _torch()
+        out = torch.empty_like(rows)
+        rc = self._L.acb_rows_to_codepoints(data.data_ptr(), offsets.data_ptr(), offsets.numel() - 1, data.numel(), rows.data_ptr(),
+                                            out.data_ptr(), torch.cuda.current_stream(data.device).cuda_stream)
+        if rc != _capi.ACB_OK:
+            raise RuntimeError(_capi.last_error())
+        return out
+
+    def first_device(self, data, offsets, codepoints: bool = False):
+        """Each haystack's first match for the match kind -> int64 CUDA tensor (n, 3) = (pattern, start, end), a row of
+        -1 where a haystack has none; code point indexes with codepoints.  Row h is element 0 of haystack h's
+        non-overlapping list (scan_device), for every match kind.
+
+        Where the engine rule of scan_device picks the sieve, its kernel runs in the first-match mode (acb_find_first:
+        no match list, work stops per haystack once no later position can beat the best match found), and the call
+        returns without waiting for the device.  Where it picks a table walker, the rows come from the walker's full
+        scan (which waits for it, as any_device's does), gathered on the device; the next scan that reuses the
+        workspace waits for that gather."""
+        torch = _require_cuda()
+        dev = data.device
+        n = offsets.numel() - 1
+        if n <= 0:
+            return torch.empty((0, 3), dtype=torch.int64, device=dev)
+        if data.numel() == 0:
+            return torch.full((n, 3), -1, dtype=torch.int64, device=dev)
+        if data.numel() > self.WINDOW_BYTES:
+            rows = self._first_device_windows(data, offsets)
+            return self._rows_to_codepoints(data, offsets, rows) if codepoints else rows
+        with self._lock, torch.cuda.device(dev):
+            if self._pick_engine(dev, data, offsets, False) is not None:
+                m, mo, total = self.scan_device(data, offsets, False, codepoints)
+                rows = torch.full((n, 3), -1, dtype=torch.int64, device=dev)
+                if total:
+                    has = mo[1:] > mo[:-1]
+                    first = m[mo[:-1].clamp(max=total - 1), 1:4].to(torch.int64)
+                    rows = torch.where(has[:, None], first, rows)
+                reader = torch.cuda.Event()
+                reader.record(torch.cuda.current_stream(dev))
+                self._ws[(dev.index if dev.index is not None else torch.cuda.current_device(), 0)]["reader"] = reader
+                self.last_stats = {"engine": self.last_stats.get("engine", "table"), "mode": "first"}
+                return rows
+            keys = torch.full((n,), -1, dtype=torch.int64, device=dev)   # all ones: no match yet
+            scratch = self.first_keys(data, offsets, keys)
+            rows = self.first_rows(data, offsets, keys)
+            task_bytes = int(self._plan(data, n).task_bytes)
+            self.last_stats = {"engine": "sieve", "mode": "first", "task_bytes": task_bytes,
+                               "tasks": (data.numel() + (data.data_ptr() & 511) + task_bytes - 1) // task_bytes,
+                               "skip_counters": scratch}   # device tensor: [task counter, tasks skipped, windows not scanned]
+        return self._rows_to_codepoints(data, offsets, rows) if codepoints else rows
+
+    def _first_device_windows(self, data, offsets):
+        """first_device (bytes) for buffers above WINDOW_BYTES: runs of whole haystacks that fit one call each get
+        their rows (positions are haystack-relative: nothing to rebase); one haystack above the limit goes to
+        _first_one_large."""
+        torch = _require_cuda()
+        dev = data.device
+        n = offsets.numel() - 1
+        limit = self.WINDOW_BYTES
+        rows = torch.full((n, 3), -1, dtype=torch.int64, device=dev)
+        lens = offsets[1:] - offsets[:-1]
+        oversized = bool((lens > limit).any().item())
+        h = 0
+        while h < n:
+            start = int(offsets[h].item())
+            if oversized and int(lens[h].item()) > limit:
+                best = self._first_one_large(data[start:start + int(lens[h].item())])
+                if best is not None:
+                    rows[h] = torch.tensor(best, dtype=torch.int64, device=dev)
+                h += 1
+                continue
+            # the longest run of whole haystacks that fits one call (and stops before an oversized one)
+            h1 = int(torch.searchsorted(offsets, torch.tensor([start + limit], dtype=torch.int64, device=dev), right=True).item()) - 1
+            h1 = max(h + 1, min(h1, n))
+            if oversized:
+                big = torch.nonzero(lens[h:h1] > limit)
+                if big.numel():
+                    h1 = h + int(big[0].item())
+            end = int(offsets[h1].item())
+            rows[h:h1] = self.first_device(data[start:end], offsets[h:h1 + 1] - start)
+            h = h1
+        return rows
+
+    def _first_one_large(self, hay):
+        """The first match (pattern, start, end) in bytes, or None, of one haystack above WINDOW_BYTES, scanned in
+        windows that share max_pattern_len - 1 bytes, in order.  A window sees every match that ends inside it and does
+        not end inside the bytes it shares with its predecessor.  Standard: the first window with a match holds the
+        earliest end.  The leftmost kinds: every match not seen yet ends past the current window, so it starts at or
+        after the next window's start; the search stops once the best start lies strictly before that."""
+        torch = _require_cuda()
+        dev = hay.device
+        limit = self.WINDOW_BYTES
+        step = limit - max(self.max_pattern_len - 1, 0)
+        best = None
+        w0 = 0
+        while True:
+            w1 = min(w0 + limit, hay.numel())
+            p, s, e = self.first_device(hay[w0:w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=dev))[0].tolist()
+            if p >= 0 and (best is None or self.first_order((p, s + w0, e + w0)) < self.first_order(best)):
+                best = (p, s + w0, e + w0)
+            if w1 == hay.numel():
+                return best
+            if best is not None and (self.matchkind == MatchKind.Standard or best[1] < w0 + step):
+                return best
+            w0 += step
+
+    def first_host_batch(self, chunks: Sequence[bytes], codepoints: bool):
+        """Host buffers (bytes-like objects, one per haystack) -> list of (pattern, start, end) or None: each one's first
+        match.  The offsets and the haystacks are gathered into the pinned staging buffer and go to the device in one
+        copy; the rows come back in one."""
+        torch = _require_cuda()
+        n = len(chunks)
+        if n == 0:
+            return []
+        offs = np.zeros(n + 1, dtype=np.int64)
+        np.cumsum(np.fromiter((len(c) for c in chunks), dtype=np.int64, count=n), out=offs[1:])
+        total_bytes = int(offs[-1])
+        head = (8 * (n + 1) + 511) & ~511   # the offsets, then the bytes at a 512-byte boundary of the buffer
+        dev = torch.device("cuda", torch.cuda.current_device())
+        with self._host_lock:
+            host = self._pinned(head + total_bytes)
+            hv = host.numpy()
+            hv[:8 * (n + 1)].view(np.int64)[:] = offs
+            if n == 1:
+                hv[head:head + total_bytes] = np.frombuffer(chunks[0], dtype=np.uint8)
+            elif total_bytes:
+                hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
+            d = host[:head + total_bytes].to(dev, non_blocking=True)
+            rows = self.first_device(d[head:], d[:8 * (n + 1)].view(torch.int64), codepoints).cpu().tolist()
+        return [tuple(r) if r[0] >= 0 else None for r in rows]
 
     def any_host_batch(self, chunks: Sequence[bytes]):
         """Host buffers (bytes-like objects, one per haystack) -> list of bool: does each contain any pattern.  The
@@ -962,6 +1133,27 @@ class AhoCorasick:
         """Device-resident UTF-8 batch -> bool tensor (n,) on its device (see _Automaton.any_device)."""
         return self._ac.any_device(data, offsets, out, sync)
 
+    # ---- additions: the first match per haystack (the crate's AhoCorasick::find) ---------------------------------
+    def find_first(self, haystack: str):
+        """-> (pattern index, start, end) in code points, or None: ``find_matches_as_indexes(haystack)[0]``, found
+        without the rest of the list."""
+        if not isinstance(haystack, str):
+            raise TypeError("argument 'haystack': 'str' expected")
+        return self._ac.first_host_batch([haystack.encode("utf-8")], codepoints=True)[0]
+
+    def find_first_batch(self, haystacks: Sequence[str]) -> list:
+        """``find_first`` for each haystack, in one transfer and one scan."""
+        hays = list(haystacks)
+        for h in hays:
+            if not isinstance(h, str):
+                raise TypeError("argument 'haystack': 'str' expected")
+        return self._ac.first_host_batch([h.encode("utf-8") for h in hays], codepoints=True)
+
+    def find_first_device(self, data, offsets):
+        """Device-resident UTF-8 batch -> int64 tensor (n, 3) of (pattern, start, end) in code points, -1 rows where a
+        haystack has no match (see _Automaton.first_device)."""
+        return self._ac.first_device(data, offsets, codepoints=True)
+
     def scan_host(self, data, offsets, overlapping: bool = False, **kw):
         """Host-resident UTF-8 batch (uint8 array + int64 offsets) -> host arrays (matches (k, 4), match_offsets (n + 1));
         code point indexes.  Copies and scans are pipelined (see _Automaton.scan_host)."""
@@ -1015,6 +1207,21 @@ class BytesAhoCorasick:
     def is_match_device(self, data, offsets, out=None, sync: bool = True):
         """Device-resident batch -> bool tensor (n,) on its device (see _Automaton.any_device)."""
         return self._ac.any_device(data, offsets, out, sync)
+
+    # ---- additions: the first match per haystack (the crate's AhoCorasick::find) ---------------------------------
+    def find_first(self, haystack):
+        """-> (pattern index, start, end) in bytes, or None: ``find_matches_as_indexes(haystack)[0]``, found without
+        the rest of the list."""
+        return self._ac.first_host_batch([_as_buffer_bytes(haystack)], codepoints=False)[0]
+
+    def find_first_batch(self, haystacks: Sequence) -> list:
+        """``find_first`` for each haystack, in one transfer and one scan."""
+        return self._ac.first_host_batch([_as_buffer_bytes(h) for h in haystacks], codepoints=False)
+
+    def find_first_device(self, data, offsets):
+        """Device-resident batch -> int64 tensor (n, 3) of (pattern, start, end) in bytes, -1 rows where a haystack has
+        no match (see _Automaton.first_device)."""
+        return self._ac.first_device(data, offsets, codepoints=False)
 
     def scan_host(self, data, offsets, overlapping: bool = False, **kw):
         """Host-resident batch (uint8 array + int64 offsets) -> host arrays (matches (k, 4), match_offsets (n + 1));

@@ -260,6 +260,51 @@ int acb_any_match(const acb_automaton *a, const void *dev_sieve, const uint8_t *
                   int64_t n_haystacks, uint64_t total_bytes, uint8_t *dev_flags, uint64_t *dev_scratch, void *stream);
 
 /*
+ * Each haystack's first match for the automaton's match kind: the first record the reference's non-overlapping
+ * iterator (try_find_iter, src/lib.rs:58-60) yields, i.e. the crate's AhoCorasick::find, once per haystack of a
+ * device-resident batch (haystack h = dev_bytes[dev_offsets[h] .. dev_offsets[h+1]); total_bytes = length of the
+ * dev_bytes buffer, below 2^31).  Three calls:
+ *
+ * acb_find_first runs the sieve kernel in its first-match mode: one launch, no match list, no epilogue, no
+ * synchronisation, every match kind.  dev_keys = u64[n_haystacks], read and written: key h is lowered (atomic minimum)
+ * to the best match found in haystack h and never raised; ~0 (UINT64_MAX) = no match.  Positions in a key are byte
+ * offsets relative to the haystack's start, and a smaller key is a better match:
+ *   ACB_STANDARD           end << 32 | (0xffffffff - (end - start))   earliest end, then the longest pattern
+ *   ACB_LEFTMOST_FIRST     start << 32 | pattern                       leftmost start, then the lowest pattern index
+ *   ACB_LEFTMOST_LONGEST   start << 32 | (0xffffffff - end)            leftmost start, then the longest pattern
+ * (patterns with the same bytes are ranked by index).  A key given on entry is a bound: positions that cannot beat it
+ * are not scanned -- a position whose haystack-relative end is e gives a key whose high word is at least e (Standard)
+ * or e - max_pattern_len (the leftmost kinds), and it cannot beat a key whose high word is strictly below that.  Fill
+ * the array with ~0 for a fresh answer; min-accumulating lets the windows of one haystack share a key.
+ * dev_scratch = u64[3], any contents: as acb_any_match's, with "flag set" read as "no position from the task's first
+ * byte (the window's first byte) on can beat the key":
+ *   [0] its task counter; [1] tasks skipped whole: tasks whose part of the stream lies inside one haystack, and whose
+ *   first byte's position could not beat that haystack's key when a warp claimed the task; [2] windows not scanned: in
+ *   the other tasks, the 512-byte windows of the grid from the first one, past the task's first, that lies inside the
+ *   haystack holding the rest of the task, if its first byte's position could not beat that haystack's key when the
+ *   previous window was loaded, through the task's last window.
+ * Skipping changes speed only, never the keys.  Argument checks, the 2^31 limit and the empty cases are acb_any_match's.
+ *
+ * acb_first_rows decodes the keys into dev_rows = int64[n_haystacks][3] = (pattern, start, end), byte offsets relative
+ * to the haystack, and (-1, -1, -1) where the key is ~0.  It reads the sieve image (pattern lengths, and the reverse
+ * trie that names the pattern of a Standard or LeftmostLongest key) and, for those two kinds, the bytes of the
+ * haystacks with a match; dev_bytes and dev_offsets must be the buffers the keys were found in.  One launch.
+ *
+ * acb_rows_to_codepoints converts such rows, of a UTF-8 batch, to code point indexes (what codepoints != 0 gives
+ * acb_scan_batch): dev_cp_rows (same shape, not dev_rows) gets dev_rows with start and end lowered by the continuation
+ * bytes of the haystack before them.  Positions are 64-bit: total_bytes may exceed 2^31.  Work is the bytes before each
+ * row's end, spread over the whole grid.  One device-to-device copy and one launch, no synchronisation.
+ *
+ * All three return ACB_EINVAL, before any CUDA call, for a null pointer or n_haystacks outside [0, 2^32 - 2].
+ */
+int acb_find_first(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                   int64_t n_haystacks, uint64_t total_bytes, uint64_t *dev_keys, uint64_t *dev_scratch, void *stream);
+int acb_first_rows(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                   int64_t n_haystacks, const uint64_t *dev_keys, int64_t *dev_rows, void *stream);
+int acb_rows_to_codepoints(const uint8_t *dev_bytes, const int64_t *dev_offsets, int64_t n_haystacks, uint64_t total_bytes,
+                           const int64_t *dev_rows, int64_t *dev_cp_rows, void *stream);
+
+/*
  * Multi-GPU: the fixed-size block a rank contributes to the gather of the per-shard match lists (the only exchange
  * of the sharded path; NCCL all-gather over NVLink).  dev_block holds (cap + 1) records of 16 bytes: record 0 =
  * (match count, hay_base, complete flag, 0), then the first `cap` matches of a finished scan (dev_total / dev_out of
