@@ -12,6 +12,7 @@ LIB_PATH = os.environ.get("ACB200_LIB") or os.path.join(HERE, "libacb200.so")
 
 ACB_OK = 0
 ACB_EINVAL, ACB_EBUILD, ACB_EUNSUPPORTED, ACB_ECUDA, ACB_ECAPACITY = -1, -2, -3, -4, -5
+ACB_LONG_STRETCH = 4096   # include/acb200.h: longer per-haystack overlapping lists are counted by the whole grid
 
 
 class Plan(C.Structure):
@@ -90,6 +91,11 @@ def lib():
                                     C.c_void_p]
         L.acb_find_first.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64, C.c_void_p, C.c_void_p,
                                      C.c_void_p]
+        L.acb_count_overlapping.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64, C.c_void_p,
+                                            C.c_void_p, C.c_void_p]
+        L.acb_count_non_overlapping.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64, C.POINTER(Plan),
+                                                C.POINTER(Workspace), C.c_void_p, C.c_void_p]
+        L.acb_count_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
         L.acb_first_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
         L.acb_rows_to_codepoints.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
         L.acb_pack_gather_block.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p, C.c_void_p]
@@ -127,4 +133,5 @@ EXPORTS = [
     "acb_profile", "acb_hot_bytes", "acb_hot_build", "acb_hot_rows", "acb_hot_describe",
     "acb_sieve_build", "acb_sieve_write", "acb_sieve_describe", "acb_pack_gather_block", "acb_select_non_overlapping",
     "acb_any_match", "acb_find_first", "acb_first_rows", "acb_rows_to_codepoints",
+    "acb_count_overlapping", "acb_count_non_overlapping", "acb_count_rows",
 ]

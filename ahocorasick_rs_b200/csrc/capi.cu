@@ -478,8 +478,9 @@ __device__ __forceinline__ unsigned long long first_of_haystack(const acb_match 
 }
 
 // The reference's non-overlapping iteration over ONE haystack, as a selection from its overlapping list r[0 .. n)
-// (sorted by end, start, pattern).  The selected records are packed to the front; returns how many.
-template <int MODE>
+// (sorted by end, start, pattern).  The selected records are packed to the front (PACK = false: only counted); returns
+// how many.
+template <int MODE, bool PACK = true>
 __device__ __forceinline__ uint32_t select_non_overlapping(acb_match *r, unsigned long long n, uint32_t max_len, int longest) {
     unsigned long long w = 0;
     uint32_t s = 0;  // the search restarts here (the end of the previous match)
@@ -488,7 +489,10 @@ __device__ __forceinline__ uint32_t select_non_overlapping(acb_match *r, unsigne
         for (unsigned long long i = 0; i < n; i++) {
             const uint4 m = reinterpret_cast<const uint4 *>(r)[i];
             if (m.z >= s) {
-                reinterpret_cast<uint4 *>(r)[w++] = m;
+                if (PACK)
+                    reinterpret_cast<uint4 *>(r)[w++] = m;
+                else
+                    w++;
                 s = m.w;
             }
         }
@@ -510,17 +514,20 @@ __device__ __forceinline__ uint32_t select_non_overlapping(acb_match *r, unsigne
             }
         }
         if (!have) break;
-        reinterpret_cast<uint4 *>(r)[w++] = best;  // w <= i: only records that can no longer be chosen are overwritten
+        if (PACK)
+            reinterpret_cast<uint4 *>(r)[w++] = best;  // w <= i: only records that can no longer be chosen are overwritten
+        else
+            w++;
         s = best.w;
         while (i < n && r[i].end <= s) i++;
     }
     return (uint32_t)w;
 }
 
-template <int MODE, bool CP>
-__global__ void __launch_bounds__(kScanThreads) sieve_epilogue_kernel(SieveEpiArgs E) {
-    namespace cg = cooperative_groups;
-    cg::grid_group grid = cg::this_grid();
+// phases 1-3 of the sieve epilogue: the ordered overlapping list, and totals[6] / [7] = its length / the raw records
+// emitted (the caller's grid barrier publishes them)
+template <bool CP>
+__device__ __forceinline__ void sieve_order_list(const SieveEpiArgs &E, cooperative_groups::grid_group &grid) {
     const uint64_t tiles = (E.n_tasks + kScanTile - 1) / kScanTile;
     const uint64_t ctiles = CP ? tiles : 0;
     // phase 1 + 2: where each task's matches go (and, code points, the continuation bytes before each task)
@@ -564,6 +571,15 @@ __global__ void __launch_bounds__(kScanThreads) sieve_epilogue_kernel(SieveEpiAr
             E.totals[6] = E.unit_offsets[E.n_tasks];
             E.totals[7] = E.acc[kAccRaw];
         }
+    }
+}
+
+template <int MODE, bool CP>
+__global__ void __launch_bounds__(kScanThreads) sieve_epilogue_kernel(SieveEpiArgs E) {
+    namespace cg = cooperative_groups;
+    cg::grid_group grid = cg::this_grid();
+    sieve_order_list<CP>(E, grid);
+    {
         if (MODE != kModeOverlap) {
             // the per-haystack selection counts start at zero (the task counts in this array were consumed by phase 2)
             for (int64_t h = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; h < E.B.n_haystacks; h += (int64_t)gridDim.x * blockDim.x) E.unit_counts[h] = 0;
@@ -654,6 +670,224 @@ __global__ void __launch_bounds__(kScanThreads) sieve_epilogue_kernel(SieveEpiAr
         E.totals[7] = 0;
         E.acc[kAccRaw] = E.acc[kAccGroups] = E.acc[kAccTraps] = E.acc[kAccRepairs] = 0;
         E.acc[kAccQueue] = 0;
+    }
+}
+
+// ---------------------------------------------------------------------------
+// Non-overlapping COUNTS (acb_count_non_overlapping, acb_count_rows).  The serial selection restarts at the end s of
+// every match it picks, and what it picks next depends on s alone:
+//   NEXT(s) = the serial inner loop of select_non_overlapping started at the first record whose end is after s --
+//             Standard: the first record with start >= s; leftmost: the best such record, with the look-ahead break.
+// NEXT(s) has a higher index than every record ending at or before s.  Give record i the successor NEXT(end_i): the
+// selected matches are the chain NEXT(0), NEXT(end of that), ..., and the count is its length, found by pointer
+// jumping over (next, rank) pairs in ceil(log2(stretch)) rounds -- a few grid barriers instead of one thread walking
+// the whole stretch.  A stretch of at most ACB_LONG_STRETCH records is still counted by one thread (the serial loop is
+// faster than the barriers there).
+// ---------------------------------------------------------------------------
+constexpr uint32_t kNoNext = 0xffffffffu;   // end of a chain
+constexpr uint32_t kLongMark = 0xffffffffu; // unit_counts[h]: haystack h's stretch takes the parallel path
+
+struct SelRec {
+    long long pid, start, end;
+};
+__device__ __forceinline__ SelRec sel_rec(const acb_match *r, unsigned long long j) {
+    const uint4 m = reinterpret_cast<const uint4 *>(r)[j];
+    return {(long long)m.y, (long long)m.z, (long long)m.w};
+}
+__device__ __forceinline__ SelRec sel_rec(const long long *rows, unsigned long long j) {  // (haystack, pattern, start, end)
+    return {rows[4 * j + 1], rows[4 * j + 2], rows[4 * j + 3]};
+}
+
+// NEXT(s) in r[0 .. n), sorted by (end, start, pattern); n = none
+template <int MODE, class T>
+__device__ __forceinline__ unsigned long long next_selected(const T *r, unsigned long long n, long long s, long long max_len, int longest) {
+    unsigned long long lo = 0, hi = n;  // the first record whose end is after s
+    while (lo < hi) {
+        const unsigned long long mid = (lo + hi) >> 1;
+        if (sel_rec(r, mid).end <= s)
+            lo = mid + 1;
+        else
+            hi = mid;
+    }
+    if (MODE == kModeStandard) {
+        for (unsigned long long j = lo; j < n; j++)
+            if (sel_rec(r, j).start >= s) return j;
+        return n;
+    }
+    bool have = false;
+    SelRec best = {0, 0, 0};
+    unsigned long long at = n;
+    for (unsigned long long j = lo; j < n; j++) {
+        const SelRec m = sel_rec(r, j);
+        if (have && m.end > best.start + max_len) break;  // everything from here on starts after `best` does
+        if (m.start < s) continue;
+        bool better = !have || m.start < best.start;
+        if (have && m.start == best.start) better = longest ? (m.end > best.end || (m.end == best.end && m.pid < best.pid)) : (m.pid < best.pid);
+        if (better) {
+            best = m;
+            at = j;
+            have = true;
+        }
+    }
+    return at;
+}
+
+// one round of pointer jumping for record i: pairs[i] = (next, rank) -- rank = records on the chain from i on that
+// the rounds so far have summed; half `src` holds the current pairs, the other half gets the next ones
+__device__ __forceinline__ void jump_pair(uint4 *pairs, unsigned long long i, int src) {
+    const uint4 p = pairs[i];
+    uint32_t nx = src ? p.z : p.x, rk = src ? p.w : p.y;
+    if (nx != kNoNext) {
+        const uint4 q = pairs[nx];
+        rk += src ? q.w : q.y;
+        nx = src ? q.z : q.x;
+    }
+    if (src)
+        reinterpret_cast<uint2 *>(pairs + i)[0] = make_uint2(nx, rk);
+    else
+        reinterpret_cast<uint2 *>(pairs + i)[1] = make_uint2(nx, rk);
+}
+
+__device__ __forceinline__ uint32_t ceil_log2(unsigned long long x) { return x <= 1 ? 0u : 64u - (uint32_t)__clzll(x - 1); }
+
+// a block's sum into *dst (every thread of the block calls it)
+__device__ __forceinline__ void block_add(unsigned long long *dst, unsigned long long v) {
+#pragma unroll
+    for (int d = 16; d >= 1; d >>= 1) v += __shfl_down_sync(0xffffffffu, v, d);
+    if ((threadIdx.x & 31) == 0 && v) atomicAdd(dst, v);
+}
+
+// The count variant of sieve_epilogue_kernel (MODE kModeStandard / kModeLeftmost, no code points): phases 1-3 place
+// the overlapping list (from E.raw = dev_raw into E.ordered = dev_out), phase 4 counts each haystack's selection
+// without packing it, straight into counts[h].  Stretches longer than ACB_LONG_STRETCH are counted by the whole grid
+// (successors, then pointer jumping over (next, rank) pairs kept in dev_raw, which phase 3 has consumed: 16 bytes per
+// record are two pairs, double-buffered).  totals[2] = haystacks counted that way; during the launch totals[3] sums the
+// counts and totals[5] holds the longest such stretch.
+template <int MODE>
+__global__ void __launch_bounds__(kScanThreads) sieve_count_epilogue_kernel(SieveEpiArgs E, unsigned long long *counts) {
+    namespace cg = cooperative_groups;
+    cg::grid_group grid = cg::this_grid();
+    if (blockIdx.x == 0 && threadIdx.x == 0) E.totals[2] = E.totals[3] = E.totals[5] = 0;  // (read only after phase 4's barrier)
+    sieve_order_list<false>(E, grid);
+    for (int64_t h = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; h < E.B.n_haystacks; h += (int64_t)gridDim.x * blockDim.x) counts[h] = 0;
+    grid.sync();
+    const unsigned long long list_total = E.totals[6];
+    const unsigned long long raw_total = E.totals[7];
+    auto finish = [&](bool complete) {
+        if (blockIdx.x == 0 && threadIdx.x == 0) {
+            E.totals[0] = complete ? E.totals[3] : list_total;
+            E.totals[1] = complete ? 1 : 0;
+            E.totals[3] = E.totals[5] = E.totals[7] = 0;
+            E.totals[4] = raw_total > list_total ? raw_total : list_total;  // room the overlapping list needs
+            E.acc[kAccRaw] = E.acc[kAccGroups] = E.acc[kAccTraps] = E.acc[kAccRepairs] = 0;
+            E.acc[kAccQueue] = 0;
+        }
+    };
+    if (list_total > E.out_cap || raw_total > E.raw_cap) {
+        finish(false);  // the list has holes: every count stays zero, the caller retries with the room reported
+        return;
+    }
+    const unsigned long long avail = list_total;
+    const acb_match *const list = E.ordered;
+    uint4 *const pairs = reinterpret_cast<uint4 *>(const_cast<acb_match *>(E.raw));
+    const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+    const unsigned long long first_i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    // phase 4: the thread that sees a haystack's first record owns its stretch
+    unsigned long long sum = 0;
+    for (unsigned long long i = first_i; i < avail; i += stride) {
+        const uint32_t hc = list[i].haystack;
+        if (i && list[i - 1].haystack == hc) continue;
+        // the stretch's end: galloping, then binary search (a long stretch is not walked by one thread)
+        unsigned long long a = i + 1, step = 1;  // list[a - 1] is in the stretch
+        for (;;) {
+            const unsigned long long b = a + step - 1;
+            if (b >= avail || list[b].haystack != hc) break;
+            a = b + 1;
+            step <<= 1;
+        }
+        unsigned long long hi = a + step - 1 < avail ? a + step - 1 : avail;
+        while (a < hi) {
+            const unsigned long long mid = (a + hi) >> 1;
+            if (list[mid].haystack == hc)
+                a = mid + 1;
+            else
+                hi = mid;
+        }
+        const unsigned long long len = a - i;
+        if (len <= ACB_LONG_STRETCH) {
+            const uint32_t c = select_non_overlapping<MODE, false>(const_cast<acb_match *>(list) + i, len, E.max_pat_len, E.longest);
+            counts[hc] = c;
+            E.unit_counts[hc] = 0;
+            sum += c;
+        } else {
+            E.unit_counts[hc] = kLongMark;
+            E.unit_offsets[hc] = i;
+            counts[hc] = a;  // (the stretch's end, until its count replaces it)
+            atomicAdd(E.totals + 2, 1ull);
+            atomicMax(E.totals + 5, len);
+        }
+    }
+    block_add(E.totals + 3, sum);
+    grid.sync();
+    if (E.totals[2]) {
+        // successors: absolute list indices (a list of 2^32 records would not fit the device's memory twice)
+        for (unsigned long long i = first_i; i < avail; i += stride) {
+            const uint32_t hc = list[i].haystack;
+            if (E.unit_counts[hc] != kLongMark) continue;
+            const unsigned long long lo = E.unit_offsets[hc], n = counts[hc] - lo;
+            const unsigned long long nx = next_selected<MODE>(list + lo, n, (long long)list[i].end, E.max_pat_len, E.longest);
+            reinterpret_cast<uint2 *>(pairs + i)[0] = make_uint2(nx == n ? kNoNext : (uint32_t)(lo + nx), 1u);
+        }
+        grid.sync();
+        const uint32_t rounds = ceil_log2(E.totals[5]);
+        for (uint32_t r = 0; r < rounds; r++) {
+            for (unsigned long long i = first_i; i < avail; i += stride)
+                if (E.unit_counts[list[i].haystack] == kLongMark) jump_pair(pairs, i, (int)(r & 1));
+            grid.sync();
+        }
+        // the count: the rank of the chain's head, NEXT(0)
+        sum = 0;
+        for (unsigned long long i = first_i; i < avail; i += stride) {
+            const uint32_t hc = list[i].haystack;
+            if (E.unit_counts[hc] != kLongMark || (i && list[i - 1].haystack == hc)) continue;
+            const unsigned long long n = counts[hc] - i;
+            const unsigned long long head = next_selected<MODE>(list + i, n, 0, E.max_pat_len, E.longest);
+            const uint4 p = pairs[i + head];  // (head < n: the stretch has a record, so the selection picks one)
+            const uint32_t c = (rounds & 1) ? p.w : p.y;
+            counts[hc] = c;
+            sum += c;
+        }
+        block_add(E.totals + 3, sum);
+        grid.sync();
+    }
+    finish(true);
+}
+
+// acb_count_rows: the same successors and pointer jumping over the rows of ONE haystack (int64, as
+// acb_select_non_overlapping reads them), pairs in scratch (16 bytes per row).  Cooperative, one launch.
+__global__ void __launch_bounds__(kScanThreads) count_rows_kernel(const long long *rows, unsigned long long n, int mode, int longest,
+                                                                 long long max_len, uint4 *pairs, unsigned long long *count) {
+    namespace cg = cooperative_groups;
+    cg::grid_group grid = cg::this_grid();
+    const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+    const unsigned long long first_i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    for (unsigned long long i = first_i; i < n; i += stride) {
+        const long long s = rows[4 * i + 3];
+        const unsigned long long nx = mode == kModeStandard ? next_selected<kModeStandard>(rows, n, s, max_len, longest)
+                                                            : next_selected<kModeLeftmost>(rows, n, s, max_len, longest);
+        reinterpret_cast<uint2 *>(pairs + i)[0] = make_uint2(nx == n ? kNoNext : (uint32_t)nx, 1u);
+    }
+    grid.sync();
+    const uint32_t rounds = ceil_log2(n);
+    for (uint32_t r = 0; r < rounds; r++) {
+        for (unsigned long long i = first_i; i < n; i += stride) jump_pair(pairs, i, (int)(r & 1));
+        grid.sync();
+    }
+    if (first_i == 0) {
+        const unsigned long long head = mode == kModeStandard ? next_selected<kModeStandard>(rows, n, 0, max_len, longest)
+                                                              : next_selected<kModeLeftmost>(rows, n, 0, max_len, longest);
+        const uint4 p = pairs[head];
+        *count = (rounds & 1) ? p.w : p.y;
     }
 }
 
@@ -1317,6 +1551,23 @@ int launch_sieve_epilogue(SieveEpiArgs &E, const DeviceInfo &d, cudaStream_t st)
     return ACB_OK;
 }
 
+// a cooperative launch of the count kernels: every block resident at once (at most 4 per SM, as the epilogues)
+int launch_cooperative(const void *kern, void **args, const DeviceInfo &d, cudaStream_t st) {
+    int bps = 0;
+    CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, kern, kScanThreads, 0));
+    if (bps < 1) return fail(ACB_ECUDA, "count kernel does not fit on an SM");
+    if (bps > 4) bps = 4;
+    CUDA_OK(cudaLaunchCooperativeKernel(kern, dim3(d.sms * bps), dim3(kScanThreads), args, 0, st));
+    g_launches++;
+    return ACB_OK;
+}
+
+template <int MODE>
+int launch_sieve_count_epilogue(SieveEpiArgs &E, unsigned long long *counts, const DeviceInfo &d, cudaStream_t st) {
+    void *args[] = {&E, &counts};
+    return launch_cooperative(reinterpret_cast<const void *>(sieve_count_epilogue_kernel<MODE>), args, d, st);
+}
+
 int sieve_header(const acb_automaton *a, SieveHeader &sh) {
     std::lock_guard<std::mutex> lock(a->impl->sieve_mutex);
     if (a->impl->sieve.size() < sizeof(SieveHeader)) return fail(ACB_EINVAL, "acb_sieve_build has not been called");
@@ -1324,13 +1575,20 @@ int sieve_header(const acb_automaton *a, SieveHeader &sh) {
     return ACB_OK;
 }
 
-// acb_any_match (mode kSieveAny, out = u8 flags) and acb_find_first (kSieveFirst + kind, out = u64 keys): one launch of
-// the sieve kernel in a mode that writes no list and stops early
+int unsupported_overlapping(const acb_automaton *a) {
+    const int kind = (int)a->impl->hdr.match_kind;
+    return fail(ACB_EUNSUPPORTED, std::string("match kind ") + (kind == ACB_LEFTMOST_FIRST ? "LeftmostFirst" : "LeftmostLongest") +
+                                      " does not support overlapping searches");
+}
+
+// acb_any_match (mode kSieveAny, out = u8 flags), acb_find_first (kSieveFirst + kind, out = u64 keys) and
+// acb_count_overlapping (kSieveCount, out = u64 counts): one launch of the sieve kernel in a mode that writes no list
 int sieve_early_scan(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
                      int64_t n_haystacks, uint64_t total_bytes, void *dev_out, uint64_t *dev_scratch, void *stream, int mode) {
     if (!a || !dev_sieve || !dev_offsets || !dev_out || !dev_scratch || (total_bytes && !dev_bytes)) return fail(ACB_EINVAL, "null argument");
     if (n_haystacks < 0 || n_haystacks > 0xfffffffell) return fail(ACB_EINVAL, "n_haystacks out of range (0 .. 2^32 - 2)");
     if (total_bytes >= (1ull << 31)) return fail(ACB_EINVAL, "total_bytes must be below 2^31 (scan larger inputs in windows)");
+    if (mode == kSieveCount && a->impl->hdr.match_kind != ACB_STANDARD) return unsupported_overlapping(a);
     SieveHeader sh;
     if (int rc = sieve_header(a, sh)) return rc;
     DeviceInfo d;
@@ -1359,6 +1617,7 @@ int sieve_early_scan(const acb_automaton *a, const void *dev_sieve, const uint8_
         case kSieveFirst + ACB_STANDARD: rc = launch_sieve<false, kSieveFirst + ACB_STANDARD>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
         case kSieveFirst + ACB_LEFTMOST_FIRST: rc = launch_sieve<false, kSieveFirst + ACB_LEFTMOST_FIRST>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
         case kSieveFirst + ACB_LEFTMOST_LONGEST: rc = launch_sieve<false, kSieveFirst + ACB_LEFTMOST_LONGEST>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
+        case kSieveCount: rc = launch_sieve<false, kSieveCount>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
         default: return fail(ACB_EINVAL, "unknown match kind");
     }
     if (rc) return rc;
@@ -1371,6 +1630,105 @@ int check_ws(const acb_workspace *ws) {
         !ws->dev_unit_offsets || !ws->dev_seg_info || !ws->dev_scratch || !ws->dev_total || !ws->dev_out ||
         !ws->dev_match_offsets)
         return fail(ACB_EINVAL, "workspace has a null buffer");
+    return ACB_OK;
+}
+
+// The sieve's list scan: the scan kernel, then the ordering epilogue -- acb_scan_batch's kernel 5 (counts == null:
+// the list, or its selection, in dev_out) or acb_count_non_overlapping (counts: the count epilogue writes them; the raw
+// records go to dev_raw and are ordered into dev_out, so that dev_raw is free for the count's pairs).
+int sieve_list_scan(const acb_automaton *a, const void *dev_sieve, const Batch &B, uint64_t total_bytes, int mode, bool cp,
+                    const uint32_t *pat_cplen, const acb_plan *plan, const acb_workspace *ws, const DeviceInfo &d, cudaStream_t st,
+                    unsigned long long *counts) {
+    const ImageHeader &h = a->impl->hdr;
+    const int kind = (int)h.match_kind;
+    const uint8_t *dev_bytes = B.bytes;
+    const int64_t n_haystacks = B.n_haystacks;
+    int rc;
+    unsigned long long *totals = reinterpret_cast<unsigned long long *>(ws->dev_total);
+    unsigned int *task_counter = reinterpret_cast<unsigned int *>(ws->dev_scratch);
+    unsigned long long *acc = reinterpret_cast<unsigned long long *>(ws->dev_scratch);  // zero between scans (see kAcc*)
+    unsigned long long *unit_offsets = reinterpret_cast<unsigned long long *>(ws->dev_unit_offsets);
+    unsigned long long *match_offsets = reinterpret_cast<unsigned long long *>(ws->dev_match_offsets);
+    Sink out;
+    out.raw_seq = ws->dev_raw_seq;
+    out.raw_unit = ws->dev_raw_unit;
+    out.raw_aux = ws->dev_raw_aux;
+    out.unit_counts = ws->dev_unit_counts;
+    out.raw_total = acc + kAccRaw;
+    SieveHeader sh;
+    if ((rc = sieve_header(a, sh))) return rc;
+    const DevSieve sv = make_sieve_view(sh, dev_sieve);
+    SievePlan SP;
+    SP.origin = -(int64_t)(reinterpret_cast<uintptr_t>(dev_bytes) & 511u);
+    SP.task_bytes = plan->task_bytes;
+    SP.n_tasks = (int64_t)((total_bytes + (uint64_t)(-SP.origin) + plan->task_bytes - 1) / plan->task_bytes);
+    SP.buf_bytes = total_bytes;
+    SP.avg_len = total_bytes / (uint64_t)n_haystacks;
+    if (SP.avg_len < 1) SP.avg_len = 1;
+    const uint64_t cap = ws->raw_capacity < ws->out_capacity ? ws->raw_capacity : ws->out_capacity;
+    // scratch: counters | unit tile sums | cont tile sums | cont_cum | cont tails (u32)
+    const uint64_t tiles_max = (plan->n_units + kScanTile - 1) / kScanTile;
+    unsigned long long *tile_sums = acc + kAccWords;
+    unsigned long long *cont_tiles = tile_sums + tiles_max + 1;
+    unsigned long long *cont_cum = cont_tiles + tiles_max + 1;
+    const uint64_t per_piece = plan->n_segments > (uint64_t)SP.n_tasks ? plan->n_segments : (uint64_t)SP.n_tasks;
+    uint32_t *cont_tail = reinterpret_cast<uint32_t *>(cont_cum + per_piece + 2);
+    // a non-overlapping search orders the list into dev_raw's place and packs its selection into dev_out, so its
+    // raw records go through dev_out first (a count packs nothing: dev_raw -> dev_out)
+    const bool in_raw = mode == kModeOverlap || counts;
+    out.raw = in_raw ? ws->dev_raw : ws->dev_out;
+    out.cap = cap;
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    if (g_timing) {
+        CUDA_OK(cudaEventCreate(&e0));
+        CUDA_OK(cudaEventCreate(&e1));
+        CUDA_OK(cudaEventRecord(e0, st));
+    }
+    // code points: the continuation bytes each task saw before a haystack that starts in it, per haystack; lives in
+    // the match_offsets buffer until the epilogue's last phases write the offsets there
+    uint32_t *hay_cont = reinterpret_cast<uint32_t *>(match_offsets);
+    rc = cp ? launch_sieve<true>(sv, B, SP, out, cont_tail, hay_cont, task_counter, d, st)
+            : launch_sieve<false>(sv, B, SP, out, cont_tail, hay_cont, task_counter, d, st);
+    if (rc) return rc;
+    CUDA_OK(cudaGetLastError());
+    if (e1) {
+        CUDA_OK(cudaEventRecord(e1, st));
+        g_timing_events.emplace_back(e0, e1);
+    }
+    SieveEpiArgs E;
+    E.B = B;
+    E.unit_counts = ws->dev_unit_counts;
+    E.n_tasks = (uint64_t)SP.n_tasks;
+    E.tile_sums = tile_sums;
+    E.unit_offsets = unit_offsets;
+    E.cont_tail = cont_tail;
+    E.hay_cont = hay_cont;
+    E.cont_tiles = cont_tiles;
+    E.cont_cum = cont_cum;
+    E.raw = out.raw;
+    E.raw_seq = ws->dev_raw_seq;
+    E.raw_unit = ws->dev_raw_unit;
+    E.raw_aux = ws->dev_raw_aux;
+    E.raw_cap = cap;
+    E.ordered = in_raw ? ws->dev_out : ws->dev_raw;
+    E.final_out = ws->dev_out;
+    E.out_cap = cap;
+    E.pat_cplen = pat_cplen;
+    E.origin = SP.origin;
+    E.task_bytes = SP.task_bytes;
+    E.max_pat_len = h.max_pat_len;
+    E.longest = kind == ACB_LEFTMOST_LONGEST ? 1 : 0;
+    E.totals = totals;
+    E.acc = acc;
+    E.match_offsets = match_offsets;
+    if (counts)
+        rc = mode == kModeStandard ? launch_sieve_count_epilogue<kModeStandard>(E, counts, d, st) : launch_sieve_count_epilogue<kModeLeftmost>(E, counts, d, st);
+    else
+        rc = mode == kModeStandard   ? (cp ? launch_sieve_epilogue<kModeStandard, true>(E, d, st) : launch_sieve_epilogue<kModeStandard, false>(E, d, st))
+             : mode == kModeLeftmost ? (cp ? launch_sieve_epilogue<kModeLeftmost, true>(E, d, st) : launch_sieve_epilogue<kModeLeftmost, false>(E, d, st))
+                                     : (cp ? launch_sieve_epilogue<kModeOverlap, true>(E, d, st) : launch_sieve_epilogue<kModeOverlap, false>(E, d, st));
+    if (rc) return rc;
+    CUDA_OK(cudaGetLastError());
     return ACB_OK;
 }
 
@@ -1422,6 +1780,68 @@ int acb_find_first(const acb_automaton *a, const void *dev_sieve, const uint8_t 
     if (!a) return fail(ACB_EINVAL, "null argument");
     return sieve_early_scan(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, dev_keys, dev_scratch, stream,
                             kSieveFirst + (int)a->impl->hdr.match_kind);
+}
+
+int acb_count_overlapping(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                          int64_t n_haystacks, uint64_t total_bytes, uint64_t *dev_counts, uint64_t *dev_scratch, void *stream) {
+    if (!dev_counts) return fail(ACB_EINVAL, "null argument");
+    return sieve_early_scan(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, dev_counts, dev_scratch, stream, kSieveCount);
+}
+
+int acb_count_non_overlapping(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                              int64_t n_haystacks, uint64_t total_bytes, const acb_plan *plan, const acb_workspace *ws,
+                              uint64_t *dev_counts, void *stream) {
+    if (!a || !dev_sieve || !dev_offsets || !plan || !dev_counts || (total_bytes && !dev_bytes)) return fail(ACB_EINVAL, "null argument");
+    if (int rc = check_ws(ws)) return rc;
+    if (n_haystacks < 0 || n_haystacks > 0xfffffffell) return fail(ACB_EINVAL, "n_haystacks out of range (0 .. 2^32 - 2)");
+    if (total_bytes >= (1ull << 31)) return fail(ACB_EINVAL, "total_bytes must be below 2^31 (scan larger inputs in windows)");
+    acb_plan want;
+    acb_plan_scan(a, dev_bytes, total_bytes, (uint64_t)n_haystacks, &want);
+    if (want.n_segments != plan->n_segments || want.segment_bytes != plan->segment_bytes || want.n_units != plan->n_units ||
+        want.task_bytes != plan->task_bytes)
+        return fail(ACB_EINVAL, "plan does not match the arguments (call acb_plan_scan again)");
+    SieveHeader sh;
+    if (int rc = sieve_header(a, sh)) return rc;
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (n_haystacks == 0 || total_bytes == 0) {
+        if (n_haystacks) CUDA_OK(cudaMemsetAsync(dev_counts, 0, (uint64_t)n_haystacks * sizeof(uint64_t), st));
+        zero_outputs_kernel<<<(unsigned)((n_haystacks + 256) / 256), 256, 0, st>>>(
+            reinterpret_cast<unsigned long long *>(ws->dev_unit_offsets), reinterpret_cast<unsigned long long *>(ws->dev_match_offsets),
+            n_haystacks, reinterpret_cast<unsigned long long *>(ws->dev_total));
+        g_launches++;
+        CUDA_OK(cudaGetLastError());
+        return ACB_OK;
+    }
+    const int mode = a->impl->hdr.match_kind == ACB_STANDARD ? kModeStandard : kModeLeftmost;
+    return sieve_list_scan(a, dev_sieve, Batch{dev_bytes, dev_offsets, n_haystacks}, total_bytes, mode, false, nullptr, plan, ws, d, st,
+                           reinterpret_cast<unsigned long long *>(dev_counts));
+}
+
+int acb_count_rows(const acb_automaton *a, const int64_t *dev_rows, uint64_t n_rows, uint64_t *dev_scratch, uint64_t *dev_count,
+                   void *stream) {
+    if (!a || !dev_count || (n_rows && (!dev_rows || !dev_scratch))) return fail(ACB_EINVAL, "null argument");
+    if (n_rows >= 0xffffffffull) return fail(ACB_EINVAL, "n_rows out of range (0 .. 2^32 - 2)");
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (n_rows == 0) {
+        CUDA_OK(cudaMemsetAsync(dev_count, 0, sizeof(uint64_t), st));
+        return ACB_OK;
+    }
+    const ImageHeader &h = a->impl->hdr;
+    const long long *rows = reinterpret_cast<const long long *>(dev_rows);
+    unsigned long long n = n_rows;
+    int mode = h.match_kind == ACB_STANDARD ? kModeStandard : kModeLeftmost;
+    int longest = h.match_kind == ACB_LEFTMOST_LONGEST ? 1 : 0;
+    long long max_len = (long long)h.max_pat_len;
+    uint4 *pairs = reinterpret_cast<uint4 *>(dev_scratch);
+    unsigned long long *count = reinterpret_cast<unsigned long long *>(dev_count);
+    void *args[] = {&rows, &n, &mode, &longest, &max_len, &pairs, &count};
+    if (int rc = launch_cooperative(reinterpret_cast<const void *>(count_rows_kernel), args, d, st)) return rc;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
 }
 
 int acb_first_rows(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
@@ -1539,85 +1959,7 @@ int acb_scan_batch(const acb_automaton *a, const void *dev_image, const void *de
     if (kernel == 2 && g_tuning.kernel == 0 && hot_desc && (hot_desc->reserved & 1u)) kernel = 4;
     if (kernel == 5 && !dev_sieve) return fail(ACB_EINVAL, "the sieve kernel needs a sieve image (acb_sieve_build / acb_sieve_write)");
     if ((!dev_hot || !hot_desc) && kernel != 4 && kernel != 5) kernel = 1;  // no hot image: the plain kernel (one thread per haystack)
-    if (kernel == 5) {
-        // ---- position-parallel scan: filter + exact verification, then order (+ select) ----
-        const Automaton &A = *a->impl;
-        SieveHeader sh;
-        {
-            std::lock_guard<std::mutex> lock(a->impl->sieve_mutex);
-            if (A.sieve.size() < sizeof(SieveHeader)) return fail(ACB_EINVAL, "acb_sieve_build has not been called");
-            std::memcpy(&sh, A.sieve.data(), sizeof(sh));
-        }
-        const DevSieve sv = make_sieve_view(sh, dev_sieve);
-        SievePlan SP;
-        SP.origin = -(int64_t)(reinterpret_cast<uintptr_t>(dev_bytes) & 511u);
-        SP.task_bytes = plan->task_bytes;
-        SP.n_tasks = (int64_t)((total_bytes + (uint64_t)(-SP.origin) + plan->task_bytes - 1) / plan->task_bytes);
-        SP.buf_bytes = total_bytes;
-        SP.avg_len = total_bytes / (uint64_t)n_haystacks;
-        if (SP.avg_len < 1) SP.avg_len = 1;
-        const uint64_t cap = ws->raw_capacity < ws->out_capacity ? ws->raw_capacity : ws->out_capacity;
-        // scratch: counters | unit tile sums | cont tile sums | cont_cum | cont tails (u32)
-        const uint64_t tiles_max = (plan->n_units + kScanTile - 1) / kScanTile;
-        unsigned long long *tile_sums = acc + kAccWords;
-        unsigned long long *cont_tiles = tile_sums + tiles_max + 1;
-        unsigned long long *cont_cum = cont_tiles + tiles_max + 1;
-        const uint64_t per_piece = plan->n_segments > (uint64_t)SP.n_tasks ? plan->n_segments : (uint64_t)SP.n_tasks;
-        uint32_t *cont_tail = reinterpret_cast<uint32_t *>(cont_cum + per_piece + 2);
-        // a non-overlapping search orders the list into dev_raw's place and packs its selection into dev_out, so its
-        // raw records go through dev_out first
-        out.raw = mode == kModeOverlap ? ws->dev_raw : ws->dev_out;
-        out.cap = cap;
-        cudaEvent_t e0 = nullptr, e1 = nullptr;
-        if (g_timing) {
-            CUDA_OK(cudaEventCreate(&e0));
-            CUDA_OK(cudaEventCreate(&e1));
-            CUDA_OK(cudaEventRecord(e0, st));
-        }
-        // code points: the continuation bytes each task saw before a haystack that starts in it, per haystack; lives in
-        // the match_offsets buffer until the epilogue's last phases write the offsets there
-        uint32_t *hay_cont = reinterpret_cast<uint32_t *>(match_offsets);
-        rc = cp ? launch_sieve<true>(sv, B, SP, out, cont_tail, hay_cont, task_counter, d, st)
-                : launch_sieve<false>(sv, B, SP, out, cont_tail, hay_cont, task_counter, d, st);
-        if (rc) return rc;
-        CUDA_OK(cudaGetLastError());
-        if (e1) {
-            CUDA_OK(cudaEventRecord(e1, st));
-            g_timing_events.emplace_back(e0, e1);
-        }
-        SieveEpiArgs E;
-        E.B = B;
-        E.unit_counts = ws->dev_unit_counts;
-        E.n_tasks = (uint64_t)SP.n_tasks;
-        E.tile_sums = tile_sums;
-        E.unit_offsets = unit_offsets;
-        E.cont_tail = cont_tail;
-        E.hay_cont = hay_cont;
-        E.cont_tiles = cont_tiles;
-        E.cont_cum = cont_cum;
-        E.raw = out.raw;
-        E.raw_seq = ws->dev_raw_seq;
-        E.raw_unit = ws->dev_raw_unit;
-        E.raw_aux = ws->dev_raw_aux;
-        E.raw_cap = cap;
-        E.ordered = mode == kModeOverlap ? ws->dev_out : ws->dev_raw;
-        E.final_out = ws->dev_out;
-        E.out_cap = cap;
-        E.pat_cplen = im.pat_cplen;
-        E.origin = SP.origin;
-        E.task_bytes = SP.task_bytes;
-        E.max_pat_len = h.max_pat_len;
-        E.longest = kind == ACB_LEFTMOST_LONGEST ? 1 : 0;
-        E.totals = totals;
-        E.acc = acc;
-        E.match_offsets = match_offsets;
-        rc = mode == kModeStandard   ? (cp ? launch_sieve_epilogue<kModeStandard, true>(E, d, st) : launch_sieve_epilogue<kModeStandard, false>(E, d, st))
-             : mode == kModeLeftmost ? (cp ? launch_sieve_epilogue<kModeLeftmost, true>(E, d, st) : launch_sieve_epilogue<kModeLeftmost, false>(E, d, st))
-                                     : (cp ? launch_sieve_epilogue<kModeOverlap, true>(E, d, st) : launch_sieve_epilogue<kModeOverlap, false>(E, d, st));
-        if (rc) return rc;
-        CUDA_OK(cudaGetLastError());
-        return ACB_OK;
-    }
+    if (kernel == 5) return sieve_list_scan(a, dev_sieve, B, total_bytes, mode, cp, im.pat_cplen, plan, ws, d, st, nullptr);
     const bool segments = kernel == 2 || kernel == 3 || kernel == 4;
     const int per_lane = kernel == 3 ? 2 : 1;  // segments per lane of the staged kernel (3: two interleaved chains)
     SegPlan P{};

@@ -55,6 +55,12 @@
 // key whose primary is below that bound.  The any-match skips apply with "flag set" read as "cannot beat the key"
 // (strictly: an equal primary may still win on the low word); the tail haystack's key is loaded, high word only, one
 // window ahead as its flag is.
+//
+// COUNT (acb_count_overlapping): the answer is each haystack's number of overlapping matches, one u64 counter per
+// haystack.  Stage 2 takes the deepest terminal node's chain_cnt -- every pattern ending at the position -- as the list
+// mode does, and instead of reserving and writing records adds it to the haystack's counter: lanes of one round that
+// share a haystack (most of them) are summed first, and one lane per distinct haystack adds.  Every position counts, so
+// nothing is skipped.
 #pragma once
 #include "scan_staged.cuh"
 #include "sieve.h"
@@ -144,6 +150,7 @@ __device__ __forceinline__ uint32_t ld_key_hi(const unsigned long long *p) {
 constexpr int kSieveList = 0;   // the overlapping match list (acb_scan_batch)
 constexpr int kSieveAny = 1;    // one flag per haystack (acb_any_match)
 constexpr int kSieveFirst = 2;  // one first-match key per haystack (acb_find_first): kSieveFirst + the match kind (ACB_*)
+constexpr int kSieveCount = 5;  // one overlapping match count per haystack (acb_count_overlapping)
 
 // continuation bytes among the first nbytes (0..16) of the 16-byte chunk at shared address a
 __device__ __forceinline__ uint32_t cont_prefix(uint32_t a, uint32_t nbytes) {
@@ -173,18 +180,20 @@ __device__ __forceinline__ uint32_t warp_excl_scan(uint32_t v, uint32_t lane, ui
 //
 // Positions inside a task are 32-bit offsets from the task's start (`rel`); the 64-bit stream position is t_lo + rel.
 //
-// MODE kSieveAny and kSieveFirst + kind (CP = false only): `out` is unused, and the two code-point pointers carry the
-// mode's outputs instead (so the list-mode instantiations keep their parameter block): hay_cont -> flags =
-// u8[n_haystacks] (any) or keys = u64[n_haystacks] (first), task_cont -> skipped = u64[2] = [tasks skipped whole,
-// windows not scanned] (see acb_any_match, acb_find_first).
+// MODE kSieveAny, kSieveFirst + kind and kSieveCount (CP = false only): `out` is unused, and the two code-point
+// pointers carry the mode's outputs instead (so the list-mode instantiations keep their parameter block): hay_cont ->
+// flags = u8[n_haystacks] (any), keys = u64[n_haystacks] (first) or counts = u64[n_haystacks] (count), task_cont ->
+// skipped = u64[2] = [tasks skipped whole, windows not scanned] (see acb_any_match, acb_find_first; count: unused).
 template <bool CP, int WC, int MODE = kSieveList>
 __global__ void __launch_bounds__(kSieveThreads, 1)
 sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_cont, uint32_t *hay_cont, unsigned int *task_counter) {
-    constexpr bool ANY = MODE == kSieveAny, FIRST = MODE >= kSieveFirst, EARLY = ANY || FIRST;  // EARLY: no list, work stops early
+    constexpr bool ANY = MODE == kSieveAny, FIRST = MODE >= kSieveFirst && MODE < kSieveCount, EARLY = ANY || FIRST;  // EARLY: no list, work stops early
+    constexpr bool COUNT = MODE == kSieveCount, LIST = MODE == kSieveList;
     constexpr int KIND = MODE - kSieveFirst;  // (FIRST)
-    static_assert(!(EARLY && CP), "the any-match and first-match modes have no positions to count");
+    static_assert(!(!LIST && CP), "the any-match, first-match and count modes have no positions to count");
     uint8_t *const flags = reinterpret_cast<uint8_t *>(hay_cont);
     unsigned long long *const keys = reinterpret_cast<unsigned long long *>(hay_cont);
+    unsigned long long *const counts = reinterpret_cast<unsigned long long *>(hay_cont);
     unsigned long long *const skipped = reinterpret_cast<unsigned long long *>(task_cont);
     extern __shared__ __align__(128) uint8_t smem[];
     const uint32_t bloom_s = (uint32_t)__cvta_generic_to_shared(smem);
@@ -259,7 +268,7 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
         if (lane == 0) claimed = atomicAdd(task_counter, 1u);  // the next one: its round trip overlaps this task
         const int64_t t_lo = P.origin + (int64_t)task * T;
         if (t_lo >= vhi || t_lo + (int64_t)T <= vlo) {
-            if (lane == 0 && !EARLY) {
+            if (lane == 0 && LIST) {
                 out.unit_counts[task] = 0;
                 if (CP) task_cont[task] = 0;
             }
@@ -454,7 +463,14 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
                 }
             }
             const uint32_t hits = EARLY ? 0u : __ballot_sync(0xffffffffu, cnt != 0);
-            if (hits) {
+            if (COUNT) {
+                if (cnt) {
+                    // one add per distinct haystack of the round: lanes of one round mostly share a haystack
+                    const uint32_t peers = __match_any_sync(hits, (uint32_t)h);  // (haystack ids fit 32 bits)
+                    const uint32_t sum = __reduce_add_sync(peers, cnt);          // (at most 32 chain counts)
+                    if (lane == (uint32_t)__ffs(peers) - 1u) atomicAdd(counts + (uint32_t)h, (unsigned long long)sum);
+                }
+            } else if (hits) {
                 uint32_t total;
                 const uint32_t exc = warp_excl_scan(cnt, lane, &total);
                 unsigned long long rbase = 0;
@@ -707,7 +723,7 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
             carry_w = __shfl_sync(0xffffffffu, cur.w, 31);
             cur = nxt;
         }
-        if (lane == 0 && !EARLY) out.unit_counts[task] = n_emitted;
+        if (lane == 0 && LIST) out.unit_counts[task] = n_emitted;
         if (CP && lane == 0) task_cont[task] = cp_before;
         __syncwarp();
     }

@@ -12,7 +12,8 @@ call): ``find_matches_as_indexes_batch`` and ``scan_device`` for batches that
 are already device resident; ``is_match`` / ``is_match_batch`` /
 ``is_match_device``, the crate's ``AhoCorasick::is_match`` per haystack;
 ``find_first`` / ``find_first_batch`` / ``find_first_device``, the crate's
-``AhoCorasick::find`` per haystack.
+``AhoCorasick::find`` per haystack; ``count_matches`` / ``count_matches_batch`` /
+``count_matches_device``, the length of each haystack's match list without the list.
 """
 from __future__ import annotations
 
@@ -646,6 +647,158 @@ class _Automaton:
             mask = self.any_device(d[head:], d[:8 * (n + 1)].view(torch.int64))
             return mask.cpu().tolist()
 
+    # ---- match counts per haystack: len(find_matches_as_indexes(h, overlapping)) without the list ----------------
+    def count_device(self, data, offsets, overlapping=False, capacity: Optional[int] = None):
+        """How many matches each haystack of a device-resident batch has -> int64 CUDA tensor (n,): the length of
+        its list in scan_device, for every match kind.  Counts are the same in bytes and in code points, so no code
+        point work is ever done.  An overlapping search on a leftmost automaton raises ValueError, as scan_device does.
+
+        Where the engine rule of scan_device picks the sieve: an overlapping count is the sieve kernel's count mode
+        (acb_count_overlapping: no list, no epilogue) and returns without waiting for the device; a non-overlapping
+        count is the sieve's list scan and a count epilogue (acb_count_non_overlapping: the selection is counted, not
+        packed; long per-haystack lists are counted by the whole grid), which waits for the device and scans again with
+        more room when the list did not fit the workspace, as scan_device does.  Where the rule picks a table walker,
+        the counts are diff(match_offsets) of its full scan, which waits for it; the next scan that reuses the
+        workspace waits for that difference.  `capacity`: the workspace's first size, in records, as for scan_device."""
+        self.check_overlapping(overlapping)
+        torch = _require_cuda()
+        dev = data.device
+        n = offsets.numel() - 1
+        if n <= 0 or data.numel() == 0:
+            return torch.zeros(max(n, 0), dtype=torch.int64, device=dev)
+        if data.numel() > self.WINDOW_BYTES:
+            return self._count_device_windows(data, offsets, overlapping)
+        with self._lock, torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev)
+            if self._pick_engine(dev, data, offsets, overlapping) is not None:
+                _, mo, _ = self.scan_device(data, offsets, overlapping, False)
+                counts = mo[1:] - mo[:-1]
+                reader = torch.cuda.Event()
+                reader.record(stream)
+                self._ws[(dev.index if dev.index is not None else torch.cuda.current_device(), 0)]["reader"] = reader
+                self.last_stats = {"engine": self.last_stats.get("engine", "table"), "mode": "count", "long_stretches": 0}
+                return counts
+            sieve_t, _ = self.sieve(dev)
+            counts = torch.zeros(n, dtype=torch.int64, device=dev)
+            if overlapping:
+                scratch = torch.empty(3, dtype=torch.int64, device=dev)
+                rc = self._L.acb_count_overlapping(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
+                                                   counts.data_ptr(), scratch.data_ptr(), stream.cuda_stream)
+                if rc != _capi.ACB_OK:
+                    raise RuntimeError(_capi.last_error())
+                self.last_stats = {"engine": "sieve", "mode": "count", "long_stretches": 0}
+                return counts
+            plan = self._plan(data, n)
+            cap = capacity or max(1024, n * 2)
+            while True:
+                ws = self._workspace(dev, plan, n, cap, 0)
+                reader = ws.pop("reader", None)
+                if reader is not None:   # a comparison of an earlier call (maybe on another stream) reads this workspace first
+                    stream.wait_event(reader)
+                st = self._ws_struct(ws)
+                rc = self._L.acb_count_non_overlapping(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
+                                                       C.byref(plan), C.byref(st), counts.data_ptr(), stream.cuda_stream)
+                if rc != _capi.ACB_OK:
+                    err = _capi.last_error()
+                    ws["scratch"][:8].zero_()   # a scan that failed half way may have left its counters dirty
+                    raise RuntimeError(err)
+                tot = ws["total"].tolist()
+                total, complete, long_stretches, raw_total = tot[0], tot[1], tot[2], tot[4]
+                if complete or (total == 0 and raw_total == 0):
+                    break
+                cap = max(total, raw_total) + max(total, raw_total) // 8 + 16
+            self.last_stats = {"engine": "sieve", "mode": "count", "task_bytes": plan.task_bytes, "list_records": raw_total,
+                               "long_stretches": long_stretches}
+            return counts
+
+    def _count_device_windows(self, data, offsets, overlapping):
+        """count_device for buffers above WINDOW_BYTES: runs of whole haystacks that fit one call each get their slice
+        of the counts; one haystack above the limit goes to _count_one_large.  last_stats["long_stretches"] sums the
+        runs'."""
+        torch = _require_cuda()
+        dev = data.device
+        n = offsets.numel() - 1
+        limit = self.WINDOW_BYTES
+        counts = torch.zeros(n, dtype=torch.int64, device=dev)
+        lens = offsets[1:] - offsets[:-1]
+        oversized = bool((lens > limit).any().item())
+        long_stretches = 0
+        h = 0
+        while h < n:
+            start = int(offsets[h].item())
+            if oversized and int(lens[h].item()) > limit:
+                counts[h:h + 1] = self._count_one_large(data[start:start + int(lens[h].item())], overlapping)
+                h += 1
+                continue
+            # the longest run of whole haystacks that fits one call (and stops before an oversized one)
+            h1 = int(torch.searchsorted(offsets, torch.tensor([start + limit], dtype=torch.int64, device=dev), right=True).item()) - 1
+            h1 = max(h + 1, min(h1, n))
+            if oversized:
+                big = torch.nonzero(lens[h:h1] > limit)
+                if big.numel():
+                    h1 = h + int(big[0].item())
+            end = int(offsets[h1].item())
+            counts[h:h1] = self.count_device(data[start:end], offsets[h:h1 + 1] - start, overlapping)
+            long_stretches += self.last_stats.get("long_stretches", 0)
+            h = h1
+        torch.cuda.current_stream(dev).synchronize()
+        self.last_stats = {"engine": self.last_stats.get("engine"), "mode": "count", "long_stretches": long_stretches, "windows": True}
+        return counts
+
+    def _count_one_large(self, hay, overlapping):
+        """The count (an int64 CUDA tensor (1,)) of one haystack above WINDOW_BYTES.
+        Overlapping: windows that share max_pattern_len - 1 bytes (the head of each window but the first).  A window
+        counts every match inside it; a match that lies wholly inside a window's head was counted by the window before,
+        so the count of the head alone is subtracted.  Every other match ends past a head and starts inside its window.
+        Non-overlapping: the overlapping rows of the windows, and acb_count_rows counts what the selection would pick."""
+        torch = _require_cuda()
+        dev = hay.device
+        if overlapping:
+            limit, halo = self.WINDOW_BYTES, max(self.max_pattern_len - 1, 0)
+            total = torch.zeros(1, dtype=torch.int64, device=dev)
+            w0 = 0
+            while True:
+                w1 = min(w0 + limit, hay.numel())
+                total += self.count_device(hay[w0:w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=dev), True)
+                if w0 and halo:
+                    total -= self.count_device(hay[w0:w0 + halo], torch.tensor([0, halo], dtype=torch.int64, device=dev), True)
+                if w1 == hay.numel():
+                    return total
+                w0 += limit - halo
+        rows = self._overlapping_rows_large(hay, False).contiguous()
+        count = torch.zeros(1, dtype=torch.int64, device=dev)
+        if rows.shape[0]:
+            scratch = torch.empty((rows.shape[0], 2), dtype=torch.int64, device=dev)   # 16 bytes per row
+            rc = self._L.acb_count_rows(self._h, rows.data_ptr(), rows.shape[0], scratch.data_ptr(), count.data_ptr(),
+                                        torch.cuda.current_stream(dev).cuda_stream)
+            if rc != _capi.ACB_OK:
+                raise RuntimeError(_capi.last_error())
+        return count
+
+    def count_host_batch(self, chunks: Sequence[bytes], overlapping):
+        """Host buffers (bytes-like objects, one per haystack) -> list of int: each one's match count.  The offsets and
+        the haystacks are gathered into the pinned staging buffer and go to the device in one copy."""
+        torch = _require_cuda()
+        self.check_overlapping(overlapping)
+        n = len(chunks)
+        if n == 0:
+            return []
+        offs = np.zeros(n + 1, dtype=np.int64)
+        np.cumsum(np.fromiter((len(c) for c in chunks), dtype=np.int64, count=n), out=offs[1:])
+        total_bytes = int(offs[-1])
+        head = (8 * (n + 1) + 511) & ~511   # the offsets, then the bytes at a 512-byte boundary of the buffer
+        dev = torch.device("cuda", torch.cuda.current_device())
+        with self._host_lock:
+            host = self._pinned(head + total_bytes)
+            hv = host.numpy()
+            hv[:8 * (n + 1)].view(np.int64)[:] = offs
+            if n == 1:
+                hv[head:head + total_bytes] = np.frombuffer(chunks[0], dtype=np.uint8)
+            elif total_bytes:
+                hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
+            d = host[:head + total_bytes].to(dev, non_blocking=True)
+            return self.count_device(d[head:], d[:8 * (n + 1)].view(torch.int64), overlapping).cpu().tolist()
+
     def scan_device(self, data, offsets, overlapping=False, codepoints=False, capacity: Optional[int] = None,
                     sync: bool = True, ws_slot: int = 0):
         """Scan a device-resident batch.  data: uint8 CUDA tensor, offsets: int64
@@ -775,14 +928,7 @@ class _Automaton:
         overlapping list afterwards (acb_select_non_overlapping; SURVEY.md 8c), for all three match kinds."""
         torch = _require_cuda()
         dev = hay.device
-
-        def scan_window(window):
-            one = torch.tensor([0, window.numel()], dtype=torch.int64, device=dev)
-            m, _, _ = self._scan_overlapping_list(window, one, codepoints)
-            return m.to(torch.int64)
-
-        parts = scan_in_windows(scan_window, hay, self.WINDOW_BYTES, max(self.max_pattern_len - 1, 0), codepoints)
-        rows = torch.cat(parts, dim=0) if parts else torch.zeros((0, 4), dtype=torch.int64, device=dev)
+        rows = self._overlapping_rows_large(hay, codepoints)
         if overlapping or rows.shape[0] == 0:
             return rows
         rows = rows.contiguous()
@@ -793,6 +939,20 @@ class _Automaton:
         if rc != _capi.ACB_OK:
             raise RuntimeError(_capi.last_error())
         return out[: int(count.item())]
+
+    def _overlapping_rows_large(self, hay, codepoints):
+        """The overlapping list of one haystack above WINDOW_BYTES, whatever the match kind, as int64 rows (haystack,
+        pattern, start, end) in the reference's order (see _scan_one_large)."""
+        torch = _require_cuda()
+        dev = hay.device
+
+        def scan_window(window):
+            one = torch.tensor([0, window.numel()], dtype=torch.int64, device=dev)
+            m, _, _ = self._scan_overlapping_list(window, one, codepoints)
+            return m.to(torch.int64)
+
+        parts = scan_in_windows(scan_window, hay, self.WINDOW_BYTES, max(self.max_pattern_len - 1, 0), codepoints)
+        return torch.cat(parts, dim=0) if parts else torch.zeros((0, 4), dtype=torch.int64, device=dev)
 
     def _scan_overlapping_list(self, data, offsets, codepoints):
         """The overlapping match list whatever the automaton's match kind: the sieve's structures do not depend on the
@@ -1154,6 +1314,27 @@ class AhoCorasick:
         haystack has no match (see _Automaton.first_device)."""
         return self._ac.first_device(data, offsets, codepoints=True)
 
+    # ---- additions: match counts per haystack ------------------------------------------------------------------
+    def count_matches(self, haystack: str, overlapping: bool = False) -> int:
+        """-> ``len(find_matches_as_indexes(haystack, overlapping))``, counted without building the list."""
+        if not isinstance(haystack, str):
+            raise TypeError("argument 'haystack': 'str' expected")
+        self._ac.check_overlapping(overlapping)
+        return self._ac.count_host_batch([haystack.encode("utf-8")], overlapping)[0]
+
+    def count_matches_batch(self, haystacks: Sequence[str], overlapping: bool = False) -> list:
+        """``count_matches`` for each haystack, in one transfer and one scan."""
+        hays = list(haystacks)
+        for h in hays:
+            if not isinstance(h, str):
+                raise TypeError("argument 'haystack': 'str' expected")
+        self._ac.check_overlapping(overlapping)
+        return self._ac.count_host_batch([h.encode("utf-8") for h in hays], overlapping)
+
+    def count_matches_device(self, data, offsets, overlapping: bool = False):
+        """Device-resident UTF-8 batch -> int64 tensor (n,) of match counts (see _Automaton.count_device)."""
+        return self._ac.count_device(data, offsets, overlapping)
+
     def scan_host(self, data, offsets, overlapping: bool = False, **kw):
         """Host-resident UTF-8 batch (uint8 array + int64 offsets) -> host arrays (matches (k, 4), match_offsets (n + 1));
         code point indexes.  Copies and scans are pipelined (see _Automaton.scan_host)."""
@@ -1222,6 +1403,23 @@ class BytesAhoCorasick:
         """Device-resident batch -> int64 tensor (n, 3) of (pattern, start, end) in bytes, -1 rows where a haystack has
         no match (see _Automaton.first_device)."""
         return self._ac.first_device(data, offsets, codepoints=False)
+
+    # ---- additions: match counts per haystack ------------------------------------------------------------------
+    def count_matches(self, haystack, overlapping: bool = False) -> int:
+        """-> ``len(find_matches_as_indexes(haystack, overlapping))``, counted without building the list."""
+        hay = _as_buffer_bytes(haystack)
+        self._ac.check_overlapping(overlapping)
+        return self._ac.count_host_batch([hay], overlapping)[0]
+
+    def count_matches_batch(self, haystacks: Sequence, overlapping: bool = False) -> list:
+        """``count_matches`` for each haystack, in one transfer and one scan."""
+        hays = [_as_buffer_bytes(h) for h in haystacks]
+        self._ac.check_overlapping(overlapping)
+        return self._ac.count_host_batch(hays, overlapping)
+
+    def count_matches_device(self, data, offsets, overlapping: bool = False):
+        """Device-resident batch -> int64 tensor (n,) of match counts (see _Automaton.count_device)."""
+        return self._ac.count_device(data, offsets, overlapping)
 
     def scan_host(self, data, offsets, overlapping: bool = False, **kw):
         """Host-resident batch (uint8 array + int64 offsets) -> host arrays (matches (k, 4), match_offsets (n + 1));

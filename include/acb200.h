@@ -305,6 +305,45 @@ int acb_rows_to_codepoints(const uint8_t *dev_bytes, const int64_t *dev_offsets,
                            const int64_t *dev_rows, int64_t *dev_cp_rows, void *stream);
 
 /*
+ * How many matches each haystack has: len(find_matches_as_indexes(haystack, overlapping)) of the reference
+ * (get_matches, src/lib.rs:42-68), once per haystack of a device-resident batch, without the match list.  Counts are
+ * the same in bytes and in code points.  Three calls:
+ *
+ * acb_count_overlapping counts the overlapping matches (try_find_overlapping_iter, src/lib.rs:52-54): one launch of the
+ * sieve kernel in its count mode -- no records, no epilogue, no synchronisation, nothing skipped.  Standard automata
+ * only: any other kind returns ACB_EUNSUPPORTED before any byte is read, like the reference.  dev_counts =
+ * u64[n_haystacks], read and written: haystack h's count is ADDED to dev_counts[h] (zero the array for a fresh answer;
+ * accumulating lets the windows of one haystack share a counter).  dev_scratch = u64[3], any contents: the call clears
+ * it and leaves its task counter in [0].  Argument checks, the 2^31 limit and the empty cases are acb_any_match's.
+ *
+ * acb_count_non_overlapping counts the non-overlapping matches (try_find_iter, src/lib.rs:58-60) for every match kind:
+ * the sieve's list scan, as acb_scan_batch runs it (same plan, same workspace, kernel 5 whatever the tuning), then a
+ * count epilogue that places the overlapping list and counts each haystack's selection without packing it.  A haystack
+ * whose overlapping list has more than ACB_LONG_STRETCH records is counted by the whole grid (successor of every
+ * record, then pointer jumping), the others by one thread each.  dev_counts = u64[n_haystacks] is WRITTEN.  ws->dev_total:
+ * [0] = the sum of the counts, [1] = 1 when the counts are complete (0: the workspace was too small, every count is
+ * zero and [0] / [4] say how much room a second call needs, as for acb_scan_batch), [2] = haystacks counted by the
+ * whole grid, [3] = [5] = 0, [4] = records of the overlapping list.  Two launches, no synchronisation.  ws->dev_out and
+ * ws->dev_raw are overwritten; ws->dev_match_offsets is not used.
+ *
+ * acb_count_rows counts what acb_select_non_overlapping would select from the rows of ONE haystack (same shape and
+ * order): *dev_count = the count.  dev_scratch = 16 * n_rows bytes.  The work is spread over the grid (pointer jumping,
+ * as above) in one cooperative launch.
+ *
+ * All three return ACB_EINVAL, before any CUDA call, for a null pointer (a null dev_bytes is accepted when total_bytes
+ * == 0; dev_rows and dev_scratch may be null when n_rows == 0), n_haystacks outside [0, 2^32 - 2], total_bytes >= 2^31,
+ * n_rows >= 2^32 - 1, a workspace with a null buffer or a plan that acb_plan_scan does not give for these arguments.
+ */
+#define ACB_LONG_STRETCH 4096
+int acb_count_overlapping(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                          int64_t n_haystacks, uint64_t total_bytes, uint64_t *dev_counts, uint64_t *dev_scratch, void *stream);
+int acb_count_non_overlapping(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                              int64_t n_haystacks, uint64_t total_bytes, const acb_plan *plan, const acb_workspace *ws,
+                              uint64_t *dev_counts, void *stream);
+int acb_count_rows(const acb_automaton *a, const int64_t *dev_rows, uint64_t n_rows, uint64_t *dev_scratch, uint64_t *dev_count,
+                   void *stream);
+
+/*
  * Multi-GPU: the fixed-size block a rank contributes to the gather of the per-shard match lists (the only exchange
  * of the sharded path; NCCL all-gather over NVLink).  dev_block holds (cap + 1) records of 16 bytes: record 0 =
  * (match count, hay_base, complete flag, 0), then the first `cap` matches of a finished scan (dev_total / dev_out of
