@@ -32,7 +32,8 @@ class Workspace(C.Structure):
 
 
 class Tuning(C.Structure):
-    _fields_ = [("kernel", C.c_int), ("hot_rows", C.c_int), ("segment_bytes", C.c_int), ("table", C.c_int)]
+    _fields_ = [("kernel", C.c_int), ("hot_rows", C.c_int), ("segment_bytes", C.c_int), ("table", C.c_int),
+                ("sieve_ring", C.c_int)]
 
 
 class SieveDesc(C.Structure):
@@ -61,6 +62,8 @@ def lib():
         L.acb_version.restype = C.c_char_p
         L.acb_launch_count.restype = C.c_uint64
         L.acb_set_tuning.argtypes = [C.POINTER(Tuning)]
+        L.acb_sieve_ring.restype = C.c_uint32
+        L.acb_sieve_ring.argtypes = [C.c_uint32, C.c_uint32]
         L.acb_timing_enable.argtypes = [C.c_int]
         L.acb_timing_read.argtypes = [C.POINTER(C.c_double), C.POINTER(C.c_uint64)]
         L.acb_build.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.POINTER(C.c_void_p)]
@@ -108,10 +111,10 @@ def lib():
 _tls = __import__("threading").local()
 
 
-def set_tuning(kernel: int = 0, hot_rows: int = 0, segment_bytes: int = 0, table: int = 0) -> None:
+def set_tuning(kernel: int = 0, hot_rows: int = 0, segment_bytes: int = 0, table: int = 0, sieve_ring: int = 0) -> None:
     """acb_set_tuning for the calling thread (the library keeps the knobs per thread); the host layer reads
     the choice back with current_kernel() to decide which device images a scan needs."""
-    t = Tuning(kernel, hot_rows, segment_bytes, table)
+    t = Tuning(kernel, hot_rows, segment_bytes, table, sieve_ring)
     if lib().acb_set_tuning(C.byref(t)) != ACB_OK:
         raise RuntimeError(last_error())
     _tls.kernel = kernel
@@ -129,7 +132,7 @@ EXPORTS = [
     "acb_last_error", "acb_version", "acb_build", "acb_free", "acb_num_patterns", "acb_num_states",
     "acb_num_columns", "acb_max_pattern_len", "acb_min_pattern_len", "acb_match_kind", "acb_image_bytes",
     "acb_image_write", "acb_plan_scan", "acb_scan_batch",
-    "acb_launch_count", "acb_set_tuning", "acb_timing_enable", "acb_timing_read",
+    "acb_launch_count", "acb_set_tuning", "acb_sieve_ring", "acb_timing_enable", "acb_timing_read",
     "acb_profile", "acb_hot_bytes", "acb_hot_build", "acb_hot_rows", "acb_hot_describe",
     "acb_sieve_build", "acb_sieve_write", "acb_sieve_describe", "acb_pack_gather_block", "acb_select_non_overlapping",
     "acb_any_match", "acb_find_first", "acb_first_rows", "acb_rows_to_codepoints",

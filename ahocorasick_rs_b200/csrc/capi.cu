@@ -1102,7 +1102,7 @@ struct acb_automaton {
 // thread (two automata scanned from two threads do not see each other's settings); the launch counter is atomic.
 static thread_local std::string g_err;
 static std::atomic<unsigned long long> g_launches{0};
-static thread_local acb_tuning g_tuning = {0, 0, 0, 0};  // kernel, hot_rows, segment_bytes, table
+static thread_local acb_tuning g_tuning = {0, 0, 0, 0, 0};  // kernel, hot_rows, segment_bytes, table, sieve_ring
 
 // optional device timing of the dominant (scan) kernel, for bench.py's roofline
 static thread_local bool g_timing = false;
@@ -1300,6 +1300,17 @@ int acb_plan_scan(const acb_automaton *a, const void *dev_bytes, uint64_t total_
     // | table walkers' epilogue: one "has matches" bit per unit
     plan->scratch_words = 8 + (tiles + 1) + (tiles + 1) + (per_piece + 2) + (per_piece / 2 + 2) + (plan->n_units / 64 + 2);
     return ACB_OK;
+}
+
+// as many windows of text per warp as fit next to the filters (a power of two): the more, the fuller the rounds of the
+// later stages when survivors are rare.  tuning.sieve_ring caps it (rounded down to a power of two); 0 = nothing fits
+uint32_t acb_sieve_ring(uint32_t bloom_bytes, uint32_t smem_optin) {
+    auto fits = [&](uint32_t ring) { return uint64_t(bloom_bytes) + sieve_smem_bytes(0, ring, false) <= smem_optin; };  // (no wrap)
+    uint32_t ring = kRingMax;
+    if (g_tuning.sieve_ring > 0)
+        while (ring > (uint32_t)g_tuning.sieve_ring) ring >>= 1;
+    while (ring > 1 && !fits(ring)) ring >>= 1;
+    return fits(ring) ? ring : 0u;
 }
 
 }  // extern "C"
@@ -1501,13 +1512,9 @@ DevSieve make_sieve_view(const SieveHeader &h, const void *dev_sieve) {
 template <bool CP, int MODE = kSieveList>
 int launch_sieve(const DevSieve &sv, const Batch &B, SievePlan &P, const Sink &out, uint32_t *task_cont, uint32_t *hay_cont,
                  unsigned int *task_counter, const DeviceInfo &d, cudaStream_t st) {
-    // as many windows of text per warp as fit next to the filters (a power of two): the more, the fuller the rounds of
-    // the later stages when survivors are rare
-    const uint32_t filter_bytes = sv.bloom_words * 4;
-    uint32_t ring = kRingMax;
-    while (ring > 1 && sieve_smem_bytes(filter_bytes, ring, CP) > (uint32_t)d.max_smem_optin) ring >>= 1;
-    const uint32_t smem = sieve_smem_bytes(filter_bytes, ring, CP);
-    if (smem > (uint32_t)d.max_smem_optin) return fail(ACB_ECUDA, "the sieve's filters do not fit in shared memory (rebuild them with a smaller bloom_bytes_max)");
+    const uint32_t ring = acb_sieve_ring(sv.bloom_words * 4, (uint32_t)d.max_smem_optin);
+    if (ring == 0) return fail(ACB_ECUDA, "the sieve's filters do not fit in shared memory (rebuild them with a smaller bloom_bytes_max)");
+    const uint32_t smem = sieve_smem_bytes(sv.bloom_words * 4, ring, CP);
     P.ring = ring;
 #define ACB_SIEVE_GO(WC)                                                                                  \
     do {                                                                                                  \

@@ -182,14 +182,18 @@ class _Automaton:
     SIEVE_SMEM_RESERVE = int(__import__("os").environ.get("ACB200_SIEVE_RESERVE_KB", "46")) * 1024   # 24 warps x (one ring slot of text + two queues); barrier
     SIEVE_W_MAX = 0                  # 0 = the builder chooses the primary window
 
+    @staticmethod
+    def _smem_optin(idx):
+        props = _torch().cuda.get_device_properties(idx)
+        return int(getattr(props, "shared_memory_per_block_optin", 227 * 1024))
+
     def sieve(self, device):
         """(device tensor, SieveDesc) of the sieve image on `device`, built and uploaded once."""
         torch = _require_cuda()
         idx = device.index if device.index is not None else torch.cuda.current_device()
         ent = self._sieves.get(idx)
         if ent is None:
-            props = torch.cuda.get_device_properties(idx)
-            smem = int(getattr(props, "shared_memory_per_block_optin", 227 * 1024))
+            smem = self._smem_optin(idx)
             nbytes = int(self._L.acb_sieve_build(self._h, max(4096, smem - self.SIEVE_SMEM_RESERVE), self.SIEVE_W_MAX))
             if nbytes == 0:
                 raise RuntimeError(_capi.last_error())
@@ -202,6 +206,17 @@ class _Automaton:
             ent = (host.to(torch.device("cuda", idx)), desc)
             self._sieves[idx] = ent
         return ent
+
+    def sieve_geometry(self, device, task_bytes):
+        """What shapes a sieve scan on `device` (for last_stats): the image's primary window, filter depth, probes and
+        filter bytes, the ring depth the kernel runs with (acb_sieve_ring: the calling thread's tuning applies) and the
+        task size.  None of it changes results; tests check it to know that an input reached the geometry it was made
+        for."""
+        torch = _torch()
+        idx = device.index if device.index is not None else torch.cuda.current_device()
+        desc = self.sieve(device)[1]
+        return {"window": desc.window, "last_level": desc.last_level, "probes": desc.probes, "bloom_bytes": desc.bloom_bytes,
+                "ring": int(self._L.acb_sieve_ring(desc.bloom_bytes, self._smem_optin(idx))), "task_bytes": int(task_bytes)}
 
     # ---- the hot image (rows kept in shared memory), chosen from a sample of the data ----
     HOT_TABLE_BYTES = 40 * 1024   # with 32 warps of staging buffers next to it, this is what fits on chip
@@ -413,7 +428,7 @@ class _Automaton:
             _, skipped, windows = scratch.tolist()
             task_bytes = int(plan.task_bytes)
             tasks = (data.numel() + (data.data_ptr() & 511) + task_bytes - 1) // task_bytes
-            self.last_stats = {"engine": "sieve", "mode": "any", "task_bytes": task_bytes, "tasks": tasks,
+            self.last_stats = {"engine": "sieve", "mode": "any", **self.sieve_geometry(dev, task_bytes), "tasks": tasks,
                                "tasks_skipped": skipped, "windows_skipped": windows}
         return out
 
@@ -538,7 +553,7 @@ class _Automaton:
             scratch = self.first_keys(data, offsets, keys)
             rows = self.first_rows(data, offsets, keys)
             task_bytes = int(self._plan(data, n).task_bytes)
-            self.last_stats = {"engine": "sieve", "mode": "first", "task_bytes": task_bytes,
+            self.last_stats = {"engine": "sieve", "mode": "first", **self.sieve_geometry(dev, task_bytes),
                                "tasks": (data.numel() + (data.data_ptr() & 511) + task_bytes - 1) // task_bytes,
                                "skip_counters": scratch}   # device tensor: [task counter, tasks skipped, windows not scanned]
         return self._rows_to_codepoints(data, offsets, rows) if codepoints else rows
@@ -686,7 +701,8 @@ class _Automaton:
                                                    counts.data_ptr(), scratch.data_ptr(), stream.cuda_stream)
                 if rc != _capi.ACB_OK:
                     raise RuntimeError(_capi.last_error())
-                self.last_stats = {"engine": "sieve", "mode": "count", "long_stretches": 0}
+                self.last_stats = {"engine": "sieve", "mode": "count", **self.sieve_geometry(dev, self._plan(data, n).task_bytes),
+                                   "long_stretches": 0}
                 return counts
             plan = self._plan(data, n)
             cap = capacity or max(1024, n * 2)
@@ -707,7 +723,7 @@ class _Automaton:
                 if complete or (total == 0 and raw_total == 0):
                     break
                 cap = max(total, raw_total) + max(total, raw_total) // 8 + 16
-            self.last_stats = {"engine": "sieve", "mode": "count", "task_bytes": plan.task_bytes, "list_records": raw_total,
+            self.last_stats = {"engine": "sieve", "mode": "count", **self.sieve_geometry(dev, plan.task_bytes), "list_records": raw_total,
                                "long_stretches": long_stretches}
             return counts
 
@@ -857,10 +873,8 @@ class _Automaton:
                                        "global_table": bool(hot["rows"].reserved & 1),
                                        "segment_bytes": plan.segment_bytes, "lane_stride": plan.lane_stride}
                 else:
-                    self.last_stats = {"engine": "sieve", "window": sieve_d.window, "last_level": sieve_d.last_level,
-                                       "probes": sieve_d.probes, "bloom_bytes": sieve_d.bloom_bytes, "nodes": sieve_d.nodes,
-                                       "keys": sieve_d.keys, "filter_entries": sieve_d.filter_entries,
-                                       "task_bytes": plan.task_bytes, "list_records": raw_total}
+                    self.last_stats = {"engine": "sieve", **self.sieve_geometry(dev, plan.task_bytes), "nodes": sieve_d.nodes,
+                                       "keys": sieve_d.keys, "filter_entries": sieve_d.filter_entries, "list_records": raw_total}
                 if complete or (total == 0 and raw_total == 0):
                     return ws["out"][:total], ws["match_offsets"][: n + 1], total
                 cap = max(total, raw_total) + max(total, raw_total) // 8 + 16

@@ -372,8 +372,18 @@ typedef struct acb_tuning {
     int hot_rows;      /* cap on rows kept in shared memory */
     int segment_bytes; /* segment size (rounded up to a multiple of 64 and to 8 x the warm-up); kernel 5: task size (multiple of 512) */
     int table;         /* 0 auto, 1 = column-indexed compact table only, 2 = byte-indexed 128-wide table when available */
+    int sieve_ring;    /* cap on the sieve's ring depth (512-byte windows of text each warp keeps in shared memory), rounded
+                          down to a power of two in [1, 8] (0 or less: as many as fit); it never raises the ring above what
+                          fits next to the filters (see acb_sieve_ring) */
 } acb_tuning;
 int acb_set_tuning(const acb_tuning *t);
+
+/*
+ * The ring depth every sieve scan on this thread runs with for filters of bloom_bytes (acb_sieve_desc.bloom_bytes) on
+ * a device with smem_optin bytes of opt-in shared memory per block: the largest power of two up to 8 whose ring fits
+ * next to the filters, capped by the calling thread's acb_tuning.sieve_ring.  0 = the filters do not fit at all.
+ */
+uint32_t acb_sieve_ring(uint32_t bloom_bytes, uint32_t smem_optin);
 
 #ifdef __cplusplus
 }

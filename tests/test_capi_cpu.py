@@ -26,6 +26,54 @@ def test_library_exports_every_declared_symbol():
     assert b"sm_90a" in L.acb_version()
 
 
+H100_SMEM_OPTIN = 232_448   # opt-in shared memory per block on an H100 (227 KiB)
+
+
+def sieve_smem(bloom_bytes, ring):
+    """scan_sieve.cuh sieve_smem_bytes: the filters, the mbarrier (16 B), then per warp (24) a ring of 576-byte slots
+    (16 B of history, a 512-byte window, 48 B of code point counts), a 16-byte pad and two 64-entry queues (4 B, 16 B)."""
+    return bloom_bytes + 16 + 24 * (ring * (16 + 512 + 48) + 16 + 64 * 4 + 64 * 16)
+
+
+def test_sieve_ring_export():
+    L = _capi.lib()
+    assert "acb_sieve_ring" in _capi.EXPORTS and L.acb_sieve_ring is not None
+    assert [f[0] for f in _capi.Tuning._fields_][-1] == "sieve_ring"
+
+
+@pytest.mark.parametrize("ring,largest", [(8, 90_736), (4, 146_032), (2, 173_680), (1, 187_504)])
+def test_sieve_ring_at_its_boundaries(ring, largest):
+    """The deepest ring that fits next to the filters, for each of the four depths: at the largest filter that leaves
+    room for it, and one byte past it (the next smaller ring, or 0 when not even one window fits)."""
+    L = _capi.lib()
+    _capi.set_tuning()
+    assert sieve_smem(largest, ring) == H100_SMEM_OPTIN
+    assert L.acb_sieve_ring(largest, H100_SMEM_OPTIN) == ring
+    assert L.acb_sieve_ring(largest + 1, H100_SMEM_OPTIN) == ring // 2
+    assert L.acb_sieve_ring(largest - 16, H100_SMEM_OPTIN) == ring
+    assert L.acb_sieve_ring(4096, H100_SMEM_OPTIN) == 8
+    assert L.acb_sieve_ring(0xFFFF_FFF0, H100_SMEM_OPTIN) == 0
+
+
+@pytest.mark.parametrize("bloom_bytes,fits", [(4096, 8), (90_736, 8), (90_737, 4), (146_033, 2), (173_681, 1)])
+def test_sieve_ring_cap_rounds_down_and_never_raises(bloom_bytes, fits):
+    L = _capi.lib()
+    try:
+        for cap in range(0, 20):
+            _capi.set_tuning(5, 0, 512, 0, sieve_ring=cap)
+            want = fits if cap == 0 else min(fits, 1 << (cap.bit_length() - 1))
+            assert L.acb_sieve_ring(bloom_bytes, H100_SMEM_OPTIN) == want, cap
+        _capi.set_tuning(sieve_ring=3)
+        assert L.acb_sieve_ring(4096, H100_SMEM_OPTIN) == 2
+        _capi.set_tuning(sieve_ring=9)
+        assert L.acb_sieve_ring(4096, H100_SMEM_OPTIN) == 8
+        _capi.set_tuning(sieve_ring=-1)   # not a cap: as many as fit
+        assert L.acb_sieve_ring(bloom_bytes, H100_SMEM_OPTIN) == fits
+    finally:
+        _capi.set_tuning()
+    assert L.acb_sieve_ring(bloom_bytes, H100_SMEM_OPTIN) == fits
+
+
 def test_build_and_image_roundtrip_without_gpu():
     L = _capi.lib()
     pats = [b"hello", b"world", b"fish"]

@@ -1,0 +1,200 @@
+"""GPU tests of the sieve (scan_sieve.cuh) at geometries the builder would not pick for these inputs (-m gpu): every
+primary window W (1..8) against every ring depth R (1, 2, 4, 8 windows of text per warp), 16 KiB and 512-byte tasks,
+code points, the filter budget (default, shallow: nothing on chip beyond the primary window, saturated: a 4 KiB
+filter whose primary bitmap is nearly full), and reverse-trie nodes with 1, 8, 9, 255 and 256 children.  Every case
+runs all four of the kernel's modes -- the match list (three kinds and overlapping), is_match, find_first and the
+counts -- against the CPU oracle, and asserts after every call that last_stats report the geometry it was built for
+(a changed default that stops an input from reaching its corner fails here instead of passing silently)."""
+import contextlib
+import functools
+
+import numpy as np
+import pytest
+
+pytestmark = pytest.mark.gpu
+
+torch = pytest.importorskip("torch")
+
+from ahocorasick_rs_b200 import MatchKind, _capi, matcher  # noqa: E402
+from oracle import Oracle  # noqa: E402
+
+from .gpu_helpers import KINDS, check_batch, dev, dev_at, make_ac  # noqa: E402
+from .sieve_inputs import FANOUTS, TWO_LEVEL, dense_case, fanout_case, planted_case  # noqa: E402
+from .sieve_interp import SieveImage  # noqa: E402
+
+RINGS = (1, 2, 4, 8)
+SHIFTS = (0, 1, 511)   # where the data starts after a 512-byte aligned address: moves the window and task grids
+DEFAULT_TASK = 16384
+
+
+@functools.lru_cache(maxsize=None)
+def planted(utf8, decoys=0):
+    return planted_case(utf8, decoys=decoys)
+
+
+@functools.lru_cache(maxsize=None)
+def dense(utf8):
+    return dense_case(utf8)
+
+
+@functools.lru_cache(maxsize=None)
+def fanout(f):
+    return fanout_case(f)
+
+
+@functools.lru_cache(maxsize=None)
+def host_geometry(case, budget, w):
+    """What the builder makes of a case at a filter budget, on the host (tests/sieve_interp.SieveImage: the same C
+    builder) -> (window, last_level, probes, bloom_bytes, primary bitmap fill)."""
+    pats = case_inputs(case)[0]
+    img = SieveImage(pats, 0, budget, w)
+    fill = float(np.unpackbits(img.bloom[:img.prim_words].view(np.uint8)).mean())
+    return img.W, img.last_level, img.n_probes, img.bloom_words * 4, fill
+
+
+def case_inputs(case):
+    name, utf8 = case
+    if name == "dense":
+        return dense(utf8)
+    return planted(utf8, 1000 if name == "decoys" else 0)
+
+
+@contextlib.contextmanager
+def geometry(monkeypatch, w, ring, task_bytes, budget=None):
+    """Sieve scans on this thread with primary window w (automata built inside: the image is built at the first
+    scan), ring depth `ring`, tasks of task_bytes and, when given, filters built for `budget` bytes."""
+    monkeypatch.setattr(matcher._Automaton, "SIEVE_W_MAX", w)
+    if budget is not None:
+        smem = matcher._Automaton._smem_optin(torch.cuda.current_device())
+        monkeypatch.setattr(matcher._Automaton, "SIEVE_SMEM_RESERVE", smem - budget)
+    _capi.set_tuning(5, 0, task_bytes, 0, sieve_ring=ring)
+    try:
+        yield
+    finally:
+        _capi.set_tuning(0)
+
+
+def assert_geometry(ac, want):
+    st = ac._ac.last_stats
+    assert st["engine"] == "sieve", st
+    for k, v in want.items():
+        assert st[k] == v, (k, v, st)
+
+
+def oracle(pats, kind, data, offs, overlapping=False, codepoints=False):
+    return Oracle(pats, kind.name).scan_batch(data, offs, overlapping=overlapping, codepoints=codepoints)
+
+
+def first_rows(pats, kind, data, offs, codepoints):
+    """The oracle's first record per haystack, (n, 3) rows with -1 where there is none."""
+    _, counts, rec = oracle(pats, kind, data, offs, codepoints=codepoints)
+    rows = np.full((len(offs) - 1, 3), -1, dtype=np.int64)
+    at = np.concatenate([[0], np.cumsum(counts.astype(np.int64))[:-1]])
+    has = counts > 0
+    rows[has] = rec[at[has]][:, 1:4].astype(np.int64)
+    return rows
+
+
+def check_all_modes(pats, data, offs, want, codepoints=False, shift=0):
+    """The four searches' lists, is_match, find_first for every kind and both counts, each against the oracle, with
+    the geometry asserted after every call.  -> overlapping matches in the batch."""
+    d, o = dev_at(data, shift), dev(offs)
+    over_total, over_counts, _ = oracle(pats, MatchKind.Standard, data, offs, overlapping=True)
+    assert over_total > 0
+    for kind in KINDS:
+        ac = make_ac(pats, kind, codepoints)
+        check_batch(pats, kind, data, offs, codepoints=codepoints, ac=ac, shift=shift)
+        assert_geometry(ac, want)
+        got = ac.find_first_device(d, o).cpu().numpy()
+        assert_geometry(ac, want)
+        assert np.array_equal(got, first_rows(pats, kind, data, offs, codepoints)), kind
+        _, counts, _ = oracle(pats, kind, data, offs)
+        got = ac.count_matches_device(d, o).cpu().numpy()
+        assert_geometry(ac, want)
+        assert np.array_equal(got, counts.astype(np.int64)), kind
+        if kind == MatchKind.Standard:
+            check_batch(pats, kind, data, offs, overlapping=True, codepoints=codepoints, ac=ac, shift=shift)
+            assert_geometry(ac, want)
+            got = ac.count_matches_device(d, o, overlapping=True).cpu().numpy()
+            assert_geometry(ac, want)
+            assert np.array_equal(got, over_counts.astype(np.int64))
+            got = ac.is_match_device(d, o).cpu().numpy()
+            assert_geometry(ac, want)
+            assert np.array_equal(got, over_counts > 0)
+    return over_total
+
+
+# ---------------------------------------------------------------- W x R, planted batch
+@pytest.mark.parametrize("ring", RINGS)
+@pytest.mark.parametrize("w", range(1, 9))
+def test_window_by_ring(monkeypatch, w, ring):
+    pats, data, offs = planted(False)
+    with geometry(monkeypatch, w, ring, DEFAULT_TASK):
+        check_all_modes(pats, data, offs, {"window": w, "ring": ring, "task_bytes": DEFAULT_TASK}, shift=SHIFTS[(w + ring) % 3])
+
+
+@pytest.mark.parametrize("ring", (1, 8))
+@pytest.mark.parametrize("w", (1, 4, 5, 8))
+def test_window_by_ring_small_tasks(monkeypatch, w, ring):
+    """One window per task: every queue is drained at every task's end, every window starts a task."""
+    pats, data, offs = planted(False)
+    with geometry(monkeypatch, w, ring, 512):
+        check_all_modes(pats, data, offs, {"window": w, "ring": ring, "task_bytes": 512}, shift=SHIFTS[(w + ring) % 3])
+
+
+@pytest.mark.parametrize("ring", RINGS)
+@pytest.mark.parametrize("w", (1, 3, 4, 5, 8))
+def test_code_points_window_by_ring(monkeypatch, w, ring):
+    """Multi-byte characters between and inside the occurrences: stage 1 takes each survivor's continuation count
+    from the ring slot of its window."""
+    pats, data, offs = planted(True)
+    with geometry(monkeypatch, w, ring, DEFAULT_TASK):
+        check_all_modes(pats, data, offs, {"window": w, "ring": ring, "task_bytes": DEFAULT_TASK}, codepoints=True,
+                        shift=SHIFTS[(w + ring) % 3])
+
+
+# ---------------------------------------------------------------- filter budget
+BUDGET_W = 5
+BUDGETS = {
+    # name: (inputs, filter budget in bytes (None: what the default reserve leaves))
+    "default": ("planted", None),
+    "shallow": ("decoys", 8192),      # 1 000 more patterns in 8 KiB: the secondary filter holds the primary window only
+    "saturated": ("dense", 4096),     # 100 000 patterns in the smallest budget: the primary bitmap nearly full
+}
+
+
+@pytest.mark.parametrize("utf8", [False, True], ids=["bytes", "utf8"])
+@pytest.mark.parametrize("task_bytes", (DEFAULT_TASK, 512))
+@pytest.mark.parametrize("ring", (1, 8))
+@pytest.mark.parametrize("budget", list(BUDGETS))
+def test_filter_budget(monkeypatch, budget, ring, task_bytes, utf8):
+    name, nbytes = BUDGETS[budget]
+    case = (name, utf8)
+    pats, data, offs = case_inputs(case)
+    smem = matcher._Automaton._smem_optin(torch.cuda.current_device())
+    host_budget = nbytes if nbytes is not None else max(4096, smem - matcher._Automaton.SIEVE_SMEM_RESERVE)
+    W, last_level, probes, bloom_bytes, fill = host_geometry(case, host_budget, BUDGET_W)
+    assert W == BUDGET_W
+    if budget == "default":
+        assert last_level == 16   # kSieveMaxLevel: the on-chip walk as deep as it goes
+    elif budget == "shallow":
+        assert last_level == W and fill < 0.05
+    else:
+        assert last_level == W and bloom_bytes == 4096 and fill >= 0.95, fill   # nearly every position reaches stage 1
+    want = {"window": W, "last_level": last_level, "probes": probes, "bloom_bytes": bloom_bytes, "ring": ring,
+            "task_bytes": task_bytes}
+    with geometry(monkeypatch, BUDGET_W, ring, task_bytes, nbytes):
+        check_all_modes(pats, data, offs, want, codepoints=utf8, shift=SHIFTS[(ring + task_bytes // 512) % 3])
+
+
+# ---------------------------------------------------------------- reverse-trie fan-out
+@pytest.mark.parametrize("ring", (1, 8))
+@pytest.mark.parametrize("w", (1, 5, 8))
+@pytest.mark.parametrize("fan", list(FANOUTS) + [TWO_LEVEL])
+def test_trie_fanout(monkeypatch, fan, w, ring):
+    """A node with 1, 8 (the last linear scan), 9 (the first binary search), 255 or 256 children (a count that needs
+    the ninth bit), children 0x00 and 0xff at the ends, and two levels of many children; the text puts each of the 256
+    byte values before the core."""
+    pats, data, offs = fanout(fan)
+    with geometry(monkeypatch, w, ring, DEFAULT_TASK):
+        check_all_modes(pats, data, offs, {"window": w, "ring": ring, "task_bytes": DEFAULT_TASK}, shift=SHIFTS[w % 3])

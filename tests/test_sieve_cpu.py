@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 from oracle import Oracle
+from tests.sieve_inputs import FANOUTS, TWO_LEVEL, fanout_case
 from tests.sieve_interp import SieveImage, scan
 from ahocorasick_rs_b200 import workloads as W
 
@@ -60,6 +61,30 @@ def test_tiny_filter_still_exact():
     img = SieveImage(pats, 2, bloom_bytes_max=1024)
     assert img.last_level == img.W
     assert scan(img, data, offs, False) == oracle_rows(pats, "LeftmostLongest", data, offs, False)
+
+
+@pytest.mark.parametrize("w_max", [1, 5, 8])
+@pytest.mark.parametrize("fanout", list(FANOUTS) + [TWO_LEVEL])
+def test_trie_fanout(fanout, w_max):
+    """A trie node with 1, 8, 9, 255 or 256 children (and two levels of many), every byte value before it in the text:
+    the builder's child lists (sorted, 9-bit counts) give the oracle's matches for every kind."""
+    pats, data, offs = fanout_case(fanout)
+    for kind in range(3):
+        img = SieveImage(pats, kind, w_max=w_max)
+        assert img.W == w_max
+        for overlapping in ([False, True] if kind == 0 else [False]):
+            assert scan(img, data, offs, overlapping) == oracle_rows(pats, KINDS[kind], data, offs, overlapping)
+
+
+def test_fanout_inputs_reach_their_child_counts():
+    """The node of the core has exactly the children asked for (the count of 256 needs the 9th bit of the field)."""
+    for fanout in list(FANOUTS) + [TWO_LEVEL]:
+        pats, _, _ = fanout_case(fanout)
+        img = SieveImage(pats, 0, w_max=8)
+        counts = (img.na[: img.n_nodes, 1] >> 8) & 0x1FF
+        assert counts.max() == (12 if fanout == TWO_LEVEL else fanout), fanout
+        if fanout == TWO_LEVEL:
+            assert (counts == 10).sum() == 12
 
 
 def test_duplicates_nested_and_self_overlapping():
