@@ -1087,6 +1087,250 @@ __global__ void zero_outputs_kernel(unsigned long long *unit_offsets, unsigned l
     if (blockIdx.x == 0 && threadIdx.x == 0) unit_offsets[0] = 0;
 }
 
+// ---------------------------------------------------------------------------
+// Stream search (acb_stream_seams / acb_stream_resolve): matches in data fed in chunks.  Per stream the caller keeps a
+// carry (kCarry* words) and a tail: the last min(F, max_pattern_len - 1) bytes fed.  A feed scans the caller's chunks
+// as they are, and a SEAM per stream -- tail || the chunk's first min(len, max_pattern_len - 1) bytes -- for the
+// matches that cross into the chunk.  The sequence a stream selects from is: every record of its seam, then its chunk's
+// records that end past the seam's head (the others are in the seam too).  Both parts are sorted by (end, start,
+// pattern) and the second ends after the first, so the concatenation is the overlapping list of tail || chunk.
+// ---------------------------------------------------------------------------
+enum : int { kCarryFed = 0, kCarryRestart = 1, kCarryTail = 2, kCarryCont = 3, kCarryWords = 4 };
+
+__device__ __forceinline__ bool is_cont_byte(uint32_t b) { return (b & 0xC0u) == 0x80u; }
+
+// seam_offsets[i + 1] = tail length + head length of stream i
+__global__ void stream_seam_lengths_kernel(const int64_t *offsets, int64_t n, const int64_t *carry, uint32_t halo, int64_t *seam_offsets) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t len = offsets[i + 1] - offsets[i];
+        seam_offsets[i + 1] = carry[kCarryWords * i + kCarryTail] + min(len, (int64_t)halo);
+    }
+}
+
+// v[0] = 0, v[1 .. n] = inclusive prefix sums of v[1 .. n] (one block)
+__global__ void __launch_bounds__(kScanThreads) stream_prefix_kernel(int64_t *v, int64_t n) {
+    unsigned long long carry = 0;
+    for (int64_t base = 0; base < n; base += kScanThreads) {
+        const int64_t i = base + threadIdx.x;
+        const unsigned long long x = i < n ? (unsigned long long)v[i + 1] : 0ull;
+        unsigned long long total;
+        const unsigned long long before = block_exclusive_scan(x, &total);
+        if (i < n) v[i + 1] = (int64_t)(carry + before + x);
+        carry += total;
+    }
+    if (threadIdx.x == 0) v[0] = 0;
+}
+
+// one warp per stream: seam i = tail || head at seam_offsets[i]
+__global__ void stream_seam_fill_kernel(const uint8_t *bytes, const int64_t *offsets, int64_t n, const int64_t *carry, const uint8_t *tail,
+                                        uint32_t halo, const int64_t *seam_offsets, uint8_t *seam) {
+    const uint32_t lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
+        const int64_t t = carry[kCarryWords * i + kCarryTail], s0 = seam_offsets[i], len = seam_offsets[i + 1] - s0;
+        const uint8_t *src_tail = tail + (uint64_t)i * halo, *src_head = bytes + offsets[i];
+        for (int64_t k = lane; k < len; k += 32) seam[s0 + k] = k < t ? src_tail[k] : src_head[k - t];
+    }
+}
+
+// The records stream i selects from (see above), with absolute positions.
+struct StreamView {
+    const uint4 *seam, *chunk;
+    unsigned long long ns;     // seam records; then the chunk's, from its first that ends past the head
+    long long seam_base, chunk_base;
+};
+__device__ __forceinline__ SelRec sel_rec(const StreamView *v, unsigned long long j) {
+    const bool in_seam = j < v->ns;
+    const uint4 m = in_seam ? v->seam[j] : v->chunk[j - v->ns];
+    const long long base = in_seam ? v->seam_base : v->chunk_base;
+    return {(long long)m.y, base + (long long)m.z, base + (long long)m.w};
+}
+
+// the first record of r[lo .. hi) that ends after `after`
+__device__ __forceinline__ unsigned long long first_end_after(const uint4 *r, unsigned long long lo, unsigned long long hi, uint32_t after) {
+    while (lo < hi) {
+        const unsigned long long mid = (lo + hi) >> 1;
+        if (r[mid].w <= after)
+            lo = mid + 1;
+        else
+            hi = mid;
+    }
+    return lo;
+}
+
+struct StreamArgs {
+    Batch B;                        // the chunks: one haystack per stream
+    int64_t *carry;                 // [n][kCarryWords]
+    uint8_t *tail;                  // [n][halo]
+    const uint8_t *last;            // [n] or null
+    const uint8_t *seam;
+    const int64_t *seam_offsets;    // [n + 1]
+    const uint4 *seam_list, *chunk_list;
+    const unsigned long long *seam_mo, *chunk_mo;  // [n + 1] each
+    long long *staged;              // rows (stream, pattern, start, end) of stream i from seam_mo[i] + chunk_mo[i] on
+    long long *cont_rows;           // [n][3] (0, x, x): x = chunk bytes before the new tail (code points)
+    long long *cont_cp;             // [n][3] the same after acb_rows_to_codepoints
+    int64_t *row_offsets;           // [n + 1]
+    long long *rows;                // the released rows, packed
+    unsigned long long *stats;      // [0] records considered, [1] streams holding something back
+    const uint32_t *pat_cplen;      // code points: each pattern's length in code points
+    uint32_t halo;                  // max_pattern_len - 1
+    int mode, longest, codepoints;
+};
+
+// stream i's sequence (overlapping: only the seam's records that end past the tail are new); -> its length
+__device__ __forceinline__ unsigned long long stream_view(const StreamArgs &A, int64_t i, StreamView &v) {
+    const int64_t *c = A.carry + kCarryWords * i;
+    const long long t = c[kCarryTail], head = min((long long)(A.B.offsets[i + 1] - A.B.offsets[i]), (long long)A.halo);
+    const unsigned long long s0 = A.seam_mo[i], s1 = A.seam_mo[i + 1], c0 = A.chunk_mo[i], c1 = A.chunk_mo[i + 1];
+    const unsigned long long cf = first_end_after(A.chunk_list, c0, c1, (uint32_t)head);
+    const unsigned long long sf = A.mode == kModeOverlap ? first_end_after(A.seam_list, s0, s1, (uint32_t)t) : s0;
+    v.chunk_base = c[kCarryFed];
+    v.seam_base = c[kCarryFed] - t;
+    v.chunk = A.chunk_list + cf;
+    v.seam = A.seam_list + sf;
+    v.ns = s1 - sf;
+    return v.ns + (c1 - cf);
+}
+
+// One thread per stream: the release of this feed.  Overlapping: every record of the sequence (the emit kernel reads
+// them from the lists).  Non-overlapping: the reference's selection (next_selected, as acb_count_rows follows it),
+// continued from the carried restart point, up to the first pick that the release rule does not yet allow: Standard
+// releases every pick (it ends in the data seen), the leftmost kinds a pick that starts at least max_pattern_len bytes
+// before the end of the data seen (no later record can start before it).  Rows go to staged[], their count to
+// row_offsets[i + 1].
+template <int MODE>
+__global__ void stream_select_kernel(StreamArgs A) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < A.B.n_haystacks; i += (int64_t)gridDim.x * blockDim.x) {
+        int64_t *c = A.carry + kCarryWords * i;
+        const long long fed = c[kCarryFed], len = A.B.offsets[i + 1] - A.B.offsets[i];
+        const long long fed_after = fed + len;
+        const bool last = A.last && A.last[i];
+        StreamView v;
+        const unsigned long long n = stream_view(A, i, v);
+        long long *out = A.staged + 4 * (A.seam_mo[i] + A.chunk_mo[i]);
+        unsigned long long w = 0;
+        bool pending = false;
+        auto put = [&](const SelRec &m) {
+            out[4 * w] = i, out[4 * w + 1] = m.pid, out[4 * w + 2] = m.start, out[4 * w + 3] = m.end;
+            w++;
+        };
+        long long s = c[kCarryRestart];
+        if (MODE == kModeOverlap) {
+            w = n;
+        } else {
+            for (;;) {
+                const unsigned long long j = next_selected<MODE>(&v, n, s, (long long)A.halo + 1, A.longest);
+                if (j >= n) break;
+                const SelRec m = sel_rec(&v, j);
+                if (MODE == kModeLeftmost && !last && m.start + (long long)A.halo + 1 > fed_after) {
+                    pending = true;
+                    break;
+                }
+                put(m);
+                s = m.end;
+            }
+            c[kCarryRestart] = s;
+        }
+        A.row_offsets[i + 1] = (int64_t)w;
+        const long long t_after = min(fed_after, (long long)A.halo);
+        if (A.codepoints) {
+            const long long x = max(len - t_after, 0ll);
+            A.cont_rows[3 * i] = 0, A.cont_rows[3 * i + 1] = x, A.cont_rows[3 * i + 2] = x;
+        }
+        atomicAdd(A.stats, n);
+        if (!last && (pending || (MODE != kModeOverlap && s > fed_after - t_after))) atomicAdd(A.stats + 1, 1ull);
+    }
+}
+
+// released row k of stream i: overlapping rows are read from the lists directly, the others from the staging area
+__device__ __forceinline__ SelRec stream_row(const StreamArgs &A, int64_t i, const StreamView &v, long long k) {
+    if (A.mode == kModeOverlap) return sel_rec(&v, (unsigned long long)k);
+    const long long *src = A.staged + 4 * (A.seam_mo[i] + A.chunk_mo[i]);
+    return {src[4 * k + 1], src[4 * k + 2], src[4 * k + 3]};
+}
+
+// Byte offsets: every released row packed at its place in rows[], grid-stride over all rows (a stream with millions of
+// rows is spread over the whole grid); the stream of row g is found by a binary search in row_offsets.  Runs before
+// stream_emit_kernel, which updates the carry these rows are placed with.
+__global__ void stream_rows_kernel(StreamArgs A) {
+    const int64_t n = A.B.n_haystacks, total = A.row_offsets[n];
+    for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < total; g += (int64_t)gridDim.x * blockDim.x) {
+        int64_t i = 0, hi = n - 1;  // the last stream whose rows start at or before g: its rows hold g
+        while (i < hi) {
+            const int64_t mid = (i + hi + 1) >> 1;
+            if (A.row_offsets[mid] <= g)
+                i = mid;
+            else
+                hi = mid - 1;
+        }
+        StreamView v;
+        if (A.mode == kModeOverlap) stream_view(A, i, v);
+        const SelRec m = stream_row(A, i, v, g - A.row_offsets[i]);
+        long long *dst = A.rows + 4 * g;
+        dst[0] = i, dst[1] = m.pid, dst[2] = m.start, dst[3] = m.end;
+    }
+}
+
+// One warp per stream: code points only, the rows packed at row_offsets[i] with positions lowered by the continuation
+// bytes before them, counted from the tail on; then, for every stream, the carry: the new tail, the data fed and the
+// continuation bytes before the new tail; zero for a stream that ends with this feed.
+__global__ void stream_emit_kernel(StreamArgs A) {
+    const uint32_t lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < A.B.n_haystacks; i += warps) {
+        int64_t *c = A.carry + kCarryWords * i;
+        const long long fed = c[kCarryFed], t = c[kCarryTail], cont = c[kCarryCont];
+        const long long len = A.B.offsets[i + 1] - A.B.offsets[i];
+        const uint8_t *seam = A.seam + A.seam_offsets[i], *chunk = A.B.bytes + A.B.offsets[i];
+        // byte k of tail || chunk
+        auto byte_at = [&](long long k) -> uint32_t { return k < t ? seam[k] : chunk[k - t]; };
+        auto count_cont = [&](long long a, long long b) -> long long {  // continuation bytes of tail || chunk in [a, b)
+            unsigned long long m = 0;
+            for (long long k = a + lane; k < b; k += 32) m += is_cont_byte(byte_at(k));
+            for (int d = 16; d >= 1; d >>= 1) m += __shfl_xor_sync(0xffffffffu, m, d);
+            return (long long)m;
+        };
+        if (A.codepoints) {
+            StreamView v;
+            if (A.mode == kModeOverlap) stream_view(A, i, v);
+            long long *dst = A.rows + 4 * A.row_offsets[i];
+            const long long k_rows = A.row_offsets[i + 1] - A.row_offsets[i];
+            const long long tail_start = fed - t;
+            // rows are in order of end: the count runs forward once
+            long long at = 0, seen = cont;
+            for (long long k = 0; k < k_rows; k++) {
+                const SelRec m = stream_row(A, i, v, k);
+                const long long end = m.end - tail_start;
+                seen += count_cont(at, end);
+                at = end;
+                if (lane == 0) {
+                    const long long end_cp = tail_start + end - seen;
+                    dst[4 * k] = i, dst[4 * k + 1] = m.pid, dst[4 * k + 2] = end_cp - (long long)A.pat_cplen[m.pid], dst[4 * k + 3] = end_cp;
+                }
+            }
+        }
+        const bool last = A.last && A.last[i];
+        const long long fed_after = fed + len, t_after = last ? 0 : min(fed_after, (long long)A.halo);
+        // the new tail: the last t_after bytes of tail || chunk (read from the seam and the chunk, never the old tail)
+        const long long from = t + len - t_after;
+        uint8_t *tail = A.tail + (uint64_t)i * A.halo;
+        for (long long k = lane; k < t_after; k += 32) tail[k] = (uint8_t)byte_at(from + k);
+        long long cont_after = 0;
+        if (A.codepoints && !last) {
+            const long long x = A.cont_rows[3 * i + 1];  // chunk bytes before the new tail: counted on the whole grid
+            cont_after = cont + count_cont(0, min(from, t)) + (x - A.cont_cp[3 * i + 1]);
+        }
+        __syncwarp();
+        if (lane == 0) {
+            c[kCarryFed] = last ? 0 : fed_after;
+            c[kCarryTail] = t_after;
+            c[kCarryCont] = cont_after;
+            if (last) c[kCarryRestart] = 0;
+        }
+    }
+}
+
 }  // namespace acb
 
 // ===========================================================================
@@ -2075,6 +2319,111 @@ int acb_scan_batch(const acb_automaton *a, const void *dev_image, const void *de
     rc = ACB_DISPATCH(launch_epilogue, E, d, st);
 #undef ACB_DISPATCH
     if (rc) return rc;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+int acb_stream_seams(const acb_automaton *a, const uint8_t *dev_bytes, const int64_t *dev_offsets, int64_t n_streams, uint64_t total_bytes,
+                     const int64_t *dev_carry, const uint8_t *dev_tail, uint8_t *dev_seam_bytes, int64_t *dev_seam_offsets, void *stream) {
+    if (!a || !dev_offsets || !dev_carry || !dev_seam_offsets || (total_bytes && !dev_bytes)) return fail(ACB_EINVAL, "null argument");
+    const uint32_t halo = a->impl->hdr.max_pat_len ? a->impl->hdr.max_pat_len - 1 : 0;
+    if (halo && (!dev_tail || !dev_seam_bytes)) return fail(ACB_EINVAL, "null argument");
+    if (n_streams < 0 || n_streams > 0xfffffffell) return fail(ACB_EINVAL, "n_streams out of range (0 .. 2^32 - 2)");
+    if (total_bytes >= (1ull << 31)) return fail(ACB_EINVAL, "total_bytes must be below 2^31 (feed larger data in more chunks)");
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (n_streams == 0) {
+        CUDA_OK(cudaMemsetAsync(dev_seam_offsets, 0, sizeof(int64_t), st));
+        return ACB_OK;
+    }
+    int64_t blocks = (n_streams + 255) / 256;
+    if (blocks > 8ll * d.sms) blocks = 8ll * d.sms;
+    stream_seam_lengths_kernel<<<(unsigned)blocks, 256, 0, st>>>(dev_offsets, n_streams, dev_carry, halo, dev_seam_offsets);
+    stream_prefix_kernel<<<1, kScanThreads, 0, st>>>(dev_seam_offsets, n_streams);
+    int64_t fill_blocks = (n_streams + 7) / 8;  // a warp per stream
+    if (fill_blocks > 16ll * d.sms) fill_blocks = 16ll * d.sms;
+    if (halo)
+        stream_seam_fill_kernel<<<(unsigned)fill_blocks, 256, 0, st>>>(dev_bytes, dev_offsets, n_streams, dev_carry, dev_tail, halo,
+                                                                       dev_seam_offsets, dev_seam_bytes);
+    g_launches += halo ? 3 : 2;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+int acb_stream_resolve(const acb_automaton *a, const void *dev_image, const uint8_t *dev_bytes, const int64_t *dev_offsets, int64_t n_streams,
+                       uint64_t total_bytes, const uint8_t *dev_last, int overlapping, int codepoints, int64_t *dev_carry, uint8_t *dev_tail,
+                       const uint8_t *dev_seam_bytes, const int64_t *dev_seam_offsets, const acb_match *dev_seam_list,
+                       const uint64_t *dev_seam_match_offsets, const acb_match *dev_chunk_list, const uint64_t *dev_chunk_match_offsets,
+                       int64_t *dev_scratch, int64_t *dev_rows, int64_t *dev_row_offsets, void *stream) {
+    if (!a || !dev_offsets || !dev_carry || !dev_seam_offsets || !dev_seam_list || !dev_seam_match_offsets || !dev_chunk_list ||
+        !dev_chunk_match_offsets || !dev_scratch || !dev_rows || !dev_row_offsets || (total_bytes && !dev_bytes))
+        return fail(ACB_EINVAL, "null argument");
+    const ImageHeader &h = a->impl->hdr;
+    const int kind = (int)h.match_kind;
+    if (overlapping != 0 && overlapping != 1) return fail(ACB_EINVAL, "overlapping must be 0 or 1");
+    if (overlapping && kind != ACB_STANDARD)
+        return fail(ACB_EUNSUPPORTED, std::string("match kind ") + (kind == ACB_LEFTMOST_FIRST ? "LeftmostFirst" : "LeftmostLongest") +
+                                          " does not support overlapping searches");
+    const uint32_t halo = h.max_pat_len ? h.max_pat_len - 1 : 0;
+    if (halo && (!dev_tail || !dev_seam_bytes)) return fail(ACB_EINVAL, "null argument");
+    if (codepoints && !dev_image) return fail(ACB_EINVAL, "code points need the device image (pattern lengths in code points)");
+    if (n_streams < 0 || n_streams > 0xfffffffell) return fail(ACB_EINVAL, "n_streams out of range (0 .. 2^32 - 2)");
+    if (total_bytes >= (1ull << 31)) return fail(ACB_EINVAL, "total_bytes must be below 2^31 (feed larger data in more chunks)");
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CUDA_OK(cudaMemsetAsync(dev_scratch, 0, 2 * sizeof(uint64_t), st));
+    if (n_streams == 0) {
+        CUDA_OK(cudaMemsetAsync(dev_row_offsets, 0, sizeof(int64_t), st));
+        return ACB_OK;
+    }
+    StreamArgs A;
+    A.B = Batch{dev_bytes, dev_offsets, n_streams};
+    A.carry = dev_carry;
+    A.tail = dev_tail;
+    A.last = dev_last;
+    A.seam = dev_seam_bytes;
+    A.seam_offsets = dev_seam_offsets;
+    A.seam_list = reinterpret_cast<const uint4 *>(dev_seam_list);
+    A.chunk_list = reinterpret_cast<const uint4 *>(dev_chunk_list);
+    A.seam_mo = reinterpret_cast<const unsigned long long *>(dev_seam_match_offsets);
+    A.chunk_mo = reinterpret_cast<const unsigned long long *>(dev_chunk_match_offsets);
+    A.stats = reinterpret_cast<unsigned long long *>(dev_scratch);
+    A.cont_rows = reinterpret_cast<long long *>(dev_scratch + 2);
+    A.cont_cp = reinterpret_cast<long long *>(dev_scratch + 2 + 3 * n_streams);
+    A.staged = reinterpret_cast<long long *>(dev_scratch + 2 + 6 * n_streams);
+    A.row_offsets = dev_row_offsets;
+    A.rows = reinterpret_cast<long long *>(dev_rows);
+    A.pat_cplen = codepoints ? make_view(h, dev_image).pat_cplen : nullptr;
+    A.halo = halo;
+    A.mode = overlapping ? kModeOverlap : (kind == ACB_STANDARD ? kModeStandard : kModeLeftmost);
+    A.longest = kind == ACB_LEFTMOST_LONGEST ? 1 : 0;
+    A.codepoints = codepoints ? 1 : 0;
+    int64_t blocks = (n_streams + 127) / 128;
+    if (blocks > 16ll * d.sms) blocks = 16ll * d.sms;
+    if (A.mode == kModeOverlap)
+        stream_select_kernel<kModeOverlap><<<(unsigned)blocks, 128, 0, st>>>(A);
+    else if (A.mode == kModeStandard)
+        stream_select_kernel<kModeStandard><<<(unsigned)blocks, 128, 0, st>>>(A);
+    else
+        stream_select_kernel<kModeLeftmost><<<(unsigned)blocks, 128, 0, st>>>(A);
+    stream_prefix_kernel<<<1, kScanThreads, 0, st>>>(dev_row_offsets, n_streams);
+    g_launches += 2;
+    CUDA_OK(cudaGetLastError());
+    if (codepoints) {  // continuation bytes of each chunk before its new tail, counted on the whole grid
+        if (int rc = acb_rows_to_codepoints(dev_bytes, dev_offsets, n_streams, total_bytes, reinterpret_cast<const int64_t *>(A.cont_rows),
+                                            reinterpret_cast<int64_t *>(A.cont_cp), stream))
+            return rc;
+    }
+    if (!codepoints) {  // the row count is on the device only: a grid of 8 blocks per SM, grid-stride over the rows
+        stream_rows_kernel<<<(unsigned)(8 * d.sms), 256, 0, st>>>(A);
+        g_launches++;
+    }
+    int64_t emit_blocks = (n_streams + 7) / 8;  // a warp per stream
+    if (emit_blocks > 16ll * d.sms) emit_blocks = 16ll * d.sms;
+    stream_emit_kernel<<<(unsigned)emit_blocks, 256, 0, st>>>(A);
+    g_launches++;
     CUDA_OK(cudaGetLastError());
     return ACB_OK;
 }

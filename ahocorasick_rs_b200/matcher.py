@@ -1190,6 +1190,171 @@ class _Automaton:
             return self.scan_host(host[:total_bytes], offs, overlapping, codepoints)
 
 
+class StreamBatch:
+    """A batch of streams on one device: data that arrives in chunks, searched across the chunk boundaries.  Stream i is
+    the concatenation of the chunks fed to slot i; positions are absolute within it (int64), byte offsets, or code
+    point indexes for the str class.  The rows a stream releases over all its feeds, in order, are exactly
+    find_matches_as_indexes(concatenation, overlapping).  After a feed that brings a stream to F bytes, the rows
+    released are those of that result with end <= F (Standard), or start + max_pattern_len <= F (the leftmost kinds:
+    no later match can start before them).  The carry of every stream lives on the device (acb_stream_seams /
+    acb_stream_resolve in include/acb200.h); a feed runs the sieve on the chunks as they are, never copying them."""
+
+    _serial = __import__("itertools").count()
+
+    def __init__(self, ac: "_Automaton", n_streams: int, overlapping: bool, codepoints: bool):
+        if isinstance(n_streams, bool) or not isinstance(n_streams, int):
+            raise TypeError("n_streams must be an int")
+        if n_streams < 0 or n_streams > 0xFFFF_FFFE:
+            raise ValueError("n_streams out of range (0 .. 2^32 - 2)")
+        ac.check_overlapping(overlapping)
+        halo = max(ac.max_pattern_len - 1, 0)
+        if 2 * n_streams * halo > ac.WINDOW_BYTES:
+            # the seams (tail || head, up to 2 * (max_pattern_len - 1) bytes per stream) are scanned in one call
+            raise ValueError(f"{n_streams} streams x 2 x (max_pattern_len - 1) = {2 * n_streams * halo} seam bytes: one feed's seams "
+                             f"must fit {ac.WINDOW_BYTES} bytes (WINDOW_BYTES); use fewer streams per batch")
+        self._ac = ac
+        self.n_streams = n_streams
+        self.overlapping = bool(overlapping)
+        self._codepoints = codepoints
+        self.device = None     # the device of the first feed: the carry is allocated there
+        self._halo = max(ac.max_pattern_len - 1, 0)
+        # two workspaces of the automaton that only this batch scans with: the lists they hold are read by the resolve
+        k = next(StreamBatch._serial)
+        self._slots = (("stream", k, 0), ("stream", k, 1))
+        self._lock = threading.Lock()
+        self.last_stats = {}
+
+    def _allocate(self, dev):
+        torch = _torch()
+        n = self.n_streams
+        self.device = dev
+        self._carry = torch.zeros((n, 4), dtype=torch.int64, device=dev)   # acb_stream_resolve's carry words
+        self._tail = torch.zeros(max(n * self._halo, 1), dtype=torch.uint8, device=dev)
+        self._seam = torch.empty(max(2 * n * self._halo, 1), dtype=torch.uint8, device=dev)
+        self._seam_offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
+
+    def __del__(self):
+        ac, slots = getattr(self, "_ac", None), getattr(self, "_slots", ())
+        if ac is not None:
+            for key in [key for key in list(ac._ws) if key[1] in slots]:
+                ac._ws.pop(key, None)
+
+    def feed_device(self, data, offsets, last=None):
+        """One chunk per stream: chunk i = data[offsets[i]:offsets[i + 1]] (uint8 CUDA tensor, int64 CUDA tensor
+        (n_streams + 1); an empty chunk is allowed).  `last`: None, or a bool CUDA tensor (n_streams,) -- those streams
+        end with this feed, release everything and start again at position 0.  Returns (rows int64 (k, 4) = (stream,
+        pattern, start, end), row_offsets int64 (n_streams + 1)), the rows of stream i at row_offsets[i]:row_offsets[i+1]."""
+        torch = _torch()
+        ac, n = self._ac, self.n_streams
+        if not torch.is_tensor(data) or data.dtype != torch.uint8 or data.dim() != 1 or data.device.type != "cuda":
+            raise TypeError("data must be a 1-D uint8 CUDA tensor")
+        dev = self.device or data.device
+        if data.device != dev:
+            raise TypeError(f"data must be on {dev}, where this batch's streams live")
+        if not torch.is_tensor(offsets) or offsets.dtype != torch.int64 or offsets.shape != (n + 1,) or offsets.device != dev:
+            raise TypeError(f"offsets must be an int64 tensor of shape ({n + 1},) on {dev}")
+        if last is not None and (not torch.is_tensor(last) or last.dtype != torch.bool or last.shape != (n,) or last.device != dev):
+            raise TypeError(f"last must be None or a bool tensor of shape ({n},) on {dev}")
+        if data.numel() > ac.WINDOW_BYTES:
+            raise ValueError(f"one feed addresses at most {ac.WINDOW_BYTES} bytes (WINDOW_BYTES): feed larger data in more chunks")
+        _require_cuda()
+        data, offsets = data.contiguous(), offsets.contiguous()
+        last_u8 = last.contiguous().view(torch.uint8) if last is not None else None
+        L = ac._L
+        with self._lock, torch.cuda.device(dev):
+            if self.device is None:
+                self._allocate(dev)
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            rc = L.acb_stream_seams(ac._h, data.data_ptr(), offsets.data_ptr(), n, data.numel(), self._carry.data_ptr(),
+                                    self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(), stream)
+            if rc != _capi.ACB_OK:
+                raise RuntimeError(_capi.last_error())
+            # the overlapping lists, in bytes, of the chunks as they are and of the seams
+            m_c, mo_c, tot_c = ac.scan_device(data, offsets, 2, False, ws_slot=self._slots[0])
+            geometry = {k: ac.last_stats.get(k) for k in ("window", "last_level", "probes", "bloom_bytes", "ring", "task_bytes")}
+            m_s, mo_s, tot_s = ac.scan_device(self._seam, self._seam_offsets, 2, False, ws_slot=self._slots[1])
+            if m_c.dtype != torch.int32 or m_s.dtype != torch.int32:   # (both buffers are below WINDOW_BYTES: one call each)
+                raise RuntimeError("stream search: a list came back in the windowed int64 form acb_stream_resolve cannot read")
+            cap = int(tot_c) + int(tot_s)
+
+            def ptr(t):   # an empty list is still a view of its workspace's buffer: pass that buffer's (non-null) address
+                return t.data_ptr() if t.numel() else t.untyped_storage().data_ptr() + t.storage_offset() * t.element_size()
+
+            # the staging area of the selected rows (4 words per record) is not used by an overlapping search
+            scratch = torch.empty(2 + 6 * n + (0 if self.overlapping else 4 * cap), dtype=torch.int64, device=dev)
+            rows = torch.empty((max(cap, 1), 4), dtype=torch.int64, device=dev)
+            row_offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
+            rc = L.acb_stream_resolve(ac._h, ac.image(dev).data_ptr() if self._codepoints else None, data.data_ptr(), offsets.data_ptr(), n,
+                                      data.numel(), last_u8.data_ptr() if last_u8 is not None else None, int(self.overlapping),
+                                      int(self._codepoints), self._carry.data_ptr(), self._tail.data_ptr(), self._seam.data_ptr(),
+                                      self._seam_offsets.data_ptr(), ptr(m_s), mo_s.data_ptr(), ptr(m_c), mo_c.data_ptr(),
+                                      scratch.data_ptr(), rows.data_ptr(), row_offsets.data_ptr(), stream)
+            if rc != _capi.ACB_OK:
+                raise (ValueError if rc == _capi.ACB_EUNSUPPORTED else RuntimeError)(_capi.last_error())
+            k = int(row_offsets[n].item())
+            records, held = scratch[:2].tolist()
+        self.last_stats = {"engine": "sieve", "mode": "stream", **geometry, "seam_bytes": int(self._seam_offsets[n].item()),
+                           "records": records, "released": k, "held": held}
+        ac.last_stats = dict(self.last_stats)
+        return rows[:k], row_offsets
+
+
+class Stream:
+    """One stream fed from the host: a StreamBatch of one, with its own pinned staging buffer for the chunks (so a feed
+    does not wait for the automaton's other host-staged calls, nor they for it)."""
+
+    def __init__(self, ac: "_Automaton", overlapping: bool, codepoints: bool):
+        self._batch = StreamBatch(ac, 1, overlapping, codepoints)
+        self._ac = ac
+        self._codepoints = codepoints
+        self._offs = None
+        self._pinned = None
+        self._lock = threading.Lock()
+        self._done = False
+
+    @property
+    def last_stats(self):
+        return self._batch.last_stats
+
+    def feed(self, chunk):
+        """The next chunk (a str for AhoCorasick, a bytes-like object for BytesAhoCorasick) -> the rows
+        [(pattern, start, end), ...] this feed releases."""
+        if self._codepoints:
+            if not isinstance(chunk, str):
+                raise TypeError("argument 'chunk': 'str' expected")
+            return self._feed(chunk.encode("utf-8"), False)
+        return self._feed(_as_buffer_bytes(chunk), False)
+
+    def _feed(self, chunk, last: bool):
+        torch = _torch()
+        if self._done:
+            raise RuntimeError("the stream is finished: feed after finish()")
+        n = len(chunk)
+        if n > self._ac.WINDOW_BYTES:
+            raise ValueError(f"one feed addresses at most {self._ac.WINDOW_BYTES} bytes (WINDOW_BYTES): feed larger data in more chunks")
+        torch = _require_cuda()
+        dev = self._batch.device or torch.device("cuda", torch.cuda.current_device())
+        if self._offs is None:
+            self._offs = torch.zeros(2, dtype=torch.int64, device=dev)
+        with self._lock:   # the staging buffer is reused once the feed has synchronised (feed_device reads its row count)
+            if self._pinned is None or self._pinned.numel() < n:
+                self._pinned = torch.empty(max(n, 1 << 16), dtype=torch.uint8, pin_memory=True)
+            host = self._pinned
+            if n:
+                host.numpy()[:n] = np.frombuffer(chunk, dtype=np.uint8)
+            d = host[:n].to(dev, non_blocking=True)
+            self._offs[1] = n
+            rows, _ = self._batch.feed_device(d, self._offs, torch.ones(1, dtype=torch.bool, device=dev) if last else None)
+            rows = rows.cpu().numpy()
+        if last:
+            self._done = True
+        return list(zip(rows[:, 1].tolist(), rows[:, 2].tolist(), rows[:, 3].tolist()))
+
+    def finish(self):
+        """The rows still held; ends the stream."""
+        return self._feed(b"", True)
+
+
 def _as_buffer_bytes(obj) -> bytes:
     """reference PyBufferBytes::try_from (src/lib.rs:281-302): 1-D, C-contiguous u8 buffer."""
     if isinstance(obj, str):
@@ -1349,6 +1514,19 @@ class AhoCorasick:
         """Device-resident UTF-8 batch -> int64 tensor (n,) of match counts (see _Automaton.count_device)."""
         return self._ac.count_device(data, offsets, overlapping)
 
+    # ---- additions: stream search (data fed in chunks; the crate's stream_find_iter, for every match kind) -------------
+    def stream(self, overlapping: bool = False) -> Stream:
+        """One stream fed ``str`` chunks: ``feed(chunk)`` returns the rows (pattern, start, end) it releases, in code
+        points of the whole stream; ``finish()`` returns the rest.  All feeds together give
+        ``find_matches_as_indexes(concatenation, overlapping)`` (see StreamBatch for when a row is released)."""
+        self._ac.check_overlapping(overlapping)
+        return Stream(self._ac, overlapping, codepoints=True)
+
+    def stream_batch(self, n_streams: int, overlapping: bool = False) -> StreamBatch:
+        """``n_streams`` streams fed from the device: ``feed_device(data, offsets, last=None)`` takes one UTF-8 chunk per
+        stream (it may cut a character); positions are code point indexes (see StreamBatch)."""
+        return StreamBatch(self._ac, n_streams, overlapping, codepoints=True)
+
     def scan_host(self, data, offsets, overlapping: bool = False, **kw):
         """Host-resident UTF-8 batch (uint8 array + int64 offsets) -> host arrays (matches (k, 4), match_offsets (n + 1));
         code point indexes.  Copies and scans are pipelined (see _Automaton.scan_host)."""
@@ -1434,6 +1612,19 @@ class BytesAhoCorasick:
     def count_matches_device(self, data, offsets, overlapping: bool = False):
         """Device-resident batch -> int64 tensor (n,) of match counts (see _Automaton.count_device)."""
         return self._ac.count_device(data, offsets, overlapping)
+
+    # ---- additions: stream search (data fed in chunks; the crate's stream_find_iter, for every match kind) -------------
+    def stream(self, overlapping: bool = False) -> Stream:
+        """One stream fed bytes-like chunks: ``feed(chunk)`` returns the rows (pattern, start, end) it releases, in byte
+        offsets of the whole stream; ``finish()`` returns the rest.  All feeds together give
+        ``find_matches_as_indexes(concatenation, overlapping)`` (see StreamBatch for when a row is released)."""
+        self._ac.check_overlapping(overlapping)
+        return Stream(self._ac, overlapping, codepoints=False)
+
+    def stream_batch(self, n_streams: int, overlapping: bool = False) -> StreamBatch:
+        """``n_streams`` streams fed from the device: ``feed_device(data, offsets, last=None)`` takes one chunk per
+        stream; positions are byte offsets (see StreamBatch)."""
+        return StreamBatch(self._ac, n_streams, overlapping, codepoints=False)
 
     def scan_host(self, data, offsets, overlapping: bool = False, **kw):
         """Host-resident batch (uint8 array + int64 offsets) -> host arrays (matches (k, 4), match_offsets (n + 1));

@@ -344,6 +344,62 @@ int acb_count_rows(const acb_automaton *a, const int64_t *dev_rows, uint64_t n_r
                    void *stream);
 
 /*
+ * Stream search: matches in data that arrives in chunks, for many streams at once.  A stream is the concatenation of
+ * the chunks fed to it; positions are absolute within it and 64-bit.  The crate the reference wraps has the single-stream,
+ * Standard, non-overlapping form (AhoCorasick::stream_find_iter); here every match kind and overlapping Standard are
+ * served, and the rows a stream releases over all its feeds are exactly the one-shot result on the concatenation
+ * (get_matches, src/lib.rs:42-68), in the reference's order.  A feed gives each stream one chunk (maybe empty) of a
+ * device-resident batch: chunk i = dev_bytes[dev_offsets[i] .. dev_offsets[i + 1]); total_bytes = length of the dev_bytes
+ * buffer, below 2^31.
+ *
+ * Release rule, in bytes whatever the positions are reported in: after a feed that brings a stream to F bytes, the rows
+ * it has released are the rows of the one-shot result with end <= F (Standard, overlapping or not), or with
+ * start + max_pattern_len <= F (LeftmostFirst, LeftmostLongest: no later match can start before such a row).  A feed
+ * that ends a stream (dev_last[i] != 0) releases the rest and leaves its carry zero: the slot starts a new stream.
+ *
+ * The caller owns the state of each stream, zero-filled before its first feed (halo = acb_max_pattern_len - 1):
+ *   dev_carry = int64[n_streams][4]: [0] bytes fed so far F, [1] the restart point of the non-overlapping selection
+ *     (absolute byte offset), [2] tail length T = min(F, halo), [3] UTF-8 continuation bytes before the tail's start
+ *     (kept when codepoints != 0, else 0);
+ *   dev_tail = uint8[n_streams][halo]: stream i's last T bytes at dev_tail + i * halo (may be null when halo == 0).
+ *
+ * A feed is four calls on one CUDA stream:
+ *   1. acb_stream_seams writes each stream's seam -- its tail, then the chunk's first min(chunk length, halo) bytes --
+ *      packed into dev_seam_bytes (room for n_streams * 2 * halo bytes; may be null when halo == 0), and
+ *      dev_seam_offsets = int64[n_streams + 1] brackets them: a batch of n_streams haystacks.  Three launches.
+ *   2. acb_scan_batch with overlapping = 2, codepoints = 0 (the overlapping list of any automaton, in bytes) on the
+ *      chunks (dev_bytes, dev_offsets) as they are, and
+ *   3. the same on the seams (dev_seam_bytes, dev_seam_offsets), each with its own workspace: both lists are read in 4.
+ *   4. acb_stream_resolve merges, per stream, its seam's records with its chunk's records that end past the seam (every
+ *      match ending in the chunk starts at most halo bytes before it, so it lies in tail || chunk), continues the
+ *      selection from the carried restart point (one thread per stream: the selection is a chain), and writes
+ *      dev_rows = int64[k][4] = (stream, pattern, start, end), grouped by stream in the reference's order, and
+ *      dev_row_offsets = int64[n_streams + 1] bracketing each stream's rows (k = dev_row_offsets[n_streams]).  With
+ *      codepoints != 0 (UTF-8 data, chunks may be cut inside a character) start and end are code point indexes: the
+ *      byte offset minus the continuation bytes before it in the stream; it needs dev_image (pattern lengths in code
+ *      points).  Then it updates the carry and the tail.  dev_seam_list / dev_chunk_list and their match offsets are
+ *      ws->dev_out / ws->dev_match_offsets of the scans in 2 and 3.  With R = the two lists' lengths added
+ *      (dev_seam_match_offsets[n] + dev_chunk_match_offsets[n]), dev_rows needs room for R rows and dev_scratch =
+ *      int64[2 + 6 * n_streams + 4 * R] (int64[2 + 6 * n_streams] for overlapping = 1, whose rows are read from the
+ *      lists directly): it leaves [0] = list records the selection considered, [1] = streams holding something back
+ *      (a leftmost pick not yet released, or a restart point past the new tail's start).  dev_last = uint8[n_streams]
+ *      or null (no stream ends).  A memset and four kernel launches (select, prefix, rows, carry); with code points
+ *      the rows are written by the carry kernel and acb_rows_to_codepoints' copy and launch replace the rows kernel.
+ *      No synchronisation.
+ *
+ * Both return ACB_EINVAL, before any CUDA call, for a null pointer (dev_bytes may be null when total_bytes == 0),
+ * n_streams outside [0, 2^32 - 2], total_bytes >= 2^31, overlapping other than 0 / 1 or codepoints without dev_image;
+ * acb_stream_resolve returns ACB_EUNSUPPORTED for overlapping = 1 on a leftmost automaton, like the reference.
+ */
+int acb_stream_seams(const acb_automaton *a, const uint8_t *dev_bytes, const int64_t *dev_offsets, int64_t n_streams, uint64_t total_bytes,
+                     const int64_t *dev_carry, const uint8_t *dev_tail, uint8_t *dev_seam_bytes, int64_t *dev_seam_offsets, void *stream);
+int acb_stream_resolve(const acb_automaton *a, const void *dev_image, const uint8_t *dev_bytes, const int64_t *dev_offsets, int64_t n_streams,
+                       uint64_t total_bytes, const uint8_t *dev_last, int overlapping, int codepoints, int64_t *dev_carry, uint8_t *dev_tail,
+                       const uint8_t *dev_seam_bytes, const int64_t *dev_seam_offsets, const acb_match *dev_seam_list,
+                       const uint64_t *dev_seam_match_offsets, const acb_match *dev_chunk_list, const uint64_t *dev_chunk_match_offsets,
+                       int64_t *dev_scratch, int64_t *dev_rows, int64_t *dev_row_offsets, void *stream);
+
+/*
  * Multi-GPU: the fixed-size block a rank contributes to the gather of the per-shard match lists (the only exchange
  * of the sharded path; NCCL all-gather over NVLink).  dev_block holds (cap + 1) records of 16 bytes: record 0 =
  * (match count, hay_base, complete flag, 0), then the first `cap` matches of a finished scan (dev_total / dev_out of
