@@ -757,6 +757,28 @@ __device__ __forceinline__ void block_add(unsigned long long *dst, unsigned long
     if ((threadIdx.x & 31) == 0 && v) atomicAdd(dst, v);
 }
 
+// one past the last record of the stretch (the records of one haystack) that starts at list[i]: galloping, then binary
+// search (a long stretch is not walked by one thread)
+__device__ __forceinline__ unsigned long long stretch_end(const acb_match *list, unsigned long long i, unsigned long long avail) {
+    const uint32_t hc = list[i].haystack;
+    unsigned long long a = i + 1, step = 1;  // list[a - 1] is in the stretch
+    for (;;) {
+        const unsigned long long b = a + step - 1;
+        if (b >= avail || list[b].haystack != hc) break;
+        a = b + 1;
+        step <<= 1;
+    }
+    unsigned long long hi = a + step - 1 < avail ? a + step - 1 : avail;
+    while (a < hi) {
+        const unsigned long long mid = (a + hi) >> 1;
+        if (list[mid].haystack == hc)
+            a = mid + 1;
+        else
+            hi = mid;
+    }
+    return a;
+}
+
 // The count variant of sieve_epilogue_kernel (MODE kModeStandard / kModeLeftmost, no code points): phases 1-3 place
 // the overlapping list (from E.raw = dev_raw into E.ordered = dev_out), phase 4 counts each haystack's selection
 // without packing it, straight into counts[h].  Stretches longer than ACB_LONG_STRETCH are counted by the whole grid
@@ -797,22 +819,7 @@ __global__ void __launch_bounds__(kScanThreads) sieve_count_epilogue_kernel(Siev
     for (unsigned long long i = first_i; i < avail; i += stride) {
         const uint32_t hc = list[i].haystack;
         if (i && list[i - 1].haystack == hc) continue;
-        // the stretch's end: galloping, then binary search (a long stretch is not walked by one thread)
-        unsigned long long a = i + 1, step = 1;  // list[a - 1] is in the stretch
-        for (;;) {
-            const unsigned long long b = a + step - 1;
-            if (b >= avail || list[b].haystack != hc) break;
-            a = b + 1;
-            step <<= 1;
-        }
-        unsigned long long hi = a + step - 1 < avail ? a + step - 1 : avail;
-        while (a < hi) {
-            const unsigned long long mid = (a + hi) >> 1;
-            if (list[mid].haystack == hc)
-                a = mid + 1;
-            else
-                hi = mid;
-        }
+        const unsigned long long a = stretch_end(list, i, avail);
         const unsigned long long len = a - i;
         if (len <= ACB_LONG_STRETCH) {
             const uint32_t c = select_non_overlapping<MODE, false>(const_cast<acb_match *>(list) + i, len, E.max_pat_len, E.longest);
@@ -861,6 +868,105 @@ __global__ void __launch_bounds__(kScanThreads) sieve_count_epilogue_kernel(Siev
         grid.sync();
     }
     finish(true);
+}
+
+// The per-pattern variant of sieve_count_epilogue_kernel (acb_pattern_counts_non_overlapping): phases 1-3 place the
+// overlapping list, then each haystack's selection is found and the pid of every selected record is added to
+// pattern_counts[pid].  A stretch of at most ACB_LONG_STRETCH records is selected by one thread and packed to its front
+// (unit_counts[h] = how many).  A longer one gets successors and pointer jumping as in the count variant, and MARKS its
+// selection, the chain head = NEXT(0), NEXT(head), ...: mark[head] is set before the rounds, and in round k every marked
+// record i also marks its round-k successor J_k(i) = NEXT^(2^k)(i), which it reads anyway.  After round k every NEXT^m(head)
+// with m < 2^(k+1) is marked, so ceil(log2(stretch)) rounds mark the whole chain.  Only chain records are ever marked (the
+// chain is closed under J_k), so a mark another thread sets in the same round and this one already sees only marks a
+// chain record sooner: the race needs no barrier.  The marks live in raw_seq (u32 per record, consumed by phase 3); the
+// pairs' rank words are computed and unused.  A last pass over the list adds the pids of the selected records.
+// totals[0] sums the selected records during the launch, totals[2] = haystacks selected on the grid, totals[5] = the
+// longest such stretch; ws->dev_match_offsets holds each long stretch's end.  Nothing is added when the list did not fit.
+template <int MODE>
+__global__ void __launch_bounds__(kScanThreads) sieve_pattern_epilogue_kernel(SieveEpiArgs E, unsigned long long *pattern_counts) {
+    namespace cg = cooperative_groups;
+    cg::grid_group grid = cg::this_grid();
+    if (blockIdx.x == 0 && threadIdx.x == 0) E.totals[0] = E.totals[2] = E.totals[5] = 0;  // (read and added to only after later barriers)
+    sieve_order_list<false>(E, grid);
+    grid.sync();
+    const unsigned long long list_total = E.totals[6];
+    const unsigned long long raw_total = E.totals[7];
+    const bool complete = list_total <= E.out_cap && raw_total <= E.raw_cap;  // (else the list has holes: nothing is added)
+    if (complete) {
+        const unsigned long long avail = list_total;
+        acb_match *const list = E.ordered;
+        uint4 *const pairs = reinterpret_cast<uint4 *>(const_cast<acb_match *>(E.raw));
+        uint32_t *const mark = const_cast<uint32_t *>(E.raw_seq);
+        unsigned long long *const ends = E.match_offsets;
+        const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+        const unsigned long long first_i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+        // phase 4: the thread that sees a haystack's first record owns its stretch
+        for (unsigned long long i = first_i; i < avail; i += stride) {
+            const uint32_t hc = list[i].haystack;
+            if (i && list[i - 1].haystack == hc) continue;
+            const unsigned long long a = stretch_end(list, i, avail);
+            const unsigned long long len = a - i;
+            E.unit_offsets[hc] = i;
+            if (len <= ACB_LONG_STRETCH) {
+                E.unit_counts[hc] = select_non_overlapping<MODE>(list + i, len, E.max_pat_len, E.longest);
+            } else {
+                E.unit_counts[hc] = kLongMark;
+                ends[hc] = a;
+                // the chain's head, relative, in the second half of the first record's pair until the successors are written
+                pairs[i].z = (uint32_t)next_selected<MODE>(list + i, len, 0, E.max_pat_len, E.longest);
+                atomicAdd(E.totals + 2, 1ull);
+                atomicMax(E.totals + 5, len);
+            }
+        }
+        grid.sync();
+        if (E.totals[2]) {
+            for (unsigned long long i = first_i; i < avail; i += stride) {
+                const uint32_t hc = list[i].haystack;
+                if (E.unit_counts[hc] != kLongMark) continue;
+                const unsigned long long lo = E.unit_offsets[hc], n = ends[hc] - lo;
+                const unsigned long long nx = next_selected<MODE>(list + lo, n, (long long)list[i].end, E.max_pat_len, E.longest);
+                reinterpret_cast<uint2 *>(pairs + i)[0] = make_uint2(nx == n ? kNoNext : (uint32_t)(lo + nx), 1u);
+                mark[i] = i == lo + pairs[lo].z ? 1u : 0u;
+            }
+            grid.sync();
+            const uint32_t rounds = ceil_log2(E.totals[5]);
+            for (uint32_t r = 0; r < rounds; r++) {
+                const int src = (int)(r & 1);
+                for (unsigned long long i = first_i; i < avail; i += stride) {
+                    if (E.unit_counts[list[i].haystack] != kLongMark) continue;
+                    const uint32_t j = src ? pairs[i].z : pairs[i].x;  // J_r(i)
+                    if (j != kNoNext && mark[i]) mark[j] = 1u;
+                    jump_pair(pairs, i, src);
+                }
+                grid.sync();
+            }
+        }
+        // the selected records' pids: whole warps step through the list together, so equal pids of a step add once
+        unsigned long long sum = 0;
+        for (unsigned long long w = first_i & ~31ull; w < avail; w += stride) {
+            const unsigned long long i = w + (threadIdx.x & 31u);
+            bool sel = false;
+            uint32_t pid = 0;
+            if (i < avail) {
+                const uint4 r = reinterpret_cast<const uint4 *>(list)[i];  // haystack, pattern, start, end
+                const uint32_t c = E.unit_counts[r.x];
+                sel = c == kLongMark ? mark[i] != 0 : i - E.unit_offsets[r.x] < c;
+                pid = r.y;
+            }
+            const uint32_t act = __ballot_sync(0xffffffffu, sel);
+            if (sel) add_per_pattern(pattern_counts, act, pid);
+            sum += sel ? 1u : 0u;
+        }
+        block_add(E.totals, sum);
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        if (!complete) E.totals[0] = list_total;  // the caller retries with the room reported
+        E.totals[1] = complete ? 1 : 0;
+        E.totals[3] = E.totals[5] = E.totals[7] = 0;
+        E.totals[4] = raw_total > list_total ? raw_total : list_total;  // room the overlapping list needs
+        E.acc[kAccRaw] = E.acc[kAccGroups] = E.acc[kAccTraps] = E.acc[kAccRepairs] = 0;
+        E.acc[kAccQueue] = 0;
+    }
 }
 
 // acb_count_rows: the same successors and pointer jumping over the rows of ONE haystack (int64, as
@@ -1819,6 +1925,12 @@ int launch_sieve_count_epilogue(SieveEpiArgs &E, unsigned long long *counts, con
     return launch_cooperative(reinterpret_cast<const void *>(sieve_count_epilogue_kernel<MODE>), args, d, st);
 }
 
+template <int MODE>
+int launch_sieve_pattern_epilogue(SieveEpiArgs &E, unsigned long long *pattern_counts, const DeviceInfo &d, cudaStream_t st) {
+    void *args[] = {&E, &pattern_counts};
+    return launch_cooperative(reinterpret_cast<const void *>(sieve_pattern_epilogue_kernel<MODE>), args, d, st);
+}
+
 int sieve_header(const acb_automaton *a, SieveHeader &sh) {
     std::lock_guard<std::mutex> lock(a->impl->sieve_mutex);
     if (a->impl->sieve.size() < sizeof(SieveHeader)) return fail(ACB_EINVAL, "acb_sieve_build has not been called");
@@ -1832,14 +1944,15 @@ int unsupported_overlapping(const acb_automaton *a) {
                                       " does not support overlapping searches");
 }
 
-// acb_any_match (mode kSieveAny, out = u8 flags), acb_find_first (kSieveFirst + kind, out = u64 keys) and
-// acb_count_overlapping (kSieveCount, out = u64 counts): one launch of the sieve kernel in a mode that writes no list
+// acb_any_match (mode kSieveAny, out = u8 flags), acb_find_first (kSieveFirst + kind, out = u64 keys),
+// acb_count_overlapping (kSieveCount, out = u64 counts per haystack) and acb_pattern_counts_overlapping (kSievePatterns,
+// out = u64 counts per pattern): one launch of the sieve kernel in a mode that writes no list
 int sieve_early_scan(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
                      int64_t n_haystacks, uint64_t total_bytes, void *dev_out, uint64_t *dev_scratch, void *stream, int mode) {
     if (!a || !dev_sieve || !dev_offsets || !dev_out || !dev_scratch || (total_bytes && !dev_bytes)) return fail(ACB_EINVAL, "null argument");
     if (n_haystacks < 0 || n_haystacks > 0xfffffffell) return fail(ACB_EINVAL, "n_haystacks out of range (0 .. 2^32 - 2)");
     if (total_bytes >= (1ull << 31)) return fail(ACB_EINVAL, "total_bytes must be below 2^31 (scan larger inputs in windows)");
-    if (mode == kSieveCount && a->impl->hdr.match_kind != ACB_STANDARD) return unsupported_overlapping(a);
+    if ((mode == kSieveCount || mode == kSievePatterns) && a->impl->hdr.match_kind != ACB_STANDARD) return unsupported_overlapping(a);
     SieveHeader sh;
     if (int rc = sieve_header(a, sh)) return rc;
     DeviceInfo d;
@@ -1869,6 +1982,7 @@ int sieve_early_scan(const acb_automaton *a, const void *dev_sieve, const uint8_
         case kSieveFirst + ACB_LEFTMOST_FIRST: rc = launch_sieve<false, kSieveFirst + ACB_LEFTMOST_FIRST>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
         case kSieveFirst + ACB_LEFTMOST_LONGEST: rc = launch_sieve<false, kSieveFirst + ACB_LEFTMOST_LONGEST>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
         case kSieveCount: rc = launch_sieve<false, kSieveCount>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
+        case kSievePatterns: rc = launch_sieve<false, kSievePatterns>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
         default: return fail(ACB_EINVAL, "unknown match kind");
     }
     if (rc) return rc;
@@ -1885,11 +1999,12 @@ int check_ws(const acb_workspace *ws) {
 }
 
 // The sieve's list scan: the scan kernel, then the ordering epilogue -- acb_scan_batch's kernel 5 (counts == null:
-// the list, or its selection, in dev_out) or acb_count_non_overlapping (counts: the count epilogue writes them; the raw
-// records go to dev_raw and are ordered into dev_out, so that dev_raw is free for the count's pairs).
+// the list, or its selection, in dev_out), acb_count_non_overlapping (counts: the count epilogue writes them) or
+// acb_pattern_counts_non_overlapping (counts, by_pattern: the pattern epilogue adds to them).  For both counts the raw
+// records go to dev_raw and are ordered into dev_out, so that dev_raw is free for the pairs.
 int sieve_list_scan(const acb_automaton *a, const void *dev_sieve, const Batch &B, uint64_t total_bytes, int mode, bool cp,
                     const uint32_t *pat_cplen, const acb_plan *plan, const acb_workspace *ws, const DeviceInfo &d, cudaStream_t st,
-                    unsigned long long *counts) {
+                    unsigned long long *counts, bool by_pattern = false) {
     const ImageHeader &h = a->impl->hdr;
     const int kind = (int)h.match_kind;
     const uint8_t *dev_bytes = B.bytes;
@@ -1972,7 +2087,9 @@ int sieve_list_scan(const acb_automaton *a, const void *dev_sieve, const Batch &
     E.totals = totals;
     E.acc = acc;
     E.match_offsets = match_offsets;
-    if (counts)
+    if (counts && by_pattern)
+        rc = mode == kModeStandard ? launch_sieve_pattern_epilogue<kModeStandard>(E, counts, d, st) : launch_sieve_pattern_epilogue<kModeLeftmost>(E, counts, d, st);
+    else if (counts)
         rc = mode == kModeStandard ? launch_sieve_count_epilogue<kModeStandard>(E, counts, d, st) : launch_sieve_count_epilogue<kModeLeftmost>(E, counts, d, st);
     else
         rc = mode == kModeStandard   ? (cp ? launch_sieve_epilogue<kModeStandard, true>(E, d, st) : launch_sieve_epilogue<kModeStandard, false>(E, d, st))
@@ -1981,6 +2098,39 @@ int sieve_list_scan(const acb_automaton *a, const void *dev_sieve, const Batch &
     if (rc) return rc;
     CUDA_OK(cudaGetLastError());
     return ACB_OK;
+}
+
+// acb_count_non_overlapping (by_pattern = false: counts per haystack, written) and acb_pattern_counts_non_overlapping
+// (by_pattern: counts per pattern, added to)
+int non_overlapping_counts(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                           int64_t n_haystacks, uint64_t total_bytes, const acb_plan *plan, const acb_workspace *ws,
+                           uint64_t *dev_counts, void *stream, bool by_pattern) {
+    if (!a || !dev_sieve || !dev_offsets || !plan || !dev_counts || (total_bytes && !dev_bytes)) return fail(ACB_EINVAL, "null argument");
+    if (int rc = check_ws(ws)) return rc;
+    if (n_haystacks < 0 || n_haystacks > 0xfffffffell) return fail(ACB_EINVAL, "n_haystacks out of range (0 .. 2^32 - 2)");
+    if (total_bytes >= (1ull << 31)) return fail(ACB_EINVAL, "total_bytes must be below 2^31 (scan larger inputs in windows)");
+    acb_plan want;
+    acb_plan_scan(a, dev_bytes, total_bytes, (uint64_t)n_haystacks, &want);
+    if (want.n_segments != plan->n_segments || want.segment_bytes != plan->segment_bytes || want.n_units != plan->n_units ||
+        want.task_bytes != plan->task_bytes)
+        return fail(ACB_EINVAL, "plan does not match the arguments (call acb_plan_scan again)");
+    SieveHeader sh;
+    if (int rc = sieve_header(a, sh)) return rc;
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (n_haystacks == 0 || total_bytes == 0) {
+        if (n_haystacks && !by_pattern) CUDA_OK(cudaMemsetAsync(dev_counts, 0, (uint64_t)n_haystacks * sizeof(uint64_t), st));
+        zero_outputs_kernel<<<(unsigned)((n_haystacks + 256) / 256), 256, 0, st>>>(
+            reinterpret_cast<unsigned long long *>(ws->dev_unit_offsets), reinterpret_cast<unsigned long long *>(ws->dev_match_offsets),
+            n_haystacks, reinterpret_cast<unsigned long long *>(ws->dev_total));
+        g_launches++;
+        CUDA_OK(cudaGetLastError());
+        return ACB_OK;
+    }
+    const int mode = a->impl->hdr.match_kind == ACB_STANDARD ? kModeStandard : kModeLeftmost;
+    return sieve_list_scan(a, dev_sieve, Batch{dev_bytes, dev_offsets, n_haystacks}, total_bytes, mode, false, nullptr, plan, ws, d, st,
+                           reinterpret_cast<unsigned long long *>(dev_counts), by_pattern);
 }
 
 }  // namespace
@@ -2042,32 +2192,21 @@ int acb_count_overlapping(const acb_automaton *a, const void *dev_sieve, const u
 int acb_count_non_overlapping(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
                               int64_t n_haystacks, uint64_t total_bytes, const acb_plan *plan, const acb_workspace *ws,
                               uint64_t *dev_counts, void *stream) {
-    if (!a || !dev_sieve || !dev_offsets || !plan || !dev_counts || (total_bytes && !dev_bytes)) return fail(ACB_EINVAL, "null argument");
-    if (int rc = check_ws(ws)) return rc;
-    if (n_haystacks < 0 || n_haystacks > 0xfffffffell) return fail(ACB_EINVAL, "n_haystacks out of range (0 .. 2^32 - 2)");
-    if (total_bytes >= (1ull << 31)) return fail(ACB_EINVAL, "total_bytes must be below 2^31 (scan larger inputs in windows)");
-    acb_plan want;
-    acb_plan_scan(a, dev_bytes, total_bytes, (uint64_t)n_haystacks, &want);
-    if (want.n_segments != plan->n_segments || want.segment_bytes != plan->segment_bytes || want.n_units != plan->n_units ||
-        want.task_bytes != plan->task_bytes)
-        return fail(ACB_EINVAL, "plan does not match the arguments (call acb_plan_scan again)");
-    SieveHeader sh;
-    if (int rc = sieve_header(a, sh)) return rc;
-    DeviceInfo d;
-    if (int rc = device_info(d)) return rc;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (n_haystacks == 0 || total_bytes == 0) {
-        if (n_haystacks) CUDA_OK(cudaMemsetAsync(dev_counts, 0, (uint64_t)n_haystacks * sizeof(uint64_t), st));
-        zero_outputs_kernel<<<(unsigned)((n_haystacks + 256) / 256), 256, 0, st>>>(
-            reinterpret_cast<unsigned long long *>(ws->dev_unit_offsets), reinterpret_cast<unsigned long long *>(ws->dev_match_offsets),
-            n_haystacks, reinterpret_cast<unsigned long long *>(ws->dev_total));
-        g_launches++;
-        CUDA_OK(cudaGetLastError());
-        return ACB_OK;
-    }
-    const int mode = a->impl->hdr.match_kind == ACB_STANDARD ? kModeStandard : kModeLeftmost;
-    return sieve_list_scan(a, dev_sieve, Batch{dev_bytes, dev_offsets, n_haystacks}, total_bytes, mode, false, nullptr, plan, ws, d, st,
-                           reinterpret_cast<unsigned long long *>(dev_counts));
+    return non_overlapping_counts(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, plan, ws, dev_counts, stream, false);
+}
+
+int acb_pattern_counts_overlapping(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                                   int64_t n_haystacks, uint64_t total_bytes, uint64_t *dev_pattern_counts, uint64_t *dev_scratch,
+                                   void *stream) {
+    if (!dev_pattern_counts) return fail(ACB_EINVAL, "null argument");
+    return sieve_early_scan(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, dev_pattern_counts, dev_scratch, stream,
+                            kSievePatterns);
+}
+
+int acb_pattern_counts_non_overlapping(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                                       int64_t n_haystacks, uint64_t total_bytes, const acb_plan *plan, const acb_workspace *ws,
+                                       uint64_t *dev_pattern_counts, void *stream) {
+    return non_overlapping_counts(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, plan, ws, dev_pattern_counts, stream, true);
 }
 
 int acb_count_rows(const acb_automaton *a, const int64_t *dev_rows, uint64_t n_rows, uint64_t *dev_scratch, uint64_t *dev_count,

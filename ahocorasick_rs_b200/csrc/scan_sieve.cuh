@@ -61,6 +61,12 @@
 // mode does, and instead of reserving and writing records adds it to the haystack's counter: lanes of one round that
 // share a haystack (most of them) are summed first, and one lane per distinct haystack adds.  Every position counts, so
 // nothing is skipped.
+//
+// PATTERNS (acb_pattern_counts_overlapping): the answer is the number of overlapping matches of each pattern over the
+// whole batch, one u64 counter per pattern id.  Stage 2 walks the deepest terminal node's chain as the list mode does
+// and adds 1 per pid instead of writing a record.  The chain is walked one pid per lane per step; lanes of a step that
+// hold the same pid (a short common pattern takes most hits) are summed first, and one lane per distinct pid adds.
+// Every position counts, so nothing is skipped.
 #pragma once
 #include "scan_staged.cuh"
 #include "sieve.h"
@@ -151,6 +157,7 @@ constexpr int kSieveList = 0;   // the overlapping match list (acb_scan_batch)
 constexpr int kSieveAny = 1;    // one flag per haystack (acb_any_match)
 constexpr int kSieveFirst = 2;  // one first-match key per haystack (acb_find_first): kSieveFirst + the match kind (ACB_*)
 constexpr int kSieveCount = 5;  // one overlapping match count per haystack (acb_count_overlapping)
+constexpr int kSievePatterns = 6;  // one overlapping match count per pattern (acb_pattern_counts_overlapping)
 
 // continuation bytes among the first nbytes (0..16) of the 16-byte chunk at shared address a
 __device__ __forceinline__ uint32_t cont_prefix(uint32_t a, uint32_t nbytes) {
@@ -176,24 +183,31 @@ __device__ __forceinline__ uint32_t warp_excl_scan(uint32_t v, uint32_t lane, ui
     return x - v;
 }
 
+// counts[pid] += the lanes of `act` that hold pid: one atomic per distinct pid (called by exactly the lanes of act)
+__device__ __forceinline__ void add_per_pattern(unsigned long long *counts, uint32_t act, uint32_t pid) {
+    const uint32_t peers = __match_any_sync(act, pid);
+    if ((threadIdx.x & 31u) == (uint32_t)__ffs(peers) - 1u) atomicAdd(counts + pid, (unsigned long long)__popc(peers));
+}
+
 // WC: 0 = W < 4 (the window word is shifted down), 1 = W == 4, 2 = W in 6..8 (two words), 3 = W == 5 (a word and a byte)
 //
 // Positions inside a task are 32-bit offsets from the task's start (`rel`); the 64-bit stream position is t_lo + rel.
 //
-// MODE kSieveAny, kSieveFirst + kind and kSieveCount (CP = false only): `out` is unused, and the two code-point
-// pointers carry the mode's outputs instead (so the list-mode instantiations keep their parameter block): hay_cont ->
-// flags = u8[n_haystacks] (any), keys = u64[n_haystacks] (first) or counts = u64[n_haystacks] (count), task_cont ->
-// skipped = u64[2] = [tasks skipped whole, windows not scanned] (see acb_any_match, acb_find_first; count: unused).
+// MODE kSieveAny, kSieveFirst + kind, kSieveCount and kSievePatterns (CP = false only): `out` is unused, and the two
+// code-point pointers carry the mode's outputs instead (so the list-mode instantiations keep their parameter block):
+// hay_cont -> flags = u8[n_haystacks] (any), keys = u64[n_haystacks] (first), counts = u64[n_haystacks] (count) or
+// counts = u64[n_patterns] (patterns), task_cont -> skipped = u64[2] = [tasks skipped whole, windows not scanned] (see
+// acb_any_match, acb_find_first; count, patterns: unused).
 template <bool CP, int WC, int MODE = kSieveList>
 __global__ void __launch_bounds__(kSieveThreads, 1)
 sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_cont, uint32_t *hay_cont, unsigned int *task_counter) {
     constexpr bool ANY = MODE == kSieveAny, FIRST = MODE >= kSieveFirst && MODE < kSieveCount, EARLY = ANY || FIRST;  // EARLY: no list, work stops early
-    constexpr bool COUNT = MODE == kSieveCount, LIST = MODE == kSieveList;
+    constexpr bool COUNT = MODE == kSieveCount, PATTERNS = MODE == kSievePatterns, LIST = MODE == kSieveList;
     constexpr int KIND = MODE - kSieveFirst;  // (FIRST)
     static_assert(!(!LIST && CP), "the any-match, first-match and count modes have no positions to count");
     uint8_t *const flags = reinterpret_cast<uint8_t *>(hay_cont);
     unsigned long long *const keys = reinterpret_cast<unsigned long long *>(hay_cont);
-    unsigned long long *const counts = reinterpret_cast<unsigned long long *>(hay_cont);
+    unsigned long long *const counts = reinterpret_cast<unsigned long long *>(hay_cont);  // (COUNT: per haystack; PATTERNS: per pattern)
     unsigned long long *const skipped = reinterpret_cast<unsigned long long *>(task_cont);
     extern __shared__ __align__(128) uint8_t smem[];
     const uint32_t bloom_s = (uint32_t)__cvta_generic_to_shared(smem);
@@ -469,6 +483,20 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
                     const uint32_t peers = __match_any_sync(hits, (uint32_t)h);  // (haystack ids fit 32 bits)
                     const uint32_t sum = __reduce_add_sync(peers, cnt);          // (at most 32 chain counts)
                     if (lane == (uint32_t)__ffs(peers) - 1u) atomicAdd(counts + (uint32_t)h, (unsigned long long)sum);
+                }
+            } else if (PATTERNS) {
+                // the chain, one pid per lane per step: one add per distinct pid of the step
+                uint32_t u = cnt ? best : kSieveNoNode, t = 0;
+                uint4 nb = make_uint4(0, 0, 0, 0);  // own_off, own_cnt, term_link, depth
+                if (u != kSieveNoNode) nb = __ldg(reinterpret_cast<const uint4 *>(sv.nb + u));
+                for (uint32_t act = hits; act; act = __ballot_sync(0xffffffffu, u != kSieveNoNode)) {
+                    if (u == kSieveNoNode) continue;
+                    add_per_pattern(counts, act, __ldg(sv.pids + nb.x + t));
+                    if (++t >= nb.y) {
+                        t = 0;
+                        u = nb.z;
+                        if (u != kSieveNoNode) nb = __ldg(reinterpret_cast<const uint4 *>(sv.nb + u));
+                    }
                 }
             } else if (hits) {
                 uint32_t total;

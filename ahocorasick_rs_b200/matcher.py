@@ -13,7 +13,9 @@ are already device resident; ``is_match`` / ``is_match_batch`` /
 ``is_match_device``, the crate's ``AhoCorasick::is_match`` per haystack;
 ``find_first`` / ``find_first_batch`` / ``find_first_device``, the crate's
 ``AhoCorasick::find`` per haystack; ``count_matches`` / ``count_matches_batch`` /
-``count_matches_device``, the length of each haystack's match list without the list.
+``count_matches_device``, the length of each haystack's match list without the list;
+``count_matches_by_pattern`` / ``count_matches_by_pattern_batch`` /
+``count_matches_by_pattern_device``, how many matches each pattern has over a batch.
 """
 from __future__ import annotations
 
@@ -815,6 +817,163 @@ class _Automaton:
             d = host[:head + total_bytes].to(dev, non_blocking=True)
             return self.count_device(d[head:], d[:8 * (n + 1)].view(torch.int64), overlapping).cpu().tolist()
 
+    # ---- match counts per pattern: bincount of find_matches_as_indexes' patterns, summed over a batch, without the list
+    def pattern_counts_device(self, data, offsets, overlapping=False, capacity: Optional[int] = None):
+        """How many matches each pattern has in a device-resident batch -> int64 CUDA tensor (n_patterns,): entry p is
+        the number of records with pattern p in scan_device's list, summed over the haystacks.  Patterns with the same
+        bytes keep their own ids.  An overlapping search on a leftmost automaton raises ValueError, as scan_device does.
+
+        Where the engine rule of scan_device picks the sieve: an overlapping search is the sieve kernel's pattern mode
+        (acb_pattern_counts_overlapping: no list, no epilogue) and returns without waiting for the device; a
+        non-overlapping search is the sieve's list scan and a pattern epilogue (acb_pattern_counts_non_overlapping),
+        which waits for the device and scans again with more room when the list did not fit (nothing was added then).
+        Where the rule picks a table walker, the counts are the bincount of the pattern column of its full scan, which
+        waits for it; the next scan that reuses the workspace waits for that bincount.  Batches above WINDOW_BYTES go
+        in runs of whole haystacks, and one haystack above it in windows, all added into one tensor.  `capacity`: the
+        workspace's first size, in records, as for scan_device."""
+        self.check_overlapping(overlapping)
+        torch = _require_cuda()
+        counts = torch.zeros(self.n_patterns, dtype=torch.int64, device=data.device)
+        n = offsets.numel() - 1
+        if n <= 0 or data.numel() == 0:
+            self.last_stats = {"engine": None, "mode": "pattern_counts", "long_stretches": 0}
+            return counts
+        if data.numel() > self.WINDOW_BYTES:
+            self._pattern_counts_windows(counts, data, offsets, overlapping)
+        else:
+            self._pattern_counts_into(counts, data, offsets, overlapping, capacity)
+        return counts
+
+    def _pattern_counts_into(self, counts, data, offsets, overlapping, capacity=None):
+        """Adds the per-pattern counts of a batch of at most WINDOW_BYTES to `counts`; sets last_stats."""
+        torch = _require_cuda()
+        dev = data.device
+        n = offsets.numel() - 1
+        with self._lock, torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev)
+            if self._pick_engine(dev, data, offsets, overlapping) is not None:
+                m, _, _ = self.scan_device(data, offsets, overlapping, False)
+                counts += torch.bincount(m[:, 1].long(), minlength=self.n_patterns)
+                reader = torch.cuda.Event()
+                reader.record(stream)
+                self._ws[(dev.index if dev.index is not None else torch.cuda.current_device(), 0)]["reader"] = reader
+                self.last_stats = {"engine": self.last_stats.get("engine", "table"), "mode": "pattern_counts", "long_stretches": 0}
+                return
+            sieve_t, _ = self.sieve(dev)
+            if overlapping:
+                scratch = torch.empty(3, dtype=torch.int64, device=dev)
+                rc = self._L.acb_pattern_counts_overlapping(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n,
+                                                            data.numel(), counts.data_ptr(), scratch.data_ptr(), stream.cuda_stream)
+                if rc != _capi.ACB_OK:
+                    raise RuntimeError(_capi.last_error())
+                self.last_stats = {"engine": "sieve", "mode": "pattern_counts", **self.sieve_geometry(dev, self._plan(data, n).task_bytes),
+                                   "long_stretches": 0}
+                return
+            plan = self._plan(data, n)
+            cap = capacity or max(1024, n * 2)
+            while True:
+                ws = self._workspace(dev, plan, n, cap, 0)
+                reader = ws.pop("reader", None)
+                if reader is not None:   # a comparison of an earlier call (maybe on another stream) reads this workspace first
+                    stream.wait_event(reader)
+                st = self._ws_struct(ws)
+                rc = self._L.acb_pattern_counts_non_overlapping(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n,
+                                                                data.numel(), C.byref(plan), C.byref(st), counts.data_ptr(),
+                                                                stream.cuda_stream)
+                if rc != _capi.ACB_OK:
+                    err = _capi.last_error()
+                    ws["scratch"][:8].zero_()   # a scan that failed half way may have left its counters dirty
+                    raise RuntimeError(err)
+                tot = ws["total"].tolist()
+                total, complete, long_stretches, raw_total = tot[0], tot[1], tot[2], tot[4]
+                if complete or (total == 0 and raw_total == 0):
+                    break
+                cap = max(total, raw_total) + max(total, raw_total) // 8 + 16   # (nothing was added: the counts stay as they were)
+            self.last_stats = {"engine": "sieve", "mode": "pattern_counts", **self.sieve_geometry(dev, plan.task_bytes),
+                               "list_records": raw_total, "long_stretches": long_stretches}
+
+    def _pattern_counts_windows(self, counts, data, offsets, overlapping):
+        """pattern_counts_device above WINDOW_BYTES: runs of whole haystacks that fit one call each add their counts;
+        one haystack above the limit goes to _pattern_counts_one_large.  last_stats["long_stretches"] sums the runs'."""
+        torch = _require_cuda()
+        dev = data.device
+        n = offsets.numel() - 1
+        limit = self.WINDOW_BYTES
+        lens = offsets[1:] - offsets[:-1]
+        oversized = bool((lens > limit).any().item())
+        long_stretches = 0
+        engine = None
+        h = 0
+        while h < n:
+            start = int(offsets[h].item())
+            if oversized and int(lens[h].item()) > limit:
+                self._pattern_counts_one_large(counts, data[start:start + int(lens[h].item())], overlapping)
+                h += 1
+                continue
+            # the longest run of whole haystacks that fits one call (and stops before an oversized one)
+            h1 = int(torch.searchsorted(offsets, torch.tensor([start + limit], dtype=torch.int64, device=dev), right=True).item()) - 1
+            h1 = max(h + 1, min(h1, n))
+            if oversized:
+                big = torch.nonzero(lens[h:h1] > limit)
+                if big.numel():
+                    h1 = h + int(big[0].item())
+            end = int(offsets[h1].item())
+            if end > start:
+                self._pattern_counts_into(counts, data[start:end], offsets[h:h1 + 1] - start, overlapping)
+                long_stretches += self.last_stats.get("long_stretches", 0)
+                engine = self.last_stats.get("engine")
+            h = h1
+        torch.cuda.current_stream(dev).synchronize()
+        self.last_stats = {"engine": engine, "mode": "pattern_counts", "long_stretches": long_stretches, "windows": True}
+
+    def _pattern_counts_one_large(self, counts, hay, overlapping):
+        """Adds the per-pattern counts of one haystack above WINDOW_BYTES to `counts`.
+        Overlapping: windows that share max_pattern_len - 1 bytes, as in _count_one_large.  A match wholly inside a
+        window's head was counted by the window before, so the head's own counts are subtracted, pattern by pattern.
+        Non-overlapping: the overlapping rows of the windows, the serial selection (acb_select_non_overlapping), and
+        the bincount of the selected rows' patterns."""
+        torch = _require_cuda()
+        dev = hay.device
+        if overlapping:
+            limit, halo = self.WINDOW_BYTES, max(self.max_pattern_len - 1, 0)
+            head = torch.zeros_like(counts)
+            w0 = 0
+            while True:
+                w1 = min(w0 + limit, hay.numel())
+                self._pattern_counts_into(counts, hay[w0:w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=dev), True)
+                if w0 and halo:
+                    self._pattern_counts_into(head, hay[w0:w0 + halo], torch.tensor([0, halo], dtype=torch.int64, device=dev), True)
+                if w1 == hay.numel():
+                    counts -= head
+                    return
+                w0 += limit - halo
+        rows = self._scan_one_large(hay, False, False)
+        counts += torch.bincount(rows[:, 1], minlength=self.n_patterns)
+
+    def pattern_counts_host_batch(self, chunks: Sequence[bytes], overlapping):
+        """Host buffers (bytes-like objects, one per haystack) -> list of int: each pattern's match count over all of
+        them.  The offsets and the haystacks are gathered into the pinned staging buffer and go to the device in one copy."""
+        torch = _require_cuda()
+        self.check_overlapping(overlapping)
+        n = len(chunks)
+        if n == 0:
+            return [0] * self.n_patterns
+        offs = np.zeros(n + 1, dtype=np.int64)
+        np.cumsum(np.fromiter((len(c) for c in chunks), dtype=np.int64, count=n), out=offs[1:])
+        total_bytes = int(offs[-1])
+        head = (8 * (n + 1) + 511) & ~511   # the offsets, then the bytes at a 512-byte boundary of the buffer
+        dev = torch.device("cuda", torch.cuda.current_device())
+        with self._host_lock:
+            host = self._pinned(head + total_bytes)
+            hv = host.numpy()
+            hv[:8 * (n + 1)].view(np.int64)[:] = offs
+            if n == 1:
+                hv[head:head + total_bytes] = np.frombuffer(chunks[0], dtype=np.uint8)
+            elif total_bytes:
+                hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
+            d = host[:head + total_bytes].to(dev, non_blocking=True)
+            return self.pattern_counts_device(d[head:], d[:8 * (n + 1)].view(torch.int64), overlapping).cpu().tolist()
+
     def scan_device(self, data, offsets, overlapping=False, codepoints=False, capacity: Optional[int] = None,
                     sync: bool = True, ws_slot: int = 0):
         """Scan a device-resident batch.  data: uint8 CUDA tensor, offsets: int64
@@ -1514,6 +1673,28 @@ class AhoCorasick:
         """Device-resident UTF-8 batch -> int64 tensor (n,) of match counts (see _Automaton.count_device)."""
         return self._ac.count_device(data, offsets, overlapping)
 
+    def count_matches_by_pattern(self, haystack: str, overlapping: bool = False) -> list:
+        """-> list of length ``len(patterns)``: entry i is how many of ``find_matches_as_indexes(haystack,
+        overlapping)`` have pattern i, counted without building the list."""
+        if not isinstance(haystack, str):
+            raise TypeError("argument 'haystack': 'str' expected")
+        self._ac.check_overlapping(overlapping)
+        return self._ac.pattern_counts_host_batch([haystack.encode("utf-8")], overlapping)
+
+    def count_matches_by_pattern_batch(self, haystacks: Sequence[str], overlapping: bool = False) -> list:
+        """``count_matches_by_pattern`` summed over all the haystacks, in one transfer and one scan."""
+        hays = list(haystacks)
+        for h in hays:
+            if not isinstance(h, str):
+                raise TypeError("argument 'haystack': 'str' expected")
+        self._ac.check_overlapping(overlapping)
+        return self._ac.pattern_counts_host_batch([h.encode("utf-8") for h in hays], overlapping)
+
+    def count_matches_by_pattern_device(self, data, offsets, overlapping: bool = False):
+        """Device-resident UTF-8 batch -> int64 tensor (n_patterns,) of match counts per pattern over the whole batch
+        (see _Automaton.pattern_counts_device)."""
+        return self._ac.pattern_counts_device(data, offsets, overlapping)
+
     # ---- additions: stream search (data fed in chunks; the crate's stream_find_iter, for every match kind) -------------
     def stream(self, overlapping: bool = False) -> Stream:
         """One stream fed ``str`` chunks: ``feed(chunk)`` returns the rows (pattern, start, end) it releases, in code
@@ -1612,6 +1793,24 @@ class BytesAhoCorasick:
     def count_matches_device(self, data, offsets, overlapping: bool = False):
         """Device-resident batch -> int64 tensor (n,) of match counts (see _Automaton.count_device)."""
         return self._ac.count_device(data, offsets, overlapping)
+
+    def count_matches_by_pattern(self, haystack, overlapping: bool = False) -> list:
+        """-> list of length ``len(patterns)``: entry i is how many of ``find_matches_as_indexes(haystack,
+        overlapping)`` have pattern i, counted without building the list."""
+        hay = _as_buffer_bytes(haystack)
+        self._ac.check_overlapping(overlapping)
+        return self._ac.pattern_counts_host_batch([hay], overlapping)
+
+    def count_matches_by_pattern_batch(self, haystacks: Sequence, overlapping: bool = False) -> list:
+        """``count_matches_by_pattern`` summed over all the haystacks, in one transfer and one scan."""
+        hays = [_as_buffer_bytes(h) for h in haystacks]
+        self._ac.check_overlapping(overlapping)
+        return self._ac.pattern_counts_host_batch(hays, overlapping)
+
+    def count_matches_by_pattern_device(self, data, offsets, overlapping: bool = False):
+        """Device-resident batch -> int64 tensor (n_patterns,) of match counts per pattern over the whole batch (see
+        _Automaton.pattern_counts_device)."""
+        return self._ac.pattern_counts_device(data, offsets, overlapping)
 
     # ---- additions: stream search (data fed in chunks; the crate's stream_find_iter, for every match kind) -------------
     def stream(self, overlapping: bool = False) -> Stream:

@@ -344,6 +344,37 @@ int acb_count_rows(const acb_automaton *a, const int64_t *dev_rows, uint64_t n_r
                    void *stream);
 
 /*
+ * How often each pattern matches in a device-resident batch, without the match list: dev_pattern_counts =
+ * u64[acb_num_patterns(a)], read and written, and entry p is ADDED the number of records with pattern p in the
+ * reference's result (get_matches, src/lib.rs:42-68), summed over the batch's haystacks.  Patterns with the same bytes
+ * keep their own ids and are each counted as the reference reports them.  Accumulating lets runs of haystacks, windows
+ * of one haystack and several devices total one corpus.  Two calls:
+ *
+ * acb_pattern_counts_overlapping counts the overlapping matches: one launch of the sieve kernel in its pattern mode, no
+ * records, no epilogue, no synchronisation, nothing skipped.  Standard automata only: any other kind returns
+ * ACB_EUNSUPPORTED before any byte is read.  dev_scratch = u64[3], as for acb_count_overlapping.
+ *
+ * acb_pattern_counts_non_overlapping counts the non-overlapping matches for every match kind: the sieve's list scan
+ * (plan and workspace as for acb_count_non_overlapping), then an epilogue that places the overlapping list, selects each
+ * haystack's matches without packing a result, and adds the selected records' patterns.  A haystack whose overlapping
+ * list has more than ACB_LONG_STRETCH records is selected by the whole grid (successors, pointer jumping, and marks
+ * that follow the chain of selected records), the others by one thread each.  ws->dev_total: [0] = records added (the
+ * total of the selection), [1] = 1 when the counts were added (0: the workspace was too small, NOTHING was added, and
+ * [0] / [4] say how much room a second call needs), [2] = haystacks selected by the whole grid, [3] = [5] = 0, [4] =
+ * records of the overlapping list.  Two launches, no synchronisation.  ws->dev_out, ws->dev_raw, ws->dev_raw_seq and
+ * ws->dev_match_offsets are overwritten.
+ *
+ * Argument checks, the 2^31 limit and the empty cases are those of acb_count_overlapping and acb_count_non_overlapping
+ * (ACB_EINVAL before any CUDA call); an empty batch adds nothing.
+ */
+int acb_pattern_counts_overlapping(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                                   int64_t n_haystacks, uint64_t total_bytes, uint64_t *dev_pattern_counts, uint64_t *dev_scratch,
+                                   void *stream);
+int acb_pattern_counts_non_overlapping(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                                       int64_t n_haystacks, uint64_t total_bytes, const acb_plan *plan, const acb_workspace *ws,
+                                       uint64_t *dev_pattern_counts, void *stream);
+
+/*
  * Stream search: matches in data that arrives in chunks, for many streams at once.  A stream is the concatenation of
  * the chunks fed to it; positions are absolute within it and 64-bit.  The crate the reference wraps has the single-stream,
  * Standard, non-overlapping form (AhoCorasick::stream_find_iter); here every match kind and overlapping Standard are
