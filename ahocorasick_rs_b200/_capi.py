@@ -103,6 +103,10 @@ def lib():
                                                      C.c_void_p, C.c_void_p, C.c_void_p]
         L.acb_pattern_counts_non_overlapping.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64,
                                                          C.POINTER(Plan), C.POINTER(Workspace), C.c_void_p, C.c_void_p]
+        L.acb_pattern_hit_row_words.restype = C.c_uint64
+        L.acb_pattern_hit_row_words.argtypes = [C.c_uint64]
+        L.acb_pattern_hits.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64, C.c_int, C.POINTER(Plan),
+                                       C.POINTER(Workspace), C.c_void_p, C.c_uint64, C.c_void_p]
         L.acb_first_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
         L.acb_rows_to_codepoints.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
         L.acb_stream_seams.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -145,5 +149,6 @@ EXPORTS = [
     "acb_sieve_build", "acb_sieve_write", "acb_sieve_describe", "acb_pack_gather_block", "acb_select_non_overlapping",
     "acb_any_match", "acb_find_first", "acb_first_rows", "acb_rows_to_codepoints",
     "acb_count_overlapping", "acb_count_non_overlapping", "acb_count_rows", "acb_stream_seams", "acb_stream_resolve",
-    "acb_pattern_counts_overlapping", "acb_pattern_counts_non_overlapping",
+    "acb_pattern_counts_overlapping", "acb_pattern_counts_non_overlapping", "acb_pattern_hits",
+    "acb_pattern_hit_row_words",
 ]

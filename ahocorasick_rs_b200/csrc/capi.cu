@@ -870,18 +870,74 @@ __global__ void __launch_bounds__(kScanThreads) sieve_count_epilogue_kernel(Siev
     finish(true);
 }
 
+// Phase 4 of the pattern and hits epilogues, over the complete ordered list E.ordered[0 .. avail): each haystack's
+// selection, found and left in place.  unit_offsets[h] = the first record of h's stretch.  A stretch of at most
+// ACB_LONG_STRETCH records is selected by one thread and packed to its front (unit_counts[h] = how many; MODE
+// kModeOverlap selects every record).  A longer one (unit_counts[h] = kLongMark, match_offsets[h] = its end) gets
+// successors and pointer jumping as in the count variant, and MARKS its selection, the chain head = NEXT(0), NEXT(head),
+// ...: mark[head] is set before the rounds, and in round k every marked record i also marks its round-k successor
+// J_k(i) = NEXT^(2^k)(i), which it reads anyway.  After round k every NEXT^m(head) with m < 2^(k+1) is marked, so
+// ceil(log2(stretch)) rounds mark the whole chain.  Only chain records are ever marked (the chain is closed under J_k),
+// so a mark another thread sets in the same round and this one already sees only marks a chain record sooner: the race
+// needs no barrier.  The marks live in raw_seq (u32 per record, consumed by phase 3); the pairs' rank words are computed
+// and unused.  (kModeOverlap: a long stretch is selected whole and nothing is marked.)  totals[2] = the long stretches,
+// totals[5] = the longest.  Ends with a grid barrier.
+template <int MODE>
+__device__ __forceinline__ void select_stretches(const SieveEpiArgs &E, cooperative_groups::grid_group &grid, unsigned long long avail) {
+    acb_match *const list = E.ordered;
+    uint4 *const pairs = reinterpret_cast<uint4 *>(const_cast<acb_match *>(E.raw));
+    uint32_t *const mark = const_cast<uint32_t *>(E.raw_seq);
+    unsigned long long *const ends = E.match_offsets;
+    const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+    const unsigned long long first_i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    // the thread that sees a haystack's first record owns its stretch
+    for (unsigned long long i = first_i; i < avail; i += stride) {
+        const uint32_t hc = list[i].haystack;
+        if (i && list[i - 1].haystack == hc) continue;
+        const unsigned long long a = stretch_end(list, i, avail);
+        const unsigned long long len = a - i;
+        E.unit_offsets[hc] = i;
+        if (len <= ACB_LONG_STRETCH) {
+            E.unit_counts[hc] = MODE == kModeOverlap ? (uint32_t)len : select_non_overlapping<MODE>(list + i, len, E.max_pat_len, E.longest);
+        } else {
+            E.unit_counts[hc] = kLongMark;
+            ends[hc] = a;
+            // the chain's head, relative, in the second half of the first record's pair until the successors are written
+            if (MODE != kModeOverlap) pairs[i].z = (uint32_t)next_selected<MODE>(list + i, len, 0, E.max_pat_len, E.longest);
+            atomicAdd(E.totals + 2, 1ull);
+            atomicMax(E.totals + 5, len);
+        }
+    }
+    grid.sync();
+    if (MODE != kModeOverlap && E.totals[2]) {
+        for (unsigned long long i = first_i; i < avail; i += stride) {
+            const uint32_t hc = list[i].haystack;
+            if (E.unit_counts[hc] != kLongMark) continue;
+            const unsigned long long lo = E.unit_offsets[hc], n = ends[hc] - lo;
+            const unsigned long long nx = next_selected<MODE>(list + lo, n, (long long)list[i].end, E.max_pat_len, E.longest);
+            reinterpret_cast<uint2 *>(pairs + i)[0] = make_uint2(nx == n ? kNoNext : (uint32_t)(lo + nx), 1u);
+            mark[i] = i == lo + pairs[lo].z ? 1u : 0u;
+        }
+        grid.sync();
+        const uint32_t rounds = ceil_log2(E.totals[5]);
+        for (uint32_t r = 0; r < rounds; r++) {
+            const int src = (int)(r & 1);
+            for (unsigned long long i = first_i; i < avail; i += stride) {
+                if (E.unit_counts[list[i].haystack] != kLongMark) continue;
+                const uint32_t j = src ? pairs[i].z : pairs[i].x;  // J_r(i)
+                if (j != kNoNext && mark[i]) mark[j] = 1u;
+                jump_pair(pairs, i, src);
+            }
+            grid.sync();
+        }
+    }
+}
+
 // The per-pattern variant of sieve_count_epilogue_kernel (acb_pattern_counts_non_overlapping): phases 1-3 place the
-// overlapping list, then each haystack's selection is found and the pid of every selected record is added to
-// pattern_counts[pid].  A stretch of at most ACB_LONG_STRETCH records is selected by one thread and packed to its front
-// (unit_counts[h] = how many).  A longer one gets successors and pointer jumping as in the count variant, and MARKS its
-// selection, the chain head = NEXT(0), NEXT(head), ...: mark[head] is set before the rounds, and in round k every marked
-// record i also marks its round-k successor J_k(i) = NEXT^(2^k)(i), which it reads anyway.  After round k every NEXT^m(head)
-// with m < 2^(k+1) is marked, so ceil(log2(stretch)) rounds mark the whole chain.  Only chain records are ever marked (the
-// chain is closed under J_k), so a mark another thread sets in the same round and this one already sees only marks a
-// chain record sooner: the race needs no barrier.  The marks live in raw_seq (u32 per record, consumed by phase 3); the
-// pairs' rank words are computed and unused.  A last pass over the list adds the pids of the selected records.
-// totals[0] sums the selected records during the launch, totals[2] = haystacks selected on the grid, totals[5] = the
-// longest such stretch; ws->dev_match_offsets holds each long stretch's end.  Nothing is added when the list did not fit.
+// overlapping list, select_stretches finds each haystack's selection, and a last pass over the list adds the pid of
+// every selected record to pattern_counts[pid].  totals[0] sums the selected records during the launch, totals[2] =
+// haystacks selected on the grid, totals[5] = the longest such stretch; ws->dev_match_offsets holds each long stretch's
+// end.  Nothing is added when the list did not fit.
 template <int MODE>
 __global__ void __launch_bounds__(kScanThreads) sieve_pattern_epilogue_kernel(SieveEpiArgs E, unsigned long long *pattern_counts) {
     namespace cg = cooperative_groups;
@@ -894,53 +950,11 @@ __global__ void __launch_bounds__(kScanThreads) sieve_pattern_epilogue_kernel(Si
     const bool complete = list_total <= E.out_cap && raw_total <= E.raw_cap;  // (else the list has holes: nothing is added)
     if (complete) {
         const unsigned long long avail = list_total;
-        acb_match *const list = E.ordered;
-        uint4 *const pairs = reinterpret_cast<uint4 *>(const_cast<acb_match *>(E.raw));
-        uint32_t *const mark = const_cast<uint32_t *>(E.raw_seq);
-        unsigned long long *const ends = E.match_offsets;
+        select_stretches<MODE>(E, grid, avail);
+        const acb_match *const list = E.ordered;
+        const uint32_t *const mark = E.raw_seq;
         const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
         const unsigned long long first_i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
-        // phase 4: the thread that sees a haystack's first record owns its stretch
-        for (unsigned long long i = first_i; i < avail; i += stride) {
-            const uint32_t hc = list[i].haystack;
-            if (i && list[i - 1].haystack == hc) continue;
-            const unsigned long long a = stretch_end(list, i, avail);
-            const unsigned long long len = a - i;
-            E.unit_offsets[hc] = i;
-            if (len <= ACB_LONG_STRETCH) {
-                E.unit_counts[hc] = select_non_overlapping<MODE>(list + i, len, E.max_pat_len, E.longest);
-            } else {
-                E.unit_counts[hc] = kLongMark;
-                ends[hc] = a;
-                // the chain's head, relative, in the second half of the first record's pair until the successors are written
-                pairs[i].z = (uint32_t)next_selected<MODE>(list + i, len, 0, E.max_pat_len, E.longest);
-                atomicAdd(E.totals + 2, 1ull);
-                atomicMax(E.totals + 5, len);
-            }
-        }
-        grid.sync();
-        if (E.totals[2]) {
-            for (unsigned long long i = first_i; i < avail; i += stride) {
-                const uint32_t hc = list[i].haystack;
-                if (E.unit_counts[hc] != kLongMark) continue;
-                const unsigned long long lo = E.unit_offsets[hc], n = ends[hc] - lo;
-                const unsigned long long nx = next_selected<MODE>(list + lo, n, (long long)list[i].end, E.max_pat_len, E.longest);
-                reinterpret_cast<uint2 *>(pairs + i)[0] = make_uint2(nx == n ? kNoNext : (uint32_t)(lo + nx), 1u);
-                mark[i] = i == lo + pairs[lo].z ? 1u : 0u;
-            }
-            grid.sync();
-            const uint32_t rounds = ceil_log2(E.totals[5]);
-            for (uint32_t r = 0; r < rounds; r++) {
-                const int src = (int)(r & 1);
-                for (unsigned long long i = first_i; i < avail; i += stride) {
-                    if (E.unit_counts[list[i].haystack] != kLongMark) continue;
-                    const uint32_t j = src ? pairs[i].z : pairs[i].x;  // J_r(i)
-                    if (j != kNoNext && mark[i]) mark[j] = 1u;
-                    jump_pair(pairs, i, src);
-                }
-                grid.sync();
-            }
-        }
         // the selected records' pids: whole warps step through the list together, so equal pids of a step add once
         unsigned long long sum = 0;
         for (unsigned long long w = first_i & ~31ull; w < avail; w += stride) {
@@ -964,6 +978,264 @@ __global__ void __launch_bounds__(kScanThreads) sieve_pattern_epilogue_kernel(Si
         E.totals[1] = complete ? 1 : 0;
         E.totals[3] = E.totals[5] = E.totals[7] = 0;
         E.totals[4] = raw_total > list_total ? raw_total : list_total;  // room the overlapping list needs
+        E.acc[kAccRaw] = E.acc[kAccGroups] = E.acc[kAccTraps] = E.acc[kAccRepairs] = 0;
+        E.acc[kAccQueue] = 0;
+    }
+}
+
+// ---------------------------------------------------------------------------
+// HITS (acb_pattern_hits): each haystack's distinct patterns, with how many of its selected records have each one.
+// ---------------------------------------------------------------------------
+constexpr uint32_t kHitsSmemKeys = 1024;  // per-warp shared sort buffer: 4 KiB, 32 KiB per block (4 blocks per SM still fit)
+
+// u32 words of one counter row: n_patterns counters (padded to an even count), then u64 [haystack, nonzero counters in
+// tile 0, tile 1, ...] (tiles of kScanTile counters)
+__host__ __device__ __forceinline__ unsigned long long hit_row_words(unsigned long long n_patterns) {
+    return (n_patterns + 1) / 2 * 2 + 2 + 2 * ((n_patterns + kScanTile - 1) / kScanTile);
+}
+
+// rows[key] += the lanes of `act` that hold key: one atomic per distinct key (called by exactly the lanes of act)
+__device__ __forceinline__ void add_to_row(uint32_t *rows, uint32_t act, unsigned long long key) {
+    const uint32_t peers = __match_any_sync(act, key);
+    if ((threadIdx.x & 31u) == (uint32_t)__ffs(peers) - 1u) atomicAdd(rows + key, (uint32_t)__popc(peers));
+}
+
+// the warp's 32 values, ascending across the lanes (bitonic network over shuffles)
+__device__ __forceinline__ uint32_t warp_sort32(uint32_t x) {
+    const uint32_t lane = threadIdx.x & 31u;
+#pragma unroll
+    for (uint32_t k = 2; k <= 32; k <<= 1)
+#pragma unroll
+        for (uint32_t j = k >> 1; j; j >>= 1) {
+            const uint32_t y = __shfl_xor_sync(0xffffffffu, x, j);
+            x = (((lane & j) == 0) == ((lane & k) == 0)) ? min(x, y) : max(x, y);
+        }
+    return x;
+}
+
+// The hits of a selection of at most 32 records sel[0 .. n): the pids sorted in registers, runs found with a ballot;
+// hit k = (h, pid, run length, 0) goes to out[k].  -> how many hits.
+__device__ __forceinline__ uint32_t warp_hits32(const acb_match *sel, uint32_t n, uint32_t h, uint4 *out) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint32_t k = warp_sort32(lane < n ? sel[lane].pattern : 0xffffffffu);
+    const uint32_t prev = __shfl_up_sync(0xffffffffu, k, 1);
+    const bool head = lane < n && (lane == 0 || prev != k);
+    const uint32_t heads = __ballot_sync(0xffffffffu, head);
+    if (head) {
+        const uint32_t later = heads & ~((2u << lane) - 1u);
+        const uint32_t end = later ? (uint32_t)__ffs(later) - 1u : n;
+        out[__popc(heads & ((1u << lane) - 1u))] = make_uint4(h, k, end - lane, 0u);
+    }
+    return (uint32_t)__popc(heads);
+}
+
+// keys[0 .. n) ascending, by one warp (shared or global memory): the bitonic network in its flip form, where every
+// comparator puts the smaller key first, so positions past n act as +infinity and their comparators are skipped
+__device__ __forceinline__ void warp_sort_keys(uint32_t *keys, uint32_t n) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint32_t half = (n <= 1 ? 1u : 1u << (32 - __clz(n - 1))) >> 1;  // comparators per step
+    for (uint32_t k = 2; k <= 2 * half; k <<= 1) {
+        for (uint32_t j = k >> 1; j; j >>= 1) {
+            for (uint32_t p = lane; p < half; p += 32) {
+                const uint32_t a = ((p & ~(j - 1)) << 1) | (p & (j - 1));  // (bit j of a is clear)
+                const uint32_t b = j == k >> 1 ? a ^ (k - 1) : a ^ j;
+                if (b < n) {
+                    const uint32_t x = keys[a], y = keys[b];
+                    if (x > y) {
+                        keys[a] = y;
+                        keys[b] = x;
+                    }
+                }
+            }
+            __syncwarp();
+        }
+    }
+}
+
+// the runs of sorted keys[0 .. n) as hits (h, key, run length, 0) at out[0 ..), by one warp -> how many
+__device__ __forceinline__ uint32_t warp_runs(const uint32_t *keys, uint32_t n, uint32_t h, uint4 *out) {
+    const uint32_t lane = threadIdx.x & 31u;
+    uint32_t d = 0;
+    for (uint32_t base = 0; base < n; base += 32) {
+        const uint32_t j = base + lane;
+        const uint32_t k = j < n ? keys[j] : 0u;
+        const bool head = j < n && (j == 0 || keys[j - 1] != k);
+        const uint32_t heads = __ballot_sync(0xffffffffu, head);
+        if (head) {
+            uint32_t lo = j + 1, hi = n;  // the run's end: the first key above k
+            while (lo < hi) {
+                const uint32_t mid = (lo + hi) >> 1;
+                if (keys[mid] == k)
+                    lo = mid + 1;
+                else
+                    hi = mid;
+            }
+            out[d + __popc(heads & ((1u << lane) - 1u))] = make_uint4(h, k, lo - j, 0u);
+        }
+        d += (uint32_t)__popc(heads);
+    }
+    return d;
+}
+
+// The hits epilogue (acb_pattern_hits; MODE kModeStandard / kModeLeftmost, or kModeOverlap for the overlapping search):
+// phases 1-3 place the overlapping list, select_stretches finds each haystack's selection (kModeOverlap: all of it),
+// and each haystack's selected pids become its d_h hits (pid, count), pids ascending, staged at the haystack's stretch
+// offset in dev_raw (d_h <= the stretch's records, so the slices never overlap; the pairs there are dead by then).
+//   short stretch: one warp per haystack.  Up to 32 pids are sorted in registers; up to kHitsSmemKeys in the warp's
+//     shared buffer; up to ACB_LONG_STRETCH in the stretch's slice of raw_seq (consumed by phase 3, unmarked for a short
+//     stretch, in L2); then run-length encoded.
+//   long stretch: a dense counter row in `rows` (slot from totals[3], only the used rows are zeroed).  Whole warps add
+//     the selected pids to it, as the pattern epilogue's last pass does, and a prefix over each row's nonzero counters
+//     (tiles, as tile_sum_body / tile_apply_body) stages its hits in pid order, without a sort.
+// Then phases 5-6 of the list epilogue give the per-haystack offsets, and the hits are packed from dev_raw into dev_out
+// (where the ordered list lived).  totals[2] = long stretches, [3] = rows used, [5] = row words needed.
+template <int MODE>
+__global__ void __launch_bounds__(kScanThreads) sieve_hits_epilogue_kernel(SieveEpiArgs E, uint32_t *rows, unsigned long long row_words,
+                                                                           uint32_t n_patterns) {
+    namespace cg = cooperative_groups;
+    cg::grid_group grid = cg::this_grid();
+    __shared__ uint32_t sort_keys[kScanThreads / 32][kHitsSmemKeys];
+    if (blockIdx.x == 0 && threadIdx.x == 0) E.totals[2] = E.totals[3] = E.totals[5] = 0;  // (read and added to only after later barriers)
+    sieve_order_list<false>(E, grid);
+    const int64_t nh = E.B.n_haystacks;
+    const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+    const unsigned long long first_i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    // haystacks without records have no hits (the task counts in this array were consumed by phase 2)
+    for (int64_t h = (int64_t)first_i; h < nh; h += (int64_t)stride) E.unit_counts[h] = 0;
+    grid.sync();
+    const unsigned long long list_total = E.totals[6];
+    const unsigned long long raw_total = E.totals[7];
+    const unsigned long long rw = hit_row_words(n_patterns);
+    // (else the list has holes: nothing is written, the caller retries with the room reported)
+    bool complete = list_total <= E.out_cap && list_total <= E.raw_cap && raw_total <= E.raw_cap;
+    unsigned long long n_long = 0;
+    if (complete) {
+        select_stretches<MODE>(E, grid, list_total);
+        n_long = E.totals[2];
+        complete = n_long * rw <= row_words;
+    }
+    if (complete) {
+        const unsigned long long avail = list_total;
+        const acb_match *const list = E.ordered;
+        const uint32_t *const mark = E.raw_seq;
+        uint4 *const staged = reinterpret_cast<uint4 *>(const_cast<acb_match *>(E.raw));
+        unsigned long long *const slot = E.match_offsets;  // a long stretch's row (its end is no longer needed)
+        const uint32_t lane = threadIdx.x & 31u;
+        const uint64_t tpr = ((uint64_t)n_patterns + kScanTile - 1) / kScanTile;
+        auto meta = [&](unsigned long long s) { return reinterpret_cast<unsigned long long *>(rows + (s + 1) * rw - 2 - 2 * tpr); };
+        if (n_long) {
+            for (int64_t h = (int64_t)first_i; h < nh; h += (int64_t)stride)
+                if (E.unit_counts[h] == kLongMark) {
+                    const unsigned long long s = atomicAdd(E.totals + 3, 1ull);
+                    slot[h] = s;
+                    meta(s)[0] = (unsigned long long)h;
+                }
+            for (unsigned long long s = 0; s < n_long; s++)
+                for (unsigned long long p = first_i; p < n_patterns; p += stride) rows[s * rw + p] = 0;
+            grid.sync();
+            // the long stretches' selected pids into their rows: whole warps step through the list together, so equal
+            // counters of a step add once
+            for (unsigned long long w = first_i & ~31ull; w < avail; w += stride) {
+                const unsigned long long i = w + lane;
+                bool sel = false;
+                unsigned long long key = 0;
+                if (i < avail) {
+                    const uint4 r = reinterpret_cast<const uint4 *>(list)[i];  // haystack, pattern, start, end
+                    if (E.unit_counts[r.x] == kLongMark) {
+                        sel = MODE == kModeOverlap || mark[i] != 0;
+                        key = slot[r.x] * rw + r.y;
+                    }
+                }
+                const uint32_t act = __ballot_sync(0xffffffffu, sel);
+                if (sel) add_to_row(rows, act, key);
+            }
+        }
+        // the short stretches: one warp per haystack (a long stretch's kLongMark is never a short one's count)
+        uint32_t *const smem_keys = sort_keys[threadIdx.x >> 5];
+        for (unsigned long long h = first_i >> 5; h < (unsigned long long)nh; h += stride >> 5) {
+            const uint32_t c = E.unit_counts[h];
+            if (c == 0 || c == kLongMark) continue;
+            const unsigned long long lo = E.unit_offsets[h];
+            uint32_t d;
+            if (c <= 32) {
+                d = warp_hits32(list + lo, c, (uint32_t)h, staged + lo);
+            } else {
+                uint32_t *const keys = c <= kHitsSmemKeys ? smem_keys : const_cast<uint32_t *>(mark) + lo;
+                for (uint32_t j = lane; j < c; j += 32) keys[j] = list[lo + j].pattern;
+                __syncwarp();
+                warp_sort_keys(keys, c);
+                d = warp_runs(keys, c, (uint32_t)h, staged + lo);
+                __syncwarp();  // (the shared buffer serves the warp's next haystack)
+            }
+            if (lane == 0) E.unit_counts[h] = d;
+        }
+        grid.sync();
+        if (n_long) {
+            // each row's nonzero counters: per tile, then each tile's start within its row, and the hits staged
+            const uint64_t tiles = n_long * tpr;
+            for (uint64_t tt = blockIdx.x; tt < tiles; tt += gridDim.x) {
+                const uint64_t s = tt / tpr, t = tt % tpr;
+                const uint32_t *const row = rows + s * rw;
+                const uint64_t base = t * kScanTile + (uint64_t)threadIdx.x * kScanItems;
+                unsigned long long v = 0;
+#pragma unroll
+                for (int i = 0; i < kScanItems; i++) v += (base + i < n_patterns && row[base + i]) ? 1u : 0u;
+                unsigned long long total;
+                block_exclusive_scan(v, &total);
+                if (threadIdx.x == 0) meta(s)[1 + t] = total;
+            }
+            grid.sync();
+            for (uint64_t tt = blockIdx.x; tt < tiles; tt += gridDim.x) {
+                const uint64_t s = tt / tpr, t = tt % tpr;
+                const uint32_t *const row = rows + s * rw;
+                const unsigned long long *const m = meta(s);
+                const unsigned long long hc = m[0], lo = E.unit_offsets[hc];
+                const unsigned long long tile_start = tile_prefix(m + 1, t);
+                const uint64_t base = t * kScanTile + (uint64_t)threadIdx.x * kScanItems;
+                uint32_t vals[kScanItems];
+                unsigned long long v = 0;
+#pragma unroll
+                for (int i = 0; i < kScanItems; i++) {
+                    vals[i] = base + i < n_patterns ? row[base + i] : 0u;
+                    v += vals[i] ? 1u : 0u;
+                }
+                unsigned long long total;
+                unsigned long long at = lo + tile_start + block_exclusive_scan(v, &total);
+#pragma unroll
+                for (int i = 0; i < kScanItems; i++)
+                    if (vals[i]) staged[at++] = make_uint4((uint32_t)hc, (uint32_t)(base + i), vals[i], 0u);
+                if (t == tpr - 1 && threadIdx.x == 0) E.unit_counts[hc] = (uint32_t)(tile_start + total);
+            }
+            grid.sync();
+        }
+        // phase 5 + 6: per-haystack offsets into the output
+        const uint64_t n_hay = (uint64_t)nh;
+        const uint64_t htiles = (n_hay + kScanTile - 1) / kScanTile;
+        for (uint64_t tt = blockIdx.x; tt < htiles; tt += gridDim.x) tile_sum_body<false>(E.unit_counts, 1, n_hay, E.tile_sums, tt, nullptr);
+        grid.sync();
+        for (uint64_t tt = blockIdx.x; tt < htiles; tt += gridDim.x) tile_apply_body<false>(E.unit_counts, 1, n_hay, E.tile_sums, E.match_offsets, tt);
+        grid.sync();
+        // pack: output o belongs to the last haystack h with match_offsets[h] <= o
+        const unsigned long long n_hits = E.match_offsets[n_hay];
+        for (unsigned long long o = first_i; o < n_hits; o += stride) {
+            uint64_t lo = 0, hi = n_hay;  // match_offsets[lo] <= o < match_offsets[hi]
+            while (hi - lo > 1) {
+                const uint64_t mid = (lo + hi) >> 1;
+                if (E.match_offsets[mid] <= o)
+                    lo = mid;
+                else
+                    hi = mid;
+            }
+            reinterpret_cast<uint4 *>(E.final_out)[o] = staged[E.unit_offsets[lo] + (o - E.match_offsets[lo])];
+        }
+        if (blockIdx.x == 0 && threadIdx.x == 0) E.totals[0] = n_hits;
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        if (!complete) E.totals[0] = 0;
+        E.totals[1] = complete ? 1 : 0;
+        E.totals[3] = complete ? n_long : 0;
+        E.totals[4] = raw_total > list_total ? raw_total : list_total;  // room the overlapping list needs
+        E.totals[5] = n_long * rw;                                      // row words needed (once the list fits)
         E.acc[kAccRaw] = E.acc[kAccGroups] = E.acc[kAccTraps] = E.acc[kAccRepairs] = 0;
         E.acc[kAccQueue] = 0;
     }
@@ -1931,6 +2203,22 @@ int launch_sieve_pattern_epilogue(SieveEpiArgs &E, unsigned long long *pattern_c
     return launch_cooperative(reinterpret_cast<const void *>(sieve_pattern_epilogue_kernel<MODE>), args, d, st);
 }
 
+// acb_pattern_hits' counter rows
+struct HitRows {
+    uint32_t *rows;
+    unsigned long long words;
+    uint32_t n_patterns;
+};
+
+template <int MODE>
+int launch_sieve_hits_epilogue(SieveEpiArgs &E, const HitRows &hr, const DeviceInfo &d, cudaStream_t st) {
+    uint32_t *rows = hr.rows;
+    unsigned long long words = hr.words;
+    uint32_t n_patterns = hr.n_patterns;
+    void *args[] = {&E, &rows, &words, &n_patterns};
+    return launch_cooperative(reinterpret_cast<const void *>(sieve_hits_epilogue_kernel<MODE>), args, d, st);
+}
+
 int sieve_header(const acb_automaton *a, SieveHeader &sh) {
     std::lock_guard<std::mutex> lock(a->impl->sieve_mutex);
     if (a->impl->sieve.size() < sizeof(SieveHeader)) return fail(ACB_EINVAL, "acb_sieve_build has not been called");
@@ -2000,11 +2288,12 @@ int check_ws(const acb_workspace *ws) {
 
 // The sieve's list scan: the scan kernel, then the ordering epilogue -- acb_scan_batch's kernel 5 (counts == null:
 // the list, or its selection, in dev_out), acb_count_non_overlapping (counts: the count epilogue writes them) or
-// acb_pattern_counts_non_overlapping (counts, by_pattern: the pattern epilogue adds to them).  For both counts the raw
-// records go to dev_raw and are ordered into dev_out, so that dev_raw is free for the pairs.
+// acb_pattern_counts_non_overlapping (counts, by_pattern: the pattern epilogue adds to them) or acb_pattern_hits (hits:
+// the hits epilogue, mode kModeOverlap for the overlapping search).  For the counts and the hits the raw records go to
+// dev_raw and are ordered into dev_out, so that dev_raw is free for the pairs.
 int sieve_list_scan(const acb_automaton *a, const void *dev_sieve, const Batch &B, uint64_t total_bytes, int mode, bool cp,
                     const uint32_t *pat_cplen, const acb_plan *plan, const acb_workspace *ws, const DeviceInfo &d, cudaStream_t st,
-                    unsigned long long *counts, bool by_pattern = false) {
+                    unsigned long long *counts, bool by_pattern = false, const HitRows *hits = nullptr) {
     const ImageHeader &h = a->impl->hdr;
     const int kind = (int)h.match_kind;
     const uint8_t *dev_bytes = B.bytes;
@@ -2041,7 +2330,7 @@ int sieve_list_scan(const acb_automaton *a, const void *dev_sieve, const Batch &
     uint32_t *cont_tail = reinterpret_cast<uint32_t *>(cont_cum + per_piece + 2);
     // a non-overlapping search orders the list into dev_raw's place and packs its selection into dev_out, so its
     // raw records go through dev_out first (a count packs nothing: dev_raw -> dev_out)
-    const bool in_raw = mode == kModeOverlap || counts;
+    const bool in_raw = mode == kModeOverlap || counts || hits;
     out.raw = in_raw ? ws->dev_raw : ws->dev_out;
     out.cap = cap;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
@@ -2087,7 +2376,11 @@ int sieve_list_scan(const acb_automaton *a, const void *dev_sieve, const Batch &
     E.totals = totals;
     E.acc = acc;
     E.match_offsets = match_offsets;
-    if (counts && by_pattern)
+    if (hits)
+        rc = mode == kModeStandard   ? launch_sieve_hits_epilogue<kModeStandard>(E, *hits, d, st)
+             : mode == kModeLeftmost ? launch_sieve_hits_epilogue<kModeLeftmost>(E, *hits, d, st)
+                                     : launch_sieve_hits_epilogue<kModeOverlap>(E, *hits, d, st);
+    else if (counts && by_pattern)
         rc = mode == kModeStandard ? launch_sieve_pattern_epilogue<kModeStandard>(E, counts, d, st) : launch_sieve_pattern_epilogue<kModeLeftmost>(E, counts, d, st);
     else if (counts)
         rc = mode == kModeStandard ? launch_sieve_count_epilogue<kModeStandard>(E, counts, d, st) : launch_sieve_count_epilogue<kModeLeftmost>(E, counts, d, st);
@@ -2100,15 +2393,16 @@ int sieve_list_scan(const acb_automaton *a, const void *dev_sieve, const Batch &
     return ACB_OK;
 }
 
-// acb_count_non_overlapping (by_pattern = false: counts per haystack, written) and acb_pattern_counts_non_overlapping
-// (by_pattern: counts per pattern, added to)
+// acb_count_non_overlapping (by_pattern = false: counts per haystack, written), acb_pattern_counts_non_overlapping
+// (by_pattern: counts per pattern, added to) and acb_pattern_hits (hits, dev_counts unused; either search)
 int non_overlapping_counts(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
                            int64_t n_haystacks, uint64_t total_bytes, const acb_plan *plan, const acb_workspace *ws,
-                           uint64_t *dev_counts, void *stream, bool by_pattern) {
-    if (!a || !dev_sieve || !dev_offsets || !plan || !dev_counts || (total_bytes && !dev_bytes)) return fail(ACB_EINVAL, "null argument");
+                           uint64_t *dev_counts, void *stream, bool by_pattern, const HitRows *hits = nullptr, bool overlapping = false) {
+    if (!a || !dev_sieve || !dev_offsets || !plan || (!dev_counts && !hits) || (total_bytes && !dev_bytes)) return fail(ACB_EINVAL, "null argument");
     if (int rc = check_ws(ws)) return rc;
     if (n_haystacks < 0 || n_haystacks > 0xfffffffell) return fail(ACB_EINVAL, "n_haystacks out of range (0 .. 2^32 - 2)");
     if (total_bytes >= (1ull << 31)) return fail(ACB_EINVAL, "total_bytes must be below 2^31 (scan larger inputs in windows)");
+    if (overlapping && a->impl->hdr.match_kind != ACB_STANDARD) return unsupported_overlapping(a);
     acb_plan want;
     acb_plan_scan(a, dev_bytes, total_bytes, (uint64_t)n_haystacks, &want);
     if (want.n_segments != plan->n_segments || want.segment_bytes != plan->segment_bytes || want.n_units != plan->n_units ||
@@ -2120,7 +2414,7 @@ int non_overlapping_counts(const acb_automaton *a, const void *dev_sieve, const 
     if (int rc = device_info(d)) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (n_haystacks == 0 || total_bytes == 0) {
-        if (n_haystacks && !by_pattern) CUDA_OK(cudaMemsetAsync(dev_counts, 0, (uint64_t)n_haystacks * sizeof(uint64_t), st));
+        if (n_haystacks && !by_pattern && !hits) CUDA_OK(cudaMemsetAsync(dev_counts, 0, (uint64_t)n_haystacks * sizeof(uint64_t), st));
         zero_outputs_kernel<<<(unsigned)((n_haystacks + 256) / 256), 256, 0, st>>>(
             reinterpret_cast<unsigned long long *>(ws->dev_unit_offsets), reinterpret_cast<unsigned long long *>(ws->dev_match_offsets),
             n_haystacks, reinterpret_cast<unsigned long long *>(ws->dev_total));
@@ -2128,9 +2422,9 @@ int non_overlapping_counts(const acb_automaton *a, const void *dev_sieve, const 
         CUDA_OK(cudaGetLastError());
         return ACB_OK;
     }
-    const int mode = a->impl->hdr.match_kind == ACB_STANDARD ? kModeStandard : kModeLeftmost;
+    const int mode = overlapping ? kModeOverlap : a->impl->hdr.match_kind == ACB_STANDARD ? kModeStandard : kModeLeftmost;
     return sieve_list_scan(a, dev_sieve, Batch{dev_bytes, dev_offsets, n_haystacks}, total_bytes, mode, false, nullptr, plan, ws, d, st,
-                           reinterpret_cast<unsigned long long *>(dev_counts), by_pattern);
+                           reinterpret_cast<unsigned long long *>(dev_counts), by_pattern, hits);
 }
 
 }  // namespace
@@ -2207,6 +2501,19 @@ int acb_pattern_counts_non_overlapping(const acb_automaton *a, const void *dev_s
                                        int64_t n_haystacks, uint64_t total_bytes, const acb_plan *plan, const acb_workspace *ws,
                                        uint64_t *dev_pattern_counts, void *stream) {
     return non_overlapping_counts(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, plan, ws, dev_pattern_counts, stream, true);
+}
+
+uint64_t acb_pattern_hit_row_words(uint64_t n_patterns) { return acb::hit_row_words(n_patterns); }
+
+int acb_pattern_hits(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                     int64_t n_haystacks, uint64_t total_bytes, int overlapping, const acb_plan *plan, const acb_workspace *ws,
+                     uint32_t *dev_rows, uint64_t row_words, void *stream) {
+    if (!a || (row_words && !dev_rows)) return fail(ACB_EINVAL, "null argument");
+    if (reinterpret_cast<uintptr_t>(dev_rows) & 7u) return fail(ACB_EINVAL, "dev_rows must be 8-byte aligned");
+    if (overlapping != 0 && overlapping != 1) return fail(ACB_EINVAL, "overlapping must be 0 or 1");
+    const HitRows hits{dev_rows, row_words, (uint32_t)a->impl->hdr.n_patterns};
+    return non_overlapping_counts(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, plan, ws, nullptr, stream, false, &hits,
+                                  overlapping != 0);
 }
 
 int acb_count_rows(const acb_automaton *a, const int64_t *dev_rows, uint64_t n_rows, uint64_t *dev_scratch, uint64_t *dev_count,

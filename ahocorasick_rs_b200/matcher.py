@@ -152,6 +152,7 @@ class _Automaton:
         self._hot = {}         # device index -> dict(tensor, rows, reprofile, calls, backoff)
         self._ws = {}          # (device index, slot) -> dict of tensors
         self._small = {}       # device index -> the small-call context
+        self._hit_row_words = 0   # hits_device: the counter-row words the largest call so far needed
         self.last_stats = {}
         self._lock = threading.RLock()   # (re-entered: any_device's table-walker path scans with scan_device under it)
         self._host_lock = threading.RLock()   # host-buffer calls: staging buffer + workspaces until the results are on the host
@@ -974,6 +975,157 @@ class _Automaton:
             d = host[:head + total_bytes].to(dev, non_blocking=True)
             return self.pattern_counts_device(d[head:], d[:8 * (n + 1)].view(torch.int64), overlapping).cpu().tolist()
 
+    # ---- hits per haystack: the distinct patterns of find_matches_as_indexes with their counts, without the list ----
+    def hits_device(self, data, offsets, overlapping=False, capacity: Optional[int] = None):
+        """Which patterns each haystack of a device-resident batch contains, and how often -> (row_offsets, patterns,
+        counts), int64 CUDA tensors of shapes (n + 1,), (k,) and (k,): haystack h's hits are
+        patterns[row_offsets[h]:row_offsets[h + 1]], ascending, each with how many records of its list in scan_device
+        have that pattern.  torch.sparse_csr_tensor(row_offsets, patterns, counts, size=(n, n_patterns)) is the matrix:
+        its row sums are count_device, its column sums pattern_counts_device.  The same in bytes and in code points.
+        An overlapping search on a leftmost automaton raises ValueError, as scan_device does.
+
+        Where the engine rule of scan_device picks the sieve: the sieve's list scan and a hits epilogue
+        (acb_pattern_hits), which waits for the device and scans again with more room when the list or the counter rows
+        did not fit.  Where the rule picks a table walker: torch.unique over haystack * n_patterns + pattern of its full
+        scan, which waits for it; the next scan that reuses the workspace waits for that.  Batches above WINDOW_BYTES go
+        in runs of whole haystacks; one haystack above it gets the nonzero entries of pattern_counts_device on it.
+        `capacity`: the workspace's first size, in records, as for scan_device."""
+        self.check_overlapping(overlapping)
+        torch = _require_cuda()
+        dev = data.device
+        n = offsets.numel() - 1
+        if n <= 0 or data.numel() == 0:
+            self.last_stats = {"engine": None, "mode": "matching_patterns", "long_stretches": 0, "rows": 0, "list_records": 0, "hits": 0}
+            empty = torch.zeros(0, dtype=torch.int64, device=dev)
+            return torch.zeros(max(n, 0) + 1, dtype=torch.int64, device=dev), empty, empty.clone()
+        if data.numel() > self.WINDOW_BYTES:
+            return self._hits_windows(data, offsets, overlapping)
+        P = self.n_patterns
+        with self._lock, torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev)
+            if self._pick_engine(dev, data, offsets, overlapping) is not None:
+                m, _, _ = self.scan_device(data, offsets, overlapping, False)
+                keys, counts = torch.unique(m[:, 0].long() * P + m[:, 1].long(), return_counts=True)
+                row_offsets = torch.searchsorted(keys, torch.arange(n + 1, dtype=torch.int64, device=dev) * P)
+                reader = torch.cuda.Event()
+                reader.record(stream)
+                self._ws[(dev.index if dev.index is not None else torch.cuda.current_device(), 0)]["reader"] = reader
+                self.last_stats = {"engine": self.last_stats.get("engine", "table"), "mode": "matching_patterns", "long_stretches": 0,
+                                   "rows": 0, "list_records": int(m.shape[0]), "hits": int(keys.numel())}
+                return row_offsets, keys % P, counts
+            sieve_t, _ = self.sieve(dev)
+            plan = self._plan(data, n)
+            cap = capacity or max(1024, n * 2)
+            row_words = self._hit_row_words
+            rows = None
+            while True:
+                ws = self._workspace(dev, plan, n, cap, 0)
+                reader = ws.pop("reader", None)
+                if reader is not None:   # a comparison of an earlier call (maybe on another stream) reads this workspace first
+                    stream.wait_event(reader)
+                if row_words and (rows is None or rows.numel() < row_words):
+                    rows = torch.empty(row_words, dtype=torch.int32, device=dev)
+                st = self._ws_struct(ws)
+                rc = self._L.acb_pattern_hits(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
+                                              int(bool(overlapping)), C.byref(plan), C.byref(st),
+                                              rows.data_ptr() if rows is not None else None, row_words, stream.cuda_stream)
+                if rc != _capi.ACB_OK:
+                    err = _capi.last_error()
+                    ws["scratch"][:8].zero_()   # a scan that failed half way may have left its counters dirty
+                    raise (ValueError if rc == _capi.ACB_EUNSUPPORTED else RuntimeError)(err)
+                hits, complete, long_stretches, n_rows, raw_total, need_words = ws["total"].tolist()[:6]
+                if complete:
+                    break
+                if raw_total <= ws["capacity"] and need_words <= row_words:
+                    raise RuntimeError("acb_pattern_hits reported an incomplete result with enough room")
+                if raw_total > ws["capacity"]:
+                    cap = raw_total + raw_total // 8 + 16
+                row_words = max(row_words, need_words)
+            self._hit_row_words = max(self._hit_row_words, need_words)   # (the next call with as many long stretches fits at once)
+            row_offsets = ws["match_offsets"][: n + 1].clone()
+            out = ws["out"][:hits]
+            patterns, counts = out[:, 1].long(), out[:, 2].long()
+            reader = torch.cuda.Event()
+            reader.record(stream)
+            ws["reader"] = reader
+            self.last_stats = {"engine": "sieve", "mode": "matching_patterns", **self.sieve_geometry(dev, plan.task_bytes),
+                               "list_records": raw_total, "long_stretches": long_stretches, "rows": n_rows, "hits": hits}
+            return row_offsets, patterns, counts
+
+    def _hits_windows(self, data, offsets, overlapping):
+        """hits_device for buffers above WINDOW_BYTES: runs of whole haystacks that fit one call each give their rows;
+        one haystack above the limit gets the nonzero entries of pattern_counts_device (which windows it).  last_stats
+        sums the runs'."""
+        torch = _require_cuda()
+        dev = data.device
+        n = offsets.numel() - 1
+        limit = self.WINDOW_BYTES
+        lens = offsets[1:] - offsets[:-1]
+        oversized = bool((lens > limit).any().item())
+        sizes, patterns, counts = [], [], []
+        stats = {"long_stretches": 0, "rows": 0, "list_records": 0}
+        engine = None
+        h = 0
+        while h < n:
+            start = int(offsets[h].item())
+            if oversized and int(lens[h].item()) > limit:
+                size = int(lens[h].item())
+                pc = self.pattern_counts_device(data[start:start + size], torch.tensor([0, size], dtype=torch.int64, device=dev), overlapping)
+                pids = torch.nonzero(pc).flatten()
+                sizes.append(torch.tensor([pids.numel()], dtype=torch.int64, device=dev))
+                patterns.append(pids)
+                counts.append(pc[pids])
+                h += 1
+                continue
+            # the longest run of whole haystacks that fits one call (and stops before an oversized one)
+            h1 = int(torch.searchsorted(offsets, torch.tensor([start + limit], dtype=torch.int64, device=dev), right=True).item()) - 1
+            h1 = max(h + 1, min(h1, n))
+            if oversized:
+                big = torch.nonzero(lens[h:h1] > limit)
+                if big.numel():
+                    h1 = h + int(big[0].item())
+            end = int(offsets[h1].item())
+            ro, p, c = self.hits_device(data[start:end], offsets[h:h1 + 1] - start, overlapping)
+            sizes.append(ro[1:] - ro[:-1])
+            patterns.append(p)
+            counts.append(c)
+            for k in stats:
+                stats[k] += self.last_stats.get(k, 0)
+            engine = self.last_stats.get("engine") or engine
+            h = h1
+        row_offsets = torch.zeros(n + 1, dtype=torch.int64, device=dev)
+        torch.cumsum(torch.cat(sizes), 0, out=row_offsets[1:])
+        patterns, counts = torch.cat(patterns), torch.cat(counts)
+        self.last_stats = {"engine": engine, "mode": "matching_patterns", **stats, "hits": int(patterns.numel()), "windows": True}
+        return row_offsets, patterns, counts
+
+    def hits_host_batch(self, chunks: Sequence[bytes], overlapping):
+        """Host buffers (bytes-like objects, one per haystack) -> one list per haystack: the distinct pattern ids of its
+        matches, ascending.  The offsets and the haystacks are gathered into the pinned staging buffer and go to the
+        device in one copy."""
+        torch = _require_cuda()
+        self.check_overlapping(overlapping)
+        n = len(chunks)
+        if n == 0:
+            return []
+        offs = np.zeros(n + 1, dtype=np.int64)
+        np.cumsum(np.fromiter((len(c) for c in chunks), dtype=np.int64, count=n), out=offs[1:])
+        total_bytes = int(offs[-1])
+        head = (8 * (n + 1) + 511) & ~511   # the offsets, then the bytes at a 512-byte boundary of the buffer
+        dev = torch.device("cuda", torch.cuda.current_device())
+        with self._host_lock:
+            host = self._pinned(head + total_bytes)
+            hv = host.numpy()
+            hv[:8 * (n + 1)].view(np.int64)[:] = offs
+            if n == 1:
+                hv[head:head + total_bytes] = np.frombuffer(chunks[0], dtype=np.uint8)
+            elif total_bytes:
+                hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
+            d = host[:head + total_bytes].to(dev, non_blocking=True)
+            ro, p, _ = self.hits_device(d[head:], d[:8 * (n + 1)].view(torch.int64), overlapping)
+            ro, p = ro.cpu().tolist(), p.cpu().tolist()
+        return [p[ro[i]:ro[i + 1]] for i in range(n)]
+
     def scan_device(self, data, offsets, overlapping=False, codepoints=False, capacity: Optional[int] = None,
                     sync: bool = True, ws_slot: int = 0):
         """Scan a device-resident batch.  data: uint8 CUDA tensor, offsets: int64
@@ -1695,6 +1847,29 @@ class AhoCorasick:
         (see _Automaton.pattern_counts_device)."""
         return self._ac.pattern_counts_device(data, offsets, overlapping)
 
+    # ---- additions: the patterns each haystack contains ---------------------------------------------------------
+    def matching_patterns(self, haystack: str, overlapping: bool = False) -> list:
+        """-> the distinct pattern ids of ``find_matches_as_indexes(haystack, overlapping)``, ascending, found without
+        building the list."""
+        if not isinstance(haystack, str):
+            raise TypeError("argument 'haystack': 'str' expected")
+        self._ac.check_overlapping(overlapping)
+        return self._ac.hits_host_batch([haystack.encode("utf-8")], overlapping)[0]
+
+    def matching_patterns_batch(self, haystacks: Sequence[str], overlapping: bool = False) -> list:
+        """``matching_patterns`` for each haystack, in one transfer and one scan."""
+        hays = list(haystacks)
+        for h in hays:
+            if not isinstance(h, str):
+                raise TypeError("argument 'haystack': 'str' expected")
+        self._ac.check_overlapping(overlapping)
+        return self._ac.hits_host_batch([h.encode("utf-8") for h in hays], overlapping)
+
+    def matching_patterns_device(self, data, offsets, overlapping: bool = False):
+        """Device-resident UTF-8 batch -> (row_offsets, patterns, counts), the CSR form of each haystack's per-pattern
+        match counts (see _Automaton.hits_device); the same in bytes and in code points."""
+        return self._ac.hits_device(data, offsets, overlapping)
+
     # ---- additions: stream search (data fed in chunks; the crate's stream_find_iter, for every match kind) -------------
     def stream(self, overlapping: bool = False) -> Stream:
         """One stream fed ``str`` chunks: ``feed(chunk)`` returns the rows (pattern, start, end) it releases, in code
@@ -1811,6 +1986,25 @@ class BytesAhoCorasick:
         """Device-resident batch -> int64 tensor (n_patterns,) of match counts per pattern over the whole batch (see
         _Automaton.pattern_counts_device)."""
         return self._ac.pattern_counts_device(data, offsets, overlapping)
+
+    # ---- additions: the patterns each haystack contains ---------------------------------------------------------
+    def matching_patterns(self, haystack, overlapping: bool = False) -> list:
+        """-> the distinct pattern ids of ``find_matches_as_indexes(haystack, overlapping)``, ascending, found without
+        building the list."""
+        hay = _as_buffer_bytes(haystack)
+        self._ac.check_overlapping(overlapping)
+        return self._ac.hits_host_batch([hay], overlapping)[0]
+
+    def matching_patterns_batch(self, haystacks: Sequence, overlapping: bool = False) -> list:
+        """``matching_patterns`` for each haystack, in one transfer and one scan."""
+        hays = [_as_buffer_bytes(h) for h in haystacks]
+        self._ac.check_overlapping(overlapping)
+        return self._ac.hits_host_batch(hays, overlapping)
+
+    def matching_patterns_device(self, data, offsets, overlapping: bool = False):
+        """Device-resident batch -> (row_offsets, patterns, counts), the CSR form of each haystack's per-pattern match
+        counts (see _Automaton.hits_device)."""
+        return self._ac.hits_device(data, offsets, overlapping)
 
     # ---- additions: stream search (data fed in chunks; the crate's stream_find_iter, for every match kind) -------------
     def stream(self, overlapping: bool = False) -> Stream:

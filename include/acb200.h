@@ -375,6 +375,44 @@ int acb_pattern_counts_non_overlapping(const acb_automaton *a, const void *dev_s
                                        uint64_t *dev_pattern_counts, void *stream);
 
 /*
+ * Which patterns each haystack contains, and how often: for haystack h, with R_h the reference's result
+ * find_matches_as_indexes(h, overlapping) (get_matches, src/lib.rs:42-68), the HITS of h are the pairs (p, c) where p
+ * is a pattern id occurring in R_h and c the number of records of R_h with pattern p, p ascending.  Patterns with the
+ * same bytes keep their own ids (non-overlapping: the lower id takes the match).  The row sums are the per-haystack
+ * counts of acb_count_*; the column sums are acb_pattern_counts_*.  The list is never handed back.
+ *
+ * The sieve's list scan (plan and workspace as for acb_count_non_overlapping, kernel 5 whatever the tuning), then one
+ * epilogue that places the overlapping list, selects each haystack's matches (overlapping: all of them) and aggregates
+ * their patterns.  A haystack whose overlapping list has at most ACB_LONG_STRETCH records is aggregated by one warp
+ * (a sort of its pids); a longer one gets a counter row in dev_rows.  A row is acb_pattern_hit_row_words(n_patterns)
+ * u32 words: n_patterns counters, padded to an even count, then 8-byte bookkeeping (the haystack, then one word per
+ * 2048 counters).  dev_rows must be 8-byte aligned and hold row_words words; it may be null when row_words == 0.
+ *
+ * Outputs: ws->dev_out = the hits as acb_pattern_hit records, grouped by haystack, patterns ascending within each;
+ * ws->dev_match_offsets = u64[n_haystacks + 1] bracketing each haystack's hits.  ws->dev_total: [0] = hits, [1] = 1
+ * when the result is complete (0: the list did not fit the workspace or row_words was too small; NOTHING valid was
+ * written, and [4] / [5] say how much room a second call needs), [2] = haystacks selected on the grid (lists of more than
+ * ACB_LONG_STRETCH records), [3] = haystacks aggregated in a counter row, [4] = records of the overlapping list, [5] =
+ * counter-row words needed (known once the list fits; at most [4] / (ACB_LONG_STRETCH + 1) rows).  ws->dev_raw,
+ * ws->dev_raw_seq and dev_rows are overwritten.  Two launches, no synchronisation.  A u32 count suffices: one call
+ * addresses fewer than 2^31 bytes, and a pattern matches at most once per end position.
+ *
+ * overlapping = 1 on a leftmost automaton returns ACB_EUNSUPPORTED before any byte is read, like the reference.
+ * Argument checks, the 2^31 limit and the empty cases are those of acb_count_non_overlapping (ACB_EINVAL before any
+ * CUDA call), plus overlapping outside {0, 1} and a misaligned dev_rows.
+ */
+typedef struct acb_pattern_hit {
+    uint32_t haystack; /* index into the batch */
+    uint32_t pattern;  /* pattern id */
+    uint32_t count;    /* records of the haystack's result with this pattern */
+    uint32_t reserved; /* 0 */
+} acb_pattern_hit;     /* 16 bytes, like acb_match */
+uint64_t acb_pattern_hit_row_words(uint64_t n_patterns);
+int acb_pattern_hits(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                     int64_t n_haystacks, uint64_t total_bytes, int overlapping, const acb_plan *plan, const acb_workspace *ws,
+                     uint32_t *dev_rows, uint64_t row_words, void *stream);
+
+/*
  * Stream search: matches in data that arrives in chunks, for many streams at once.  A stream is the concatenation of
  * the chunks fed to it; positions are absolute within it and 64-bit.  The crate the reference wraps has the single-stream,
  * Standard, non-overlapping form (AhoCorasick::stream_find_iter); here every match kind and overlapping Standard are
