@@ -1319,6 +1319,7 @@ class _Automaton:
         total_bytes = int(offs[-1] - offs[0]) if n > 0 else 0
         dev = torch.device("cuda", torch.cuda.current_device())
         chunk = int(chunk_bytes or self.HOST_CHUNK_BYTES)
+        chunk = min(chunk, self.WINDOW_BYTES)   # every run is one kernel call (scanned with sync=False: no window path)
         with self._host_lock:
             if n <= 0 or total_bytes <= chunk or int(np.max(np.diff(offs))) > self.WINDOW_BYTES:
                 # one shot (small input), or the oversized-haystack window path
