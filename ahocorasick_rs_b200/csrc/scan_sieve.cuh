@@ -112,11 +112,6 @@ struct SievePlan {
 __device__ __forceinline__ void sts128(uint32_t addr, uint4 v) {
     asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};\n" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
-__device__ __forceinline__ uint32_t lds32v(uint32_t addr) {
-    uint32_t v;
-    asm volatile("ld.shared.u32 %0, [%1];\n" : "=r"(v) : "r"(addr));
-    return v;
-}
 // (hi:lo) >> (s & 31), low word
 __device__ __forceinline__ uint32_t shf_r_wrap(uint32_t lo, uint32_t hi, uint32_t s) {
     uint32_t d;

@@ -19,10 +19,12 @@
 //        in is redone, through the exact scanner.  (Addresses must fit 16 bits:
 //        the table lives in the first 64 KB of shared memory.)
 //   [ column map : 256 B ]  (kColClass only)
-//   [ mbarrier, stream bounds ]
+//   [ mbarrier, stream bounds; each warp's current task ]
 //   [ hot2full : (H + 1) x u32 ]  hot row -> automaton state, for the segment
 //        summaries and the hand-over to the exact scanner
-//   [ copy metadata : per warp 32 V x (first 16-byte unit, number of chunks) ]
+//   [ metadata : per warp 32 V x (first 16-byte unit, number of chunks, guessed start
+//        state, how the first chunk is fetched) ]  the first two are read by the copy
+//        issue; the guess waits there for the segment summary
 //   [ staging : per warp, 2 buffers x 32 V rows x 64 B ]  lane l's 64-byte
 //        chunk is row l, with its four 16-byte units XOR-swizzled by
 //        (l >> 1) & 3: the per-lane LDS.128 reads of a quarter warp hit 8
@@ -57,6 +59,18 @@
 // is what keeps the warps fed.  The copy of the chunk that completes a line
 // marks it evict_first, so the spent stream leaves the L2 first (DESIGN.md §6;
 // a third staging buffer and L2 prefetches of a lane's later bytes were slower).
+// The warm-up bytes are the exception: they end the neighbouring segment's last
+// line, so the first chunk of such a segment copies only the 16-byte units that
+// hold them, sector by sector, and leaves the line to the lane that scans it.
+//
+// Where a lane's state lives.  The chunk loop keeps position, table row, piece
+// end and a few predicates per segment in registers.  The exact scanner's state
+// and the segment bookkeeping (PieceCtx, LaneSeg: 28 words in local memory)
+// exist only for a lane that has needed the exact scanner: it builds them then
+// (seg_setup + build_cold) from the task number, its lane and the guess in its
+// metadata row.  A lane that stays on the fast path -- all but about 2 % of
+// config 2's -- writes its summary from registers and shared memory and never
+// touches local memory.
 #pragma once
 #include <type_traits>
 
@@ -75,8 +89,10 @@ constexpr int kMaxWarps2 = ACB_MAX_WARPS2;  // two segments per lane: twice the 
 constexpr int kChunk = 64;                // bytes per lane per stage
 constexpr int kRow = kChunk;              // a lane's row in the staging buffer; its 16-byte units are swizzled by (lane >> 1) & 3
 constexpr int kStageBytes = 32 * kRow;    // per warp per buffer and per segment of a lane
-constexpr int kStageOffset = 256 + 128;   // column map + mbarrier slot, after the hot table
-constexpr int kMetaBytes = 32 * 8;        // per warp and per segment of a lane: (first 16-byte unit, chunk count), read by the copy issue
+constexpr int kStageOffset = 256 + 128 + 4 * kMaxWarps;  // column map, mbarrier slot + stream bounds, each warp's current task, after the hot table
+constexpr int kMetaRow = 16;              // per segment of a lane: first 16-byte unit and chunk count (read by the copy issue), the guessed
+                                          // state at the segment start, how the first chunk is fetched (SegSetup::first_fetch)
+constexpr int kMetaBytes = 32 * kMetaRow; // per warp and per segment of a lane
 
 struct FastTab {
     uint32_t cmap;  // shared address of the byte -> column map (kColClass)
@@ -112,6 +128,12 @@ __device__ __forceinline__ uint32_t lds32(uint32_t addr) {
     asm("ld.shared.u32 %0, [%1];\n" : "=r"(v) : "r"(addr));  // (only used on tables that never change after the prologue)
     return v;
 }
+__device__ __forceinline__ uint32_t lds32v(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.u32 %0, [%1];\n" : "=r"(v) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;\n" ::"r"(addr), "r"(v) : "memory"); }
 __device__ __forceinline__ uint2 lds64(uint32_t addr) {
     uint2 v;
     asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];\n" : "=r"(v.x), "=r"(v.y) : "r"(addr));
@@ -193,6 +215,11 @@ __device__ __forceinline__ void cp_async16_last(uint32_t dst_smem, const void *s
         "}\n" ::"r"(dst_smem), "l"(src), "r"(src_bytes)
         : "memory");
 }
+// A plain 16-byte copy, no prefetch size and no policy: DRAM supplies one 32-byte sector.  For the warm-up bytes before a
+// segment: the rest of their 128-byte line belongs to the neighbouring segment, whose lane reads it at another time.
+__device__ __forceinline__ void cp_async16_sector(uint32_t dst_smem, const void *src, uint32_t src_bytes) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst_smem), "l"(src), "r"(src_bytes) : "memory");
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;\n" ::: "memory"); }
 
@@ -247,7 +274,100 @@ struct LaneSeg {
     uint32_t far;        // code points: the segment starts more than kContSpan segments into its haystack
 };
 
-// The current piece is finished (c.at >= c.stop, nothing pending): move on.  Either starts the next
+// Where a lane's segment lies and how its scan starts: a pure function of the task, the lane and the batch.  The task
+// start keeps what the chunk loop needs in registers; the rest is derived again when a lane first needs the exact
+// scanner (build_cold), so a lane that never does stores none of it.
+struct SegSetup {
+    int64_t seg, org, hs;     // segment index; stream position of relative position 0 (a 64-byte aligned address); start of the haystack
+    uint32_t h;               // the haystack the scan starts in
+    uint32_t lo_rel, hi_rel;  // the segment, relative to org
+    uint32_t at, limit;       // where the scan starts (the warm-up bytes before lo_rel, if any), and the end of the haystack
+    uint32_t off16;           // 16-byte unit of org on the copy grid
+    uint32_t first_fetch;     // a warm-up: kWarmFetch | first 16-byte unit of chunk 0 that the scan reads; else 0
+    bool live, outside;       // has bytes to scan; lies in the plan but outside the stream (an empty summary is due)
+    bool cont;                // begins inside a haystack: `warm` bytes before it are scanned silently first
+};
+constexpr uint32_t kWarmFetch = 0x80000000u;
+
+template <int V>
+__device__ __forceinline__ int64_t seg_of_lane(const SegPlan &P, unsigned int task, uint32_t vlane) {
+    const uint32_t q = P.lane_stride;
+    return (int64_t)(((uint64_t)(task / q) * (32u * V) + vlane) * q + task % q);
+}
+
+template <int V>
+__device__ __forceinline__ SegSetup seg_setup(const SegPlan &P, const Batch &B, int64_t stream_lo, int64_t stream_hi, uintptr_t gbase,
+                                              unsigned int task, uint32_t vlane) {
+    SegSetup u;
+    u.seg = seg_of_lane<V>(P, task, vlane);
+    u.org = u.hs = 0;
+    u.h = u.lo_rel = u.hi_rel = u.at = u.limit = u.off16 = u.first_fetch = 0;
+    u.cont = false;
+    const int64_t glo = P.origin + u.seg * (int64_t)P.seg_bytes;
+    const int64_t lo = max(glo, stream_lo), hi = min(glo + (int64_t)P.seg_bytes, stream_hi);
+    u.live = u.seg < P.n_segments && lo < hi;
+    u.outside = u.seg < P.n_segments && lo >= hi;  // (the plan is sized from the buffer length)
+    if (u.live) {
+        // the haystack containing lo: try the position an equal-length batch would put it at, else search
+        // (32-bit arithmetic: a buffer is shorter than 4 GiB)
+        int64_t h = P.avg_len ? (int64_t)((uint32_t)(lo - stream_lo) / (uint32_t)P.avg_len) : 0;
+        if (h >= B.n_haystacks) h = B.n_haystacks - 1;
+        int64_t hs = __ldg(B.offsets + h), he = __ldg(B.offsets + h + 1);
+        if (!(hs <= lo && lo < he)) {
+            h = find_haystack(B, lo);
+            hs = __ldg(B.offsets + h);
+            he = __ldg(B.offsets + h + 1);
+        }
+        u.cont = hs < lo;
+        const int64_t w = u.cont ? max(hs, lo - (int64_t)P.warm) : lo;
+        const uintptr_t pw = reinterpret_cast<uintptr_t>(B.bytes + w);
+        const uintptr_t a0 = pw & ~uintptr_t(kChunk - 1);
+        u.org = w - (int64_t)(pw - a0);
+        u.hs = hs;
+        u.h = (uint32_t)h;
+        u.lo_rel = (uint32_t)(lo - u.org);
+        u.hi_rel = (uint32_t)(hi - u.org);
+        u.at = (uint32_t)(w - u.org);
+        u.limit = (uint32_t)(he - u.org);
+        u.off16 = (uint32_t)((a0 - gbase) >> 4);
+        u.first_fetch = u.cont ? kWarmFetch | (u.at >> 4) : 0u;
+    }
+    return u;
+}
+
+// The exact scanner's state and the segment bookkeeping of a lane that has only run the fast path so far: nothing
+// reported, nothing pending.  `warm`: still in the warm-up; else `spec` is the state guessed at the segment start
+// (kNoState when the segment starts its haystack).  c.at, c.state and the code-point counters are the caller's.
+template <bool CP>
+__device__ __forceinline__ void build_cold(PieceCtx &c, LaneSeg &L, const SegSetup &u, const SegPlan &P, const Batch &B, bool warm,
+                                           uint32_t spec) {
+    L.org = u.org;
+    L.seg = u.seg;
+    L.lo_rel = u.lo_rel;
+    L.hi_rel = u.hi_rel;
+    L.h = u.h;
+    L.kind = !u.cont ? kPieceNormal : warm ? kPieceWarm : kPieceHead;
+    L.spec_state = warm ? kNoState : spec;
+    L.head_count = 0;
+    L.done = 0;
+    L.far = CP && u.cont && u.seg - (u.hs - P.origin) / (int64_t)P.seg_bytes > kContSpan;
+    c.base = B.bytes + u.org;
+    c.at = u.at;
+    c.stop = warm ? u.lo_rel : min(u.hi_rel, u.limit);
+    c.limit = u.limit;
+    c.emit_from = warm ? 0xffffffffu : 0u;  // the warm-up reports nothing
+    c.state = kRoot;
+    c.have = 0;
+    c.last_pid = c.last_end = 0;
+    c.hay = u.h;
+    c.hay_delta = (uint32_t)(u.org - u.hs);
+    c.unit = (uint32_t)(2 * u.seg + 1);
+    c.nemit = 0;
+    c.cp_pos = u.at;
+    c.cp_cont = 0;
+}
+
+// The current piece is finished (c.at >= c.stop, nothing pending): move on. Either starts the next
 // piece (c.at = its first byte, c.state = its start state) or sets L.done and writes the segment summary.
 template <int MODE, bool CP>
 __device__ __forceinline__ void advance_piece(PieceCtx &c, LaneSeg &L, const Batch &B, const Sink &out, const SegOut &seg_out) {
@@ -420,14 +540,14 @@ scan_staged_kernel(DevImage im, DevHot hot_img, Batch B, SegPlan P, Sink out, Se
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     constexpr uint32_t kRows = 32 * V;                 // virtual lanes (segments) per warp-task
     constexpr uint32_t kBufBytes = kRows * kRow;       // one staging buffer of a warp
-    constexpr uint32_t kWarpMeta = kRows * 8;
+    constexpr uint32_t kWarpMeta = kRows * kMetaRow;
     const uint32_t meta_s = stage_all_s + warp * kWarpMeta;
     const uint32_t stage_s = stage_all_s + (blockDim.x >> 5) * kWarpMeta + warp * 2 * kBufBytes;
     const uintptr_t gbase = reinterpret_cast<uintptr_t>(B.bytes + P.origin);  // 64-byte aligned by construction of the plan
     // copy instruction i of a stage moves 16-byte unit (lane & 3) of row (i * 8 + lane / 4); the unit's
     // place in its row is swizzled by (row >> 1) & 3, which does not depend on i
     const uint32_t cp_dst = stage_s + (lane >> 2) * kRow + (((lane & 3) ^ ((lane >> 3) & 3)) << 4);
-    const uint32_t cp_meta = meta_s + (lane >> 2) * 8;
+    const uint32_t cp_meta = meta_s + (lane >> 2) * kMetaRow;
     // this lane's rows (virtual lanes lane, lane + 32, ...): the address of unit 0 of the first
     const uint32_t row_s = stage_s + lane * kRow + (((lane >> 1) & 3) << 4);
     const uint32_t q = P.lane_stride;
@@ -436,11 +556,15 @@ scan_staged_kernel(DevImage im, DevHot hot_img, Batch B, SegPlan P, Sink out, Se
     // The exact scanner's state and the segment bookkeeping live in LOCAL memory on purpose (their
     // addresses are laundered through an empty asm so the compiler cannot promote the ~28 words per
     // segment to registers): only the careful path touches them, and the chunk loop needs the registers.
+    // They are built when a lane first hands over to the exact scanner (cold(), below), about 2 % of the
+    // segments of config 2; until then a lane's state is its registers, its guessed start state in the
+    // metadata row and the warp's task number in shared memory.
     PieceCtx c_mem[V];
     LaneSeg L_mem[V];
     PieceCtx *c_ptr = c_mem;
     LaneSeg *L_ptr = L_mem;
     asm volatile("" : "+l"(c_ptr), "+l"(L_ptr));
+    const uint32_t task_s = bar_s + 128 + warp * 4;  // this warp's current task (not kept in a register across the chunk loop)
 
     // Warp-tasks (32 * V segments, lane_stride apart) come from an atomic counter.  The claim for the NEXT task
     // is issued when the last chunk of the current one starts: the atomic's round trip overlaps that chunk,
@@ -456,82 +580,33 @@ scan_staged_kernel(DevImage im, DevHot hot_img, Batch B, SegPlan P, Sink out, Se
         uint32_t pos[V], s[V], stop[V], cpd[V];
         uint32_t hi_rel[V], stop_head[V];  // the segment end, and where the head piece (after the warm-up) stops
         bool done[V], warm[V];  // warm: the current piece is the silent warm-up before the segment
+        bool cold[V];           // PieceCtx / LaneSeg have been built: from then on they are the segment's record
         uint32_t nch_max = 0;
         __syncwarp();  // the previous task no longer reads meta / the staging buffers
+        if (lane == 0) sts32(task_s, task);
         const int64_t stream_lo = bounds[0], stream_hi = bounds[1];
 #pragma unroll
         for (int t = 0; t < V; t++) {
-            PieceCtx &c = c_ptr[t];
-            LaneSeg &L = L_ptr[t];
-            L.seg = (int64_t)(((uint64_t)(task / q) * kRows + (uint32_t)t * 32u + lane) * q + task % q);
-            L.done = 1;
-            L.spec_state = kNoState;
-            L.head_count = 0;
-            L.far = 0;
-            uint32_t off16 = 0, nchunks = 0;
-            pos[t] = 0;
+            const SegSetup u = seg_setup<V>(P, B, stream_lo, stream_hi, gbase, task, (uint32_t)t * 32u + lane);
+            if (u.outside) write_summary(seg_out, u.seg, kNoState, kRoot, 0u, 0u, 0u, 0u, false);  // nothing to scan
+            // the first piece is never empty (lo < hi, and a warm-up starts before lo) and starts in the
+            // root state, which is hot row 0: straight into the fast path
+            pos[t] = u.at;
             s[t] = hot_s;
-            stop[t] = 0;
+            stop[t] = u.cont ? u.lo_rel : min(u.hi_rel, u.limit);
             cpd[t] = 0;
-            warm[t] = false;
-            hi_rel[t] = stop_head[t] = 0;
-            const int64_t glo = P.origin + L.seg * (int64_t)P.seg_bytes;
-            const int64_t lo = max(glo, stream_lo), hi = min(glo + (int64_t)P.seg_bytes, stream_hi);
-            if (L.seg < P.n_segments && lo >= hi) {
-                // a segment outside the stream (the plan is sized from the buffer length): nothing to scan
-                write_summary(seg_out, L.seg, kNoState, kRoot, 0u, 0u, 0u, 0u, false);
-            } else if (L.seg < P.n_segments) {
-                // the haystack containing lo: try the position an equal-length batch would put it at, else search
-                // (32-bit arithmetic: a buffer is shorter than 4 GiB)
-                int64_t h = P.avg_len ? (int64_t)((uint32_t)(lo - stream_lo) / (uint32_t)P.avg_len) : 0;
-                if (h >= B.n_haystacks) h = B.n_haystacks - 1;
-                int64_t hs = __ldg(B.offsets + h), he = __ldg(B.offsets + h + 1);
-                if (!(hs <= lo && lo < he)) {
-                    h = find_haystack(B, lo);
-                    hs = __ldg(B.offsets + h);
-                    he = __ldg(B.offsets + h + 1);
-                }
-                const bool cont = hs < lo;
-                const int64_t w = cont ? max(hs, lo - (int64_t)P.warm) : lo;
-                const uintptr_t pw = reinterpret_cast<uintptr_t>(B.bytes + w);
-                const uintptr_t a0 = pw & ~uintptr_t(kChunk - 1);
-                L.org = w - (int64_t)(pw - a0);
-                L.lo_rel = (uint32_t)(lo - L.org);
-                L.hi_rel = (uint32_t)(hi - L.org);
-                L.h = (uint32_t)h;
-                L.kind = cont ? kPieceWarm : kPieceNormal;
-                L.done = 0;
-                L.far = CP && cont && L.seg - (hs - P.origin) / (int64_t)P.seg_bytes > kContSpan;
-                off16 = (uint32_t)((a0 - gbase) >> 4);
-                nchunks = (L.hi_rel + kChunk - 1) / kChunk;
-                c.base = B.bytes + L.org;
-                c.at = (uint32_t)(w - L.org);
-                c.limit = (uint32_t)(he - L.org);
-                c.stop = cont ? L.lo_rel : min(L.hi_rel, c.limit);
-                c.emit_from = cont ? 0xffffffffu : 0u;  // the warm-up reports nothing
-                c.state = kRoot;
-                c.have = 0;
-                c.last_pid = c.last_end = 0;
-                c.hay = (uint32_t)h;
-                c.hay_delta = (uint32_t)(L.org - hs);
-                c.unit = (uint32_t)(2 * L.seg + 1);
-                c.nemit = 0;
-                c.cp_pos = c.at;
-                c.cp_cont = 0;
-                warm[t] = cont;
-                // the first piece is never empty (lo < hi, and a warm-up starts before lo) and starts in the
-                // root state, which is hot row 0: straight into the fast path
-                pos[t] = c.at;
-                stop[t] = c.stop;
-                hi_rel[t] = L.hi_rel;
-                stop_head[t] = min(L.hi_rel, c.limit);
-            }
-            done[t] = L.done != 0;
-            if (done[t]) nchunks = 0;
+            hi_rel[t] = u.hi_rel;
+            stop_head[t] = min(u.hi_rel, u.limit);
+            warm[t] = u.cont;
+            done[t] = !u.live;
+            cold[t] = false;
+            const uint32_t nchunks = u.live ? (u.hi_rel + kChunk - 1) / kChunk : 0u;
             nch_max = max(nch_max, nchunks);
             // where each row's bytes are: read back by whichever lane copies them (no shuffles in the loop:
             // the compiler cannot prove the warp converged there and would emit a slow collective path)
-            sts64(meta_s + ((uint32_t)t * 32u + lane) * 8, make_uint2(off16, nchunks));
+            const uint32_t m = meta_s + ((uint32_t)t * 32u + lane) * kMetaRow;
+            sts64(m, make_uint2(u.off16, nchunks));
+            sts64(m + 8, make_uint2(kNoState, u.first_fetch));
         }
         const uint32_t kmax = __reduce_max_sync(0xffffffffu, nch_max);
         __syncwarp();
@@ -540,7 +615,7 @@ scan_staged_kernel(DevImage im, DevHot hot_img, Batch B, SegPlan P, Sink out, Se
         uint2 mrow[4];
         if (V == 1) {
 #pragma unroll
-            for (int i = 0; i < 4; i++) mrow[i] = lds64(cp_meta + i * 64);
+            for (int i = 0; i < 4; i++) mrow[i] = lds64(cp_meta + i * 8 * kMetaRow);
         }
 
         // stage chunk k of every row into buffer (k & 1)
@@ -548,13 +623,33 @@ scan_staged_kernel(DevImage im, DevHot hot_img, Batch B, SegPlan P, Sink out, Se
             const uint32_t dst = cp_dst + (k & 1u) * kBufBytes;
 #pragma unroll
             for (int i = 0; i < 4 * V; i++) {
-                const uint2 m = V == 1 ? mrow[i & 3] : lds64(cp_meta + i * 64);
+                const uint2 m = V == 1 ? mrow[i & 3] : lds64(cp_meta + i * 8 * kMetaRow);
                 const bool live = k < m.y;  // else the unit is zero-filled, from the grid origin (a valid address)
                 const uint8_t *src = reinterpret_cast<const uint8_t *>(gbase) + (live ? (size_t)(m.x + k * 4 + (lane & 3)) << 4 : 0);
                 if (reinterpret_cast<uintptr_t>(src) & 64)
                     cp_async16_last(dst + i * 8 * kRow, src, live ? 16u : 0u);
                 else
                     cp_async16(dst + i * 8 * kRow, src, live ? 16u : 0u);
+            }
+            cp_async_commit();
+        };
+        // Chunk 0.  A row that starts with a warm-up fetches only the 16-byte units the scan reads (it starts at
+        // the first warm-up byte; the units before it are zero-filled), sector by sector: the rest of that
+        // 128-byte line is the end of the neighbouring segment, which another lane copies at another time, so
+        // asking the L2 for the whole line (and dropping it first) would read it from DRAM twice.
+        auto issue_first = [&]() {
+#pragma unroll
+            for (int i = 0; i < 4 * V; i++) {
+                const uint2 m = lds64(cp_meta + i * 8 * kMetaRow);
+                const uint32_t first = lds32v(cp_meta + i * 8 * kMetaRow + 12);
+                const bool live = m.y != 0;
+                const uint8_t *src = reinterpret_cast<const uint8_t *>(gbase) + (live ? (size_t)(m.x + (lane & 3)) << 4 : 0);
+                if (first & kWarmFetch)
+                    cp_async16_sector(cp_dst + i * 8 * kRow, src, live && (lane & 3) >= (first & 3u) ? 16u : 0u);
+                else if (reinterpret_cast<uintptr_t>(src) & 64)
+                    cp_async16_last(cp_dst + i * 8 * kRow, src, live ? 16u : 0u);
+                else
+                    cp_async16(cp_dst + i * 8 * kRow, src, live ? 16u : 0u);
             }
             cp_async_commit();
         };
@@ -567,7 +662,7 @@ scan_staged_kernel(DevImage im, DevHot hot_img, Batch B, SegPlan P, Sink out, Se
             LaneSeg &L = L_ptr[t];
             // this segment's fast-path state, by value (the arrays stay compile-time indexed)
             uint32_t S = s[0], POS = pos[0], STOP = stop[0], CPD = cpd[0], HI = hi_rel[0], HEAD = stop_head[0];
-            bool DONE = done[0], WARM = warm[0];
+            bool DONE = done[0], WARM = warm[0], COLD = cold[0];
 #pragma unroll
             for (int u = 1; u < V; u++)
                 if (t == (uint32_t)u) {
@@ -579,9 +674,17 @@ scan_staged_kernel(DevImage im, DevHot hot_img, Batch B, SegPlan P, Sink out, Se
                     HEAD = stop_head[u];
                     DONE = done[u];
                     WARM = warm[u];
+                    COLD = cold[u];
                 }
+            const uint32_t spec_s = meta_s + (t * 32u + lane) * kMetaRow + 8;  // the guessed start state, until the record is built
             // hand the lane over to the exact scanner at position POS, come back at the next fast-resume point
             auto leave_fast = [&](uint32_t min_at) {
+                if (!COLD) {
+                    // the first time for this segment: build its record, as the fast path has left it
+                    const SegSetup u = seg_setup<V>(P, B, bounds[0], bounds[1], gbase, lds32v(task_s), t * 32u + lane);
+                    build_cold<CP>(c, L, u, P, B, WARM, lds32v(spec_s));
+                    COLD = true;
+                }
                 c.state = state_of(S);
                 c.at = POS;
                 if (CP) {
@@ -606,11 +709,15 @@ scan_staged_kernel(DevImage im, DevHot hot_img, Batch B, SegPlan P, Sink out, Se
             auto piece_end_fast = [&]() -> bool {
                 if (WARM) {
                     // arrived at the segment start in state S: that is the guess; scan the head piece from it
-                    L.spec_state = state_of(S);
-                    L.kind = kPieceHead;
                     STOP = HEAD;
-                    c.stop = STOP;
-                    c.emit_from = 0;
+                    if (COLD) {
+                        L.spec_state = state_of(S);
+                        L.kind = kPieceHead;
+                        c.stop = STOP;
+                        c.emit_from = 0;
+                    } else {
+                        sts32(spec_s, state_of(S));
+                    }
                     CPD = 0;
                     WARM = false;
                     return true;
@@ -618,10 +725,16 @@ scan_staged_kernel(DevImage im, DevHot hot_img, Batch B, SegPlan P, Sink out, Se
                 if (STOP == HI) {
                     // end of the segment: write the summary (everything it needs from local memory is read
                     // first, in one batch: the stores below would otherwise force re-reads)
-                    const int64_t seg = L.seg;
-                    const uint32_t nem = c.nemit, spec = L.spec_state, kind = L.kind, hc = L.head_count, far = L.far;
-                    write_summary(seg_out, seg, spec, state_of(S), 0u, kind == kPieceHead ? nem : hc, nem, CP ? CPD : 0u, CP && far);
-                    L.done = 1;
+                    if (COLD) {
+                        const int64_t seg = L.seg;
+                        const uint32_t nem = c.nemit, spec = L.spec_state, kind = L.kind, hc = L.head_count, far = L.far;
+                        write_summary(seg_out, seg, spec, state_of(S), 0u, kind == kPieceHead ? nem : hc, nem, CP ? CPD : 0u, CP && far);
+                        L.done = 1;
+                    } else {
+                        // nothing was reported: the guess, the end state and the continuation bytes are all there is
+                        write_summary(seg_out, seg_of_lane<V>(P, lds32v(task_s), t * 32u + lane), lds32v(spec_s), state_of(S), 0u, 0u, 0u,
+                                      CP ? CPD : 0u, false);
+                    }
                     DONE = true;
                     return true;
                 }
@@ -681,6 +794,7 @@ scan_staged_kernel(DevImage im, DevHot hot_img, Batch B, SegPlan P, Sink out, Se
                     cpd[u] = CPD;
                     done[u] = DONE;
                     warm[u] = WARM;
+                    cold[u] = COLD;
                 }
         };
 
@@ -688,7 +802,7 @@ scan_staged_kernel(DevImage im, DevHot hot_img, Batch B, SegPlan P, Sink out, Se
         // through the table with one trap check -- the V dependent chains are independent of each other and
         // interleave, hiding each other's shared-memory latency; whatever is not clean goes the careful way.
         if (kmax)
-            issue(0);
+            issue_first();
         else if (lane == 0)
             claimed = atomicAdd(task_counter, 1u);  // nothing to scan in this task (segments outside the stream)
         for (uint32_t k = 0; k <= kmax; k++) {
@@ -709,13 +823,17 @@ scan_staged_kernel(DevImage im, DevHot hot_img, Batch B, SegPlan P, Sink out, Se
                     if (!done[t] && warm[t] && pos[t] == stop[t] && pos[t] == relk) {
                         // the warm-up ended right at this chunk, in state s: that is the guess for the segment start;
                         // the head piece is scanned from it (same as piece_end_fast in the careful path)
-                        PieceCtx &c = c_ptr[t];
-                        LaneSeg &L = L_ptr[t];
-                        L.spec_state = state_of(s[t]);
-                        L.kind = kPieceHead;
                         stop[t] = stop_head[t];
-                        c.stop = stop[t];
-                        c.emit_from = 0;
+                        if (cold[t]) {
+                            PieceCtx &c = c_ptr[t];
+                            LaneSeg &L = L_ptr[t];
+                            L.spec_state = state_of(s[t]);
+                            L.kind = kPieceHead;
+                            c.stop = stop[t];
+                            c.emit_from = 0;
+                        } else {
+                            sts32(meta_s + ((uint32_t)t * 32u + lane) * kMetaRow + 8, state_of(s[t]));
+                        }
                         cpd[t] = 0;
                         warm[t] = false;
                     }

@@ -5,13 +5,18 @@
 // chunk in place of the table walk.  One CTA per SM, 400 k rows = 409.6 MB, tasks from an atomic counter.  Prints
 // the time against the spin alone, and the share of warp time spent in cp.async.wait_group.
 //
-// The full model (MODEL = true) also does what the kernel does besides copying and scanning:
-//  - 3 of every 4 segments (those that do not start a 4 KiB haystack) begin with a warm-up chunk, the 64 bytes
-//    before the segment: 17 chunks instead of 16;
-//  - each lane writes a 112-byte record to local memory at task start and reads it back at the segment end (the
-//    kernel's exact-scanner state and segment bookkeeping), and writes a 32-byte segment summary;
-//  - the next task is claimed when the last chunk starts.
-// Levers on top of it: a bulk L2 prefetch (cp.async.bulk.prefetch.L2) of each lane's own next PFC chunks, PFD
+// The model (struct Model) also does what the kernel does besides copying and scanning, each part on its own switch:
+//  - warm: 3 of every 4 segments (those that do not start a 4 KiB haystack) begin with a warm-up chunk, the 64 bytes
+//    before the segment: 17 chunks instead of 16.  1: all four units, with the policy of any other chunk (the line
+//    before the segment is fetched whole and, with evict_first, dropped first); 2: only the last 16 bytes, with a
+//    plain cp.async.cg (one 32-byte sector);
+//  - rec: each lane writes a record of `rec` words to local memory at task start and reads it back at the segment
+//    end (28: the kernel's exact-scanner state and segment bookkeeping when every lane stores them; 6: the words
+//    the segment end reads; 0: none, they are built only by lanes that need the exact scanner);
+//  - summ: a 32-byte segment summary, 1: at the segment's own index (a warp's stores lie lane_stride * 32 B
+//    apart), 2: at task * 32 + lane (a warp's stores are contiguous);
+//  - claim: the next task is claimed when the last chunk starts.
+// Levers on top of the full model (warm 1, rec 28, summ 1, claim): a bulk L2 prefetch (cp.async.bulk.prefetch.L2) of each lane's own next PFC chunks, PFD
 // chunks ahead; the next task's first bytes prefetched during the current task's last chunk (claimed one chunk
 // earlier); an evict_first L2 policy on the copies of chunks that complete their 128-byte line; 16 / 24 / 32 warps.
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 stage_copy.cu
@@ -37,16 +42,22 @@ template <int N> __device__ __forceinline__ void cp_wait() { asm volatile("cp.as
 
 constexpr uint32_t kQ = 4, kSeg = 1024, kBuf = 32 * 64, kRec = 28;  // kRec: u32 words of the per-lane local record
 
+struct Model {
+    int warm, rec, summ;
+    bool claim;
+};
+constexpr Model kNone = {0, 0, 0, false}, kFull = {1, (int)kRec, 1, true};
+
 struct Lever {
-    bool model;     // warm-up chunks, local record, summaries, claim during the last chunk
+    Model model;
     int pfc, pfd;   // bulk L2 prefetch of the lane's next pfc chunks, pfd chunks ahead (pfc 0: none)
     bool next;      // the next task's first pfc (at least 4) chunks, during the last chunk
     bool evf;       // evict_first on copies that complete a 128-byte line
     int warps;
 };
 
-template <int STAGES, int PF, bool MODEL, bool EVF>
-__global__ void __launch_bounds__(1024, 1) stage(const uint8_t *data, uint32_t n_rows, uint32_t spin, int pfc, int pfd, bool next_pf,
+template <int STAGES, int PF, bool EVF>
+__global__ void __launch_bounds__(1024, 1) stage(const uint8_t *data, uint32_t n_rows, uint32_t spin, Model md, int pfc, int pfd, bool next_pf,
                                                  unsigned int *counter, unsigned long long *stats, uint32_t *sink, uint4 *summaries) {
     extern __shared__ __align__(128) uint8_t smem[];
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -61,21 +72,20 @@ __global__ void __launch_bounds__(1024, 1) stage(const uint8_t *data, uint32_t n
     asm volatile("" : "+l"(rp));
     const long long t_start = clock64();
     unsigned int claimed = 0;
-    if (MODEL && lane == 0) claimed = atomicAdd(counter, 1u);
+    if (md.claim && lane == 0) claimed = atomicAdd(counter, 1u);
     for (;;) {
-        if (!MODEL && lane == 0) claimed = atomicAdd(counter, 1u);
+        if (!md.claim && lane == 0) claimed = atomicAdd(counter, 1u);
         const unsigned int task = __shfl_sync(0xffffffffu, claimed, 0);
         if (task >= n_tasks) break;
         // row r of the task: segment (task / q * 32 + r) * q + task % q; a segment inside its haystack starts
         // with a warm-up chunk (all rows of a task alike)
         const uint64_t seg0 = (uint64_t)(task / kQ) * 32 * kQ + task % kQ;
-        const bool warm = MODEL && task % kQ != 0;
+        const bool warm = md.warm && task % kQ != 0;
         const uint32_t kmax = kSeg / 64 + (warm ? 1 : 0);
         const int64_t first = warm ? -64 : 0;  // of the row's first chunk, relative to its segment
-        if (MODEL) {
 #pragma unroll
-            for (int i = 0; i < (int)kRec; i++) rp[i] = (uint32_t)(seg0 + lane) * (i + 1);
-        }
+        for (int i = 0; i < (int)kRec; i++)
+            if (i < md.rec) rp[i] = (uint32_t)(seg0 + lane) * (i + 1);
         const uint8_t *mine = data + (int64_t)((seg0 + (uint64_t)lane * kQ) * kSeg) + first;
         auto issue = [&](uint32_t k) {
             if (k < kmax) {
@@ -85,7 +95,9 @@ __global__ void __launch_bounds__(1024, 1) stage(const uint8_t *data, uint32_t n
                     const uint32_t r = i * 8 + (lane >> 2);
                     const uint8_t *src = data + (int64_t)((seg0 + (uint64_t)r * kQ) * kSeg) + first + k * 64 + (lane & 3) * 16;
                     const uint32_t dst = buf + r * 64 + (((lane & 3) ^ ((r >> 1) & 3)) << 4);
-                    if (EVF && (reinterpret_cast<uintptr_t>(src) & 64))
+                    if (warm && k == 0 && md.warm == 2) {
+                        if ((lane & 3) == 3) cp_async16<0>(dst, src);  // the unit the scan reads; the others are never looked at
+                    } else if (EVF && (reinterpret_cast<uintptr_t>(src) & 64))
                         cp_async16<PF, true>(dst, src, pol);  // the second half of its 128-byte line: the line is spent
                     else
                         cp_async16<PF>(dst, src);
@@ -101,7 +113,7 @@ __global__ void __launch_bounds__(1024, 1) stage(const uint8_t *data, uint32_t n
             __syncwarp();
             waited += (unsigned long long)(clock64() - w0);
             issue(k + STAGES - 1);
-            if (MODEL && k == k_claim && lane == 0) claimed = atomicAdd(counter, 1u);
+            if (md.claim && k == k_claim && lane == 0) claimed = atomicAdd(counter, 1u);
             if (pfc && k % pfc == 0 && k + pfd < kmax) {
                 const uint32_t n = min((uint32_t)pfc, kmax - (k + pfd));
                 prefetch_l2(mine + (k + pfd) * 64, n * 64);
@@ -120,13 +132,17 @@ __global__ void __launch_bounds__(1024, 1) stage(const uint8_t *data, uint32_t n
             const long long t0 = clock64();  // stand-in for the scan of the chunk
             while (clock64() - t0 < spin) {}
         }
-        if (MODEL) {
-            // the segment end: the record read back, the summary written
-            uint32_t x = 0;
+        // the segment end: the record read back, the summary written
+        uint32_t x = 0;
 #pragma unroll
-            for (int i = 0; i < (int)kRec; i++) x += rp[i];
-            summaries[2 * (seg0 + (uint64_t)lane * kQ)] = make_uint4(x, acc, 0, 0);
-            summaries[2 * (seg0 + (uint64_t)lane * kQ) + 1] = make_uint4(0, 0, x, 1);
+        for (int i = 0; i < (int)kRec; i++)
+            if (i < md.rec) x += rp[i];
+        if (md.summ) {
+            const uint64_t slot = md.summ == 2 ? (uint64_t)task * 32 + lane : seg0 + (uint64_t)lane * kQ;
+            summaries[2 * slot] = make_uint4(x, acc, 0, 0);
+            summaries[2 * slot + 1] = make_uint4(0, 0, x, 1);
+        } else {
+            acc += x;
         }
         cp_wait<0>();
     }
@@ -137,19 +153,19 @@ __global__ void __launch_bounds__(1024, 1) stage(const uint8_t *data, uint32_t n
     if (acc == 0x12345678u) sink[0] = acc;
 }
 
-template <int STAGES, int PF, bool MODEL, bool EVF>
+template <int STAGES, int PF, bool EVF>
 void run(const char *name, const uint8_t *d, uint32_t rows, uint32_t spin, double clock_ghz, int sms, Lever lv, uint4 *summ) {
     unsigned int *ctr; unsigned long long *st; uint32_t *sink;
     cudaMalloc(&ctr, 4); cudaMalloc(&st, 16); cudaMalloc(&sink, 4);
     const size_t smem = (size_t)lv.warps * STAGES * kBuf;
-    cudaFuncSetAttribute(stage<STAGES, PF, MODEL, EVF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(stage<STAGES, PF, EVF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     float best = 1e9, sum = 0; unsigned long long h[2] = {0, 0};
     const int iters = 20;
     for (int it = 0; it < iters + 2; it++) {
         cudaMemset(ctr, 0, 4); cudaMemset(st, 0, 16);
         cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
         cudaEventRecord(e0);
-        stage<STAGES, PF, MODEL, EVF><<<sms, lv.warps * 32, smem>>>(d, rows, spin, lv.pfc, lv.pfd, lv.next, ctr, st, sink, summ);
+        stage<STAGES, PF, EVF><<<sms, lv.warps * 32, smem>>>(d, rows, spin, lv.model, lv.pfc, lv.pfd, lv.next, ctr, st, sink, summ);
         cudaEventRecord(e1); cudaEventSynchronize(e1);
         float ms; cudaEventElapsedTime(&ms, e0, e1);
         if (it >= 2) sum += ms;
@@ -157,7 +173,7 @@ void run(const char *name, const uint8_t *d, uint32_t rows, uint32_t spin, doubl
         cudaEventDestroy(e0); cudaEventDestroy(e1);
     }
     // the spin alone: chunks per warp (tasks spread evenly) x spin
-    const double chunks = MODEL ? 16.75 : 16.0;
+    const double chunks = lv.model.warm ? 16.75 : 16.0;
     const double spin_ms = (double)rows / 32 / (sms * lv.warps) * chunks * spin / clock_ghz / 1e6;
     printf("%-34s spin %5u cyc: best %.4f ms, mean %.4f (spin alone %.4f), %6.1f GB/s, wait %.1f %% of warp time  (%s)\n", name, spin,
            best, sum / iters, spin_ms, (double)rows * kSeg / best / 1e6, 100.0 * h[0] / (double)h[1], cudaGetErrorString(cudaGetLastError()));
@@ -178,24 +194,32 @@ int main() {
     // 2.8 us is the spin of the earlier rows
     for (double us : {2.4, 2.8}) {
         const uint32_t spin = (uint32_t)(us * 1e3 * ghz);
-        run<2, 1, false, false>("copies only, L2::128B", d, rows, spin, ghz, sms, {false, 0, 0, false, false, 32}, summ);
-        run<2, 1, true, false>("model, L2::128B", d, rows, spin, ghz, sms, {true, 0, 0, false, false, 32}, summ);
+        run<2, 1, false>("copies only, L2::128B", d, rows, spin, ghz, sms, {kNone, 0, 0, false, false, 32}, summ);
+        run<2, 1, false>("model, L2::128B", d, rows, spin, ghz, sms, {kFull, 0, 0, false, false, 32}, summ);
         char name[64];
         for (int pfc : {2, 4, 8})
             for (int pfd : {1, 2, 4, 8}) {
                 if (pfd < pfc / 2) continue;
                 snprintf(name, sizeof name, "(a) R=%d D=%d", pfc * 64, pfd);
-                run<2, 1, true, false>(name, d, rows, spin, ghz, sms, {true, pfc, pfd, false, false, 32}, summ);
+                run<2, 1, false>(name, d, rows, spin, ghz, sms, {kFull, pfc, pfd, false, false, 32}, summ);
             }
-        run<2, 1, true, false>("(b) next task, 256 B", d, rows, spin, ghz, sms, {true, 0, 0, true, false, 32}, summ);
-        run<2, 1, true, false>("(a)+(b) R=256 D=4", d, rows, spin, ghz, sms, {true, 4, 4, true, false, 32}, summ);
-        run<2, 1, true, true>("(c) evict_first", d, rows, spin, ghz, sms, {true, 0, 0, false, true, 32}, summ);
-        run<2, 1, true, true>("(a)+(b)+(c) R=256 D=4", d, rows, spin, ghz, sms, {true, 4, 4, true, true, 32}, summ);
+        run<2, 1, false>("(b) next task, 256 B", d, rows, spin, ghz, sms, {kFull, 0, 0, true, false, 32}, summ);
+        run<2, 1, false>("(a)+(b) R=256 D=4", d, rows, spin, ghz, sms, {kFull, 4, 4, true, false, 32}, summ);
+        run<2, 1, true>("(c) evict_first", d, rows, spin, ghz, sms, {kFull, 0, 0, false, true, 32}, summ);
+        run<2, 1, true>("(a)+(b)+(c) R=256 D=4", d, rows, spin, ghz, sms, {kFull, 4, 4, true, true, 32}, summ);
         for (int w : {16, 24}) {
             snprintf(name, sizeof name, "(d) %d warps", w);
-            run<2, 1, true, false>(name, d, rows, spin, ghz, sms, {true, 0, 0, false, false, w}, summ);
+            run<2, 1, false>(name, d, rows, spin, ghz, sms, {kFull, 0, 0, false, false, w}, summ);
             snprintf(name, sizeof name, "(d) %d warps + (a)+(b) R=512 D=8", w);
-            run<2, 1, true, false>(name, d, rows, spin, ghz, sms, {true, 8, 8, true, false, w}, summ);
+            run<2, 1, false>(name, d, rows, spin, ghz, sms, {kFull, 8, 8, true, false, w}, summ);
+        }
+        // the parts of the model one at a time, on top of (c), which is what the kernel does: the full model first and
+        // last (the spread between the two is the noise of this table)
+        const Model parts[] = {kFull,          {2, 28, 1, true}, {0, 28, 1, true}, {1, 6, 1, true}, {1, 0, 1, true}, {1, 28, 2, true},
+                               {1, 28, 0, true}, {1, 28, 1, false}, {2, 0, 1, true}, {2, 0, 2, true}, {0, 0, 0, true}, kFull};
+        for (const Model &m : parts) {
+            snprintf(name, sizeof name, "(c) warm %d rec %2d summ %d claim %d", m.warm, m.rec, m.summ, (int)m.claim);
+            run<2, 1, true>(name, d, rows, spin, ghz, sms, {m, 0, 0, false, true, 32}, summ);
         }
     }
     cudaFree(base); cudaFree(summ);
