@@ -209,24 +209,34 @@ def test_profiled_hot_set_keeps_results_and_cuts_traps():
 
 
 def test_byte_indexed_table_agrees_with_compact_table():
+    """For every pattern set with a byte-indexed table -- class columns, range columns ending at 0x7e, range columns
+    from 0x00 -- its rows equal the compact table's, byte by byte, and column 127 (where the scan folds every byte
+    >= 0x80) equals the compact table's column of each such byte."""
     import struct
     from ahocorasick_rs_b200 import _capi
-    pats = [b"hello", b"help", b"world", b"wor", b"~x"]
-    for kind in range(3):
-        im = ii.Image(pats, kind)
-        L = im._L
-        n = L.acb_hot_bytes(im._h, 40)
-        buf = np.zeros(n, dtype=np.uint8)
-        assert L.acb_hot_build(im._h, None, 40, buf.ctypes.data, n) == 0
-        desc = _capi.HotDesc()
-        assert L.acb_hot_describe(buf.ctypes.data, __import__("ctypes").byref(desc)) == 0
-        assert desc.rows == min(40, im.n_states - 1) and desc.rows128 == desc.rows and desc.visited == 1
-        magic, rows, n_cols, n_states, o_t, o_h2f, o_f2h, total, rows128, visited, o_t128 = struct.unpack_from("<4I4Q2IQ", buf.tobytes()[:64])
-        t = buf[o_t:o_t + 2 * (rows + 1) * n_cols].view(np.uint16).reshape(rows + 1, n_cols) // (2 * n_cols)
-        t128 = buf[o_t128:o_t128 + 2 * (rows128 + 1) * 128].view(np.uint16).reshape(rows128 + 1, 128) // 256
-        for h in range(rows128 + 1):
-            for b in range(128):
-                assert t128[h, b] == t[h, im.col(b)]
+    from tests.table_shapes import BYTE_TABLE
+    sets = [[b"hello", b"help", b"world", b"wor", b"~x"]] + [c.pats for c in BYTE_TABLE]
+    seen = set()
+    for pats in sets:
+        for kind in range(3):
+            im = ii.Image(pats, kind)
+            seen.add((im.col_mode, max(b for p in pats for b in p) == 0x7E, im.col_lo == 0))
+            L = im._L
+            n = L.acb_hot_bytes(im._h, 40)
+            buf = np.zeros(n, dtype=np.uint8)
+            assert L.acb_hot_build(im._h, None, 40, buf.ctypes.data, n) == 0
+            desc = _capi.HotDesc()
+            assert L.acb_hot_describe(buf.ctypes.data, __import__("ctypes").byref(desc)) == 0
+            assert desc.rows == min(40, im.n_states - 1) and desc.rows128 == desc.rows and desc.visited == 1
+            magic, rows, n_cols, n_states, o_t, o_h2f, o_f2h, total, rows128, visited, o_t128 = struct.unpack_from("<4I4Q2IQ", buf.tobytes()[:64])
+            t = buf[o_t:o_t + 2 * (rows + 1) * n_cols].view(np.uint16).reshape(rows + 1, n_cols) // (2 * n_cols)
+            t128 = buf[o_t128:o_t128 + 2 * (rows128 + 1) * 128].view(np.uint16).reshape(rows128 + 1, 128) // 256
+            for h in range(rows128 + 1):
+                for b in range(128):
+                    assert t128[h, b] == t[h, im.col(b)]
+                for b in range(128, 256):
+                    assert t128[h, 127] == t[h, im.col(b)]
+    assert {(1, True, False), (0, True, False), (0, False, True)} <= seen
     # a pattern byte >= 0x7f rules the byte-indexed table out
     im = ii.Image([b"caf\xc3\xa9"], 0)
     n = im._L.acb_hot_bytes(im._h, 40)
