@@ -113,6 +113,11 @@ def lib():
                                        C.c_void_p, C.c_void_p]
         L.acb_stream_resolve.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64, C.c_void_p, C.c_int,
                                          C.c_int] + [C.c_void_p] * 12
+        L.acb_stream_advance.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64, C.c_void_p, C.c_int] + [C.c_void_p] * 6
+        L.acb_stream_first_resolve.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64, C.c_void_p, C.c_int,
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64] + [C.c_void_p] * 6
+        L.acb_stream_count.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64, C.c_void_p, C.c_int] + [C.c_void_p] * 10 + [
+            C.c_uint64, C.c_void_p]
         L.acb_pack_gather_block.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p, C.c_void_p]
         L.acb_scan_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(HotDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                      C.c_uint64, C.c_int, C.c_int, C.POINTER(Plan), C.POINTER(Workspace), C.c_void_p]
@@ -150,5 +155,5 @@ EXPORTS = [
     "acb_any_match", "acb_find_first", "acb_first_rows", "acb_rows_to_codepoints",
     "acb_count_overlapping", "acb_count_non_overlapping", "acb_count_rows", "acb_stream_seams", "acb_stream_resolve",
     "acb_pattern_counts_overlapping", "acb_pattern_counts_non_overlapping", "acb_pattern_hits",
-    "acb_pattern_hit_row_words",
+    "acb_pattern_hit_row_words", "acb_stream_advance", "acb_stream_first_resolve", "acb_stream_count",
 ]

@@ -1709,6 +1709,306 @@ __global__ void stream_emit_kernel(StreamArgs A) {
     }
 }
 
+// ---------------------------------------------------------------------------
+// Stream queries (acb_stream_advance, acb_stream_first_resolve, acb_stream_count): is_match, find_first and
+// count_matches per stream, without the rows.  They use the seams and the carry of the stream search; the advance is
+// the carry half of stream_emit_kernel, for feeds that make no selection (or count it without rows).
+// ---------------------------------------------------------------------------
+
+// code points: cont_rows[i] = (0, x, x), x = chunk bytes before the new tail, as stream_select_kernel writes it
+__global__ void stream_cont_rows_kernel(StreamArgs A) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < A.B.n_haystacks; i += (int64_t)gridDim.x * blockDim.x) {
+        const long long len = A.B.offsets[i + 1] - A.B.offsets[i];
+        const long long x = max(len - min(A.carry[kCarryWords * i + kCarryFed] + len, (long long)A.halo), 0ll);
+        A.cont_rows[3 * i] = 0, A.cont_rows[3 * i + 1] = x, A.cont_rows[3 * i + 2] = x;
+    }
+}
+
+// One warp per stream: the new tail, the data fed, and (code points) the continuation bytes before the new tail; the
+// whole carry is zeroed for a stream that ends with this feed.
+__global__ void stream_advance_kernel(StreamArgs A) {
+    const uint32_t lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < A.B.n_haystacks; i += warps) {
+        int64_t *c = A.carry + kCarryWords * i;
+        const long long fed = c[kCarryFed], t = c[kCarryTail], cont = c[kCarryCont];
+        const long long len = A.B.offsets[i + 1] - A.B.offsets[i];
+        const uint8_t *seam = A.seam + A.seam_offsets[i], *chunk = A.B.bytes + A.B.offsets[i];
+        const bool last = A.last && A.last[i];
+        const long long fed_after = fed + len, t_after = last ? 0 : min(fed_after, (long long)A.halo);
+        const long long from = t + len - t_after;  // the new tail: bytes [from, t + len) of tail || chunk
+        uint8_t *tail = A.tail + (uint64_t)i * A.halo;
+        for (long long k = lane; k < t_after; k += 32) tail[k] = k + from < t ? seam[k + from] : chunk[k + from - t];
+        long long cont_after = 0;
+        if (A.codepoints && !last) {
+            unsigned long long m = 0;  // continuation bytes of the old tail before `from`
+            for (long long k = lane; k < min(from, t); k += 32) m += is_cont_byte(seam[k]);
+            for (int d = 16; d >= 1; d >>= 1) m += __shfl_xor_sync(0xffffffffu, m, d);
+            cont_after = cont + (long long)m + (A.cont_rows[3 * i + 1] - A.cont_cp[3 * i + 1]);
+        }
+        __syncwarp();
+        if (lane == 0) {
+            c[kCarryFed] = last ? 0 : fed_after;
+            c[kCarryTail] = t_after;
+            c[kCarryCont] = cont_after;
+            if (last) c[kCarryRestart] = 0;
+        }
+    }
+}
+
+// find_first: the best candidate a stream carries, int64[n][kBestWords]: state, then (pattern, start, end) in bytes
+// (absolute) and start, end in code points (a copy of the bytes' without code points)
+enum : int { kBestState = 0, kBestPid = 1, kBestStart = 2, kBestEnd = 3, kBestCpStart = 4, kBestCpEnd = 5, kBestWords = 6 };
+enum : int { kFirstNone = 0, kFirstPending = 1, kFirstFinal = 2 };
+
+struct FirstArgs {
+    Batch B;                          // the chunks
+    const int64_t *carry;             // before this feed's advance
+    const uint8_t *last;
+    const uint8_t *seam;
+    const int64_t *seam_offsets;
+    unsigned long long *seam_keys, *chunk_keys;  // [n] each
+    const long long *seam_rows, *chunk_rows;     // [n][3] decoded, bytes relative to the seam / the chunk
+    const long long *seam_cp, *chunk_cp;         // [n][3] the same in code points (codepoints only)
+    long long *best;                  // [n][kBestWords]
+    long long *rows;                  // [n][3] the answers after this feed
+    unsigned long long *stats;        // [1] streams with a pending candidate
+    uint32_t max_len;
+    int kind, codepoints;
+};
+
+// the streams whose keys were pre-set to 0 (their scans were skipped): the keys go back to ~0, so the rows decode none
+__global__ void stream_first_unmask_kernel(FirstArgs A) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < A.B.n_haystacks; i += (int64_t)gridDim.x * blockDim.x) {
+        const long long state = A.best[kBestWords * i + kBestState];
+        if (state == kFirstFinal) A.seam_keys[i] = ~0ull;
+        if (state == kFirstFinal || (state == kFirstPending && A.kind != ACB_STANDARD)) A.chunk_keys[i] = ~0ull;
+    }
+}
+
+// a better than b in the order of the kind's first match (the key order of acb_find_first, on absolute positions)
+__device__ __forceinline__ bool first_better(const long long *a, const long long *b, int kind) {
+    if (kind == ACB_STANDARD) {
+        if (a[2] != b[2]) return a[2] < b[2];  // earliest end,
+        if (a[1] != b[1]) return a[1] < b[1];  // then the longest,
+        return a[0] < b[0];                    // then the lowest pattern
+    }
+    if (a[1] != b[1]) return a[1] < b[1];  // leftmost start
+    if (kind == ACB_LEFTMOST_LONGEST && a[2] != b[2]) return a[2] > b[2];
+    return a[0] < b[0];
+}
+
+// One thread per stream: the carried best, the seam's candidate and the chunk's, in absolute positions; the best of
+// them is final once no later data can change it (Standard: at once; leftmost: start + max_pattern_len <= F; every
+// candidate on `last`).  Writes the answer row, the state, and the keys of the next feed: 0 where that scan can be
+// skipped (a final answer: both; a pending leftmost candidate: the chunk's, whose records all start after it).
+__global__ void stream_first_resolve_kernel(FirstArgs A) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < A.B.n_haystacks; i += (int64_t)gridDim.x * blockDim.x) {
+        long long *b = A.best + kBestWords * i;
+        const int64_t *c = A.carry + kCarryWords * i;
+        const long long fed = c[kCarryFed], t = c[kCarryTail], cont = c[kCarryCont];
+        const long long fed_after = fed + (A.B.offsets[i + 1] - A.B.offsets[i]);
+        const bool last = A.last && A.last[i];
+        long long state = b[kBestState];
+        long long cur[5] = {b[kBestPid], b[kBestStart], b[kBestEnd], b[kBestCpStart], b[kBestCpEnd]};
+        if (state != kFirstFinal) {
+            bool have = state == kFirstPending;
+            const long long *sr = A.seam_rows + 3 * i;
+            if (sr[0] >= 0) {
+                const long long base = fed - t, cp_base = fed - t - cont;
+                const long long m[5] = {sr[0], base + sr[1], base + sr[2], A.codepoints ? cp_base + A.seam_cp[3 * i + 1] : base + sr[1],
+                                        A.codepoints ? cp_base + A.seam_cp[3 * i + 2] : base + sr[2]};
+                if (!have || first_better(m, cur, A.kind)) {
+                    for (int k = 0; k < 5; k++) cur[k] = m[k];
+                    have = true;
+                }
+            }
+            const long long *cr = A.chunk_rows + 3 * i;
+            if (cr[0] >= 0) {
+                const long long m3[3] = {cr[0], fed + cr[1], fed + cr[2]};
+                if (!have || first_better(m3, cur, A.kind)) {
+                    long long cp_base = fed;
+                    if (A.codepoints) {  // the continuation bytes before the chunk: before the tail, and in it
+                        const uint8_t *seam = A.seam + A.seam_offsets[i];
+                        long long tc = 0;
+                        for (long long k = 0; k < t; k++) tc += is_cont_byte(seam[k]);
+                        cp_base = fed - cont - tc;
+                    }
+                    cur[0] = m3[0], cur[1] = m3[1], cur[2] = m3[2];
+                    cur[3] = A.codepoints ? cp_base + A.chunk_cp[3 * i + 1] : m3[1];
+                    cur[4] = A.codepoints ? cp_base + A.chunk_cp[3 * i + 2] : m3[2];
+                    have = true;
+                }
+            }
+            if (have)
+                state = (A.kind == ACB_STANDARD || last || cur[1] + (long long)A.max_len <= fed_after) ? kFirstFinal : kFirstPending;
+        }
+        const bool final_ = state == kFirstFinal;
+        long long *row = A.rows + 3 * i;
+        row[0] = final_ ? cur[0] : -1;
+        row[1] = final_ ? cur[3] : -1;
+        row[2] = final_ ? cur[4] : -1;
+        if (last) state = kFirstNone;
+        if (state == kFirstPending) atomicAdd(A.stats + 1, 1ull);
+        b[kBestState] = state;
+        b[kBestPid] = state ? cur[0] : 0;
+        b[kBestStart] = state ? cur[1] : 0;
+        b[kBestEnd] = state ? cur[2] : 0;
+        b[kBestCpStart] = state ? cur[3] : 0;
+        b[kBestCpEnd] = state ? cur[4] : 0;
+        A.seam_keys[i] = state == kFirstFinal ? 0ull : ~0ull;
+        A.chunk_keys[i] = (state == kFirstFinal || (state == kFirstPending && A.kind != ACB_STANDARD)) ? 0ull : ~0ull;
+    }
+}
+
+// count_matches: the running count of stream i is what the rows stream would have released so far
+struct CountArgs {
+    StreamArgs S;                          // the lists, the carry (before this feed's advance), last, halo, mode, longest
+    const unsigned long long *chunk_counts;  // overlapping: acb_count_overlapping's count of each chunk
+    long long *running;                    // [n]
+    long long *out;                        // [n] the counts after this feed
+    unsigned long long *stats;             // [0] records, [1] streams holding a pick, [2] streams selected on the grid, [3] the longest
+    long long *per;                        // [n][4] grid path: released count, new restart point, NEXT(restart), sequence length
+    long long *long_list;                  // [n] the streams selected on the grid
+    uint4 *pairs;                          // [R] successor pairs, double-buffered (jump_pair)
+    uint32_t *mark;                        // [R] records on the selected chain
+};
+
+__device__ __forceinline__ void count_finish(const CountArgs &A, int64_t i, long long add, bool last) {
+    const long long v = A.running[i] + add;
+    A.out[i] = v;
+    A.running[i] = last ? 0 : v;
+}
+
+// overlapping (Standard): a feed adds its chunk's count and the seam's records that cross the tail / head join
+// (start < T < end): the others lie in the head (counted with the chunk) or in the tail (counted by earlier feeds)
+__global__ void stream_count_overlap_kernel(CountArgs A) {
+    const StreamArgs &S = A.S;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < S.B.n_haystacks; i += (int64_t)gridDim.x * blockDim.x) {
+        const long long t = S.carry[kCarryWords * i + kCarryTail];
+        const unsigned long long s1 = S.seam_mo[i + 1];
+        long long cross = 0;
+        for (unsigned long long j = first_end_after(S.seam_list, S.seam_mo[i], s1, (uint32_t)t); j < s1; j++) cross += S.seam_list[j].z < (uint32_t)t;
+        atomicAdd(A.stats, s1 - S.seam_mo[i]);
+        count_finish(A, i, (long long)A.chunk_counts[i] + cross, S.last && S.last[i]);
+    }
+}
+
+// Non-overlapping, every kind: the selection continued from the carried restart point, counted up to the first pick the
+// release rule does not allow yet.  A sequence of at most ACB_LONG_STRETCH records is counted by one thread
+// (next_selected, as stream_select_kernel).  A longer one is selected by the whole grid: every record gets the successor
+// NEXT(end), the chain from NEXT(restart) is marked by pointer jumping (select_stretches' rule), and the released count
+// is the number of marked records with start + max_pattern_len <= F (all of them on `last`); the new restart point is
+// the end of the last released one.  Cooperative launch.
+template <int MODE>
+__global__ void __launch_bounds__(kScanThreads) stream_count_kernel(CountArgs A) {
+    namespace cg = cooperative_groups;
+    cg::grid_group grid = cg::this_grid();
+    const StreamArgs &S = A.S;
+    const long long max_len = (long long)S.halo + 1;
+    const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+    const unsigned long long first_i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    for (int64_t i = (int64_t)first_i; i < S.B.n_haystacks; i += (int64_t)stride) {
+        int64_t *c = S.carry + kCarryWords * i;
+        const long long fed_after = c[kCarryFed] + (S.B.offsets[i + 1] - S.B.offsets[i]);
+        const bool last = S.last && S.last[i];
+        StreamView v;
+        const unsigned long long n = stream_view(S, i, v);
+        atomicAdd(A.stats, n);
+        long long s = c[kCarryRestart];
+        if (n > ACB_LONG_STRETCH) {
+            long long *p = A.per + 4 * i;
+            p[0] = 0, p[1] = s, p[2] = (long long)next_selected<MODE>(&v, n, s, max_len, S.longest), p[3] = (long long)n;
+            A.long_list[atomicAdd(A.stats + 2, 1ull)] = i;
+            atomicMax(A.stats + 3, n);
+            continue;
+        }
+        long long k = 0;
+        bool pending = false;
+        for (;;) {
+            const unsigned long long j = next_selected<MODE>(&v, n, s, max_len, S.longest);
+            if (j >= n) break;
+            const SelRec m = sel_rec(&v, j);
+            if (MODE == kModeLeftmost && !last && m.start + max_len > fed_after) {
+                pending = true;
+                break;
+            }
+            k++;
+            s = m.end;
+        }
+        c[kCarryRestart] = s;
+        if (pending) atomicAdd(A.stats + 1, 1ull);
+        count_finish(A, i, k, last);
+    }
+    grid.sync();
+    const unsigned long long n_long = A.stats[2];
+    if (n_long == 0) return;
+    // the streams on the grid, one after another; record j of stream i sits at index seam_mo[i] + chunk_mo[i] + j
+    for (unsigned long long q = 0; q < n_long; q++) {
+        const int64_t i = A.long_list[q];
+        StreamView v;
+        const unsigned long long n = stream_view(S, i, v), base = S.seam_mo[i] + S.chunk_mo[i], head = (unsigned long long)A.per[4 * i + 2];
+        for (unsigned long long j = first_i; j < n; j += stride) {
+            const unsigned long long nx = next_selected<MODE>(&v, n, sel_rec(&v, j).end, max_len, S.longest);
+            reinterpret_cast<uint2 *>(A.pairs + base + j)[0] = make_uint2(nx >= n ? kNoNext : (uint32_t)(base + nx), 1u);
+            A.mark[base + j] = j == head ? 1u : 0u;
+        }
+    }
+    grid.sync();
+    const uint32_t rounds = ceil_log2(A.stats[3]);
+    for (uint32_t r = 0; r < rounds; r++) {
+        const int src = (int)(r & 1);
+        for (unsigned long long q = 0; q < n_long; q++) {
+            const int64_t i = A.long_list[q];
+            const unsigned long long n = (unsigned long long)A.per[4 * i + 3], base = S.seam_mo[i] + S.chunk_mo[i];
+            for (unsigned long long j = first_i; j < n; j += stride) {
+                const uint32_t nx = src ? A.pairs[base + j].z : A.pairs[base + j].x;  // J_r(base + j)
+                if (nx != kNoNext && A.mark[base + j]) A.mark[nx] = 1u;
+                jump_pair(A.pairs, base + j, src);
+            }
+        }
+        grid.sync();
+    }
+    for (unsigned long long q = 0; q < n_long; q++) {
+        const int64_t i = A.long_list[q];
+        StreamView v;
+        const unsigned long long n = stream_view(S, i, v), base = S.seam_mo[i] + S.chunk_mo[i];
+        const long long fed_after = S.carry[kCarryWords * i + kCarryFed] + (S.B.offsets[i + 1] - S.B.offsets[i]);
+        const bool last = S.last && S.last[i];
+        unsigned long long released = 0, held = 0;
+        long long end = 0;  // (every end is positive)
+        for (unsigned long long j = first_i; j < n; j += stride) {
+            if (!A.mark[base + j]) continue;
+            const SelRec m = sel_rec(&v, j);
+            if (MODE == kModeStandard || last || m.start + max_len <= fed_after) {
+                released++;
+                end = max(end, m.end);
+            } else {
+                held++;
+            }
+        }
+#pragma unroll
+        for (int d = 16; d >= 1; d >>= 1) {
+            released += __shfl_xor_sync(0xffffffffu, released, d);
+            held += __shfl_xor_sync(0xffffffffu, held, d);
+            end = max(end, (long long)__shfl_xor_sync(0xffffffffu, end, d));
+        }
+        if ((threadIdx.x & 31) == 0) {
+            if (released) atomicAdd(reinterpret_cast<unsigned long long *>(A.per + 4 * i), released);
+            if (released) atomicMax(A.per + 4 * i + 1, end);
+            if (held) atomicOr(reinterpret_cast<unsigned long long *>(A.per + 4 * i + 3), 1ull << 62);
+        }
+    }
+    grid.sync();
+    for (unsigned long long q = first_i; q < n_long; q += stride) {
+        const int64_t i = A.long_list[q];
+        const long long *p = A.per + 4 * i;
+        S.carry[kCarryWords * i + kCarryRestart] = p[1];
+        if (p[3] & (1ll << 62)) atomicAdd(A.stats + 1, 1ull);
+        count_finish(A, i, p[0], S.last && S.last[i]);
+    }
+}
+
 }  // namespace acb
 
 // ===========================================================================
@@ -2870,6 +3170,165 @@ int acb_stream_resolve(const acb_automaton *a, const void *dev_image, const uint
     if (emit_blocks > 16ll * d.sms) emit_blocks = 16ll * d.sms;
     stream_emit_kernel<<<(unsigned)emit_blocks, 256, 0, st>>>(A);
     g_launches++;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+int acb_stream_advance(const acb_automaton *a, const uint8_t *dev_bytes, const int64_t *dev_offsets, int64_t n_streams, uint64_t total_bytes,
+                       const uint8_t *dev_last, int codepoints, int64_t *dev_carry, uint8_t *dev_tail, const uint8_t *dev_seam_bytes,
+                       const int64_t *dev_seam_offsets, int64_t *dev_scratch, void *stream) {
+    if (!a || !dev_offsets || !dev_carry || !dev_seam_offsets || (total_bytes && !dev_bytes) || (codepoints && !dev_scratch))
+        return fail(ACB_EINVAL, "null argument");
+    const uint32_t halo = a->impl->hdr.max_pat_len ? a->impl->hdr.max_pat_len - 1 : 0;
+    if (halo && (!dev_tail || !dev_seam_bytes)) return fail(ACB_EINVAL, "null argument");
+    if (n_streams < 0 || n_streams > 0xfffffffell) return fail(ACB_EINVAL, "n_streams out of range (0 .. 2^32 - 2)");
+    if (total_bytes >= (1ull << 31)) return fail(ACB_EINVAL, "total_bytes must be below 2^31 (feed larger data in more chunks)");
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    if (n_streams == 0) return ACB_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    StreamArgs A = {};
+    A.B = Batch{dev_bytes, dev_offsets, n_streams};
+    A.carry = dev_carry;
+    A.tail = dev_tail;
+    A.last = dev_last;
+    A.seam = dev_seam_bytes;
+    A.seam_offsets = dev_seam_offsets;
+    A.halo = halo;
+    A.codepoints = codepoints ? 1 : 0;
+    if (codepoints) {  // continuation bytes of each chunk before its new tail, counted on the whole grid
+        A.cont_rows = reinterpret_cast<long long *>(dev_scratch);
+        A.cont_cp = reinterpret_cast<long long *>(dev_scratch + 3 * n_streams);
+        int64_t blocks = (n_streams + 255) / 256;
+        if (blocks > 8ll * d.sms) blocks = 8ll * d.sms;
+        stream_cont_rows_kernel<<<(unsigned)blocks, 256, 0, st>>>(A);
+        g_launches++;
+        CUDA_OK(cudaGetLastError());
+        if (int rc = acb_rows_to_codepoints(dev_bytes, dev_offsets, n_streams, total_bytes, reinterpret_cast<const int64_t *>(A.cont_rows),
+                                            reinterpret_cast<int64_t *>(A.cont_cp), stream))
+            return rc;
+    }
+    int64_t blocks = (n_streams + 7) / 8;  // a warp per stream
+    if (blocks > 16ll * d.sms) blocks = 16ll * d.sms;
+    stream_advance_kernel<<<(unsigned)blocks, 256, 0, st>>>(A);
+    g_launches++;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+int acb_stream_first_resolve(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                             int64_t n_streams, uint64_t total_bytes, const uint8_t *dev_last, int codepoints, const int64_t *dev_carry,
+                             const uint8_t *dev_seam_bytes, const int64_t *dev_seam_offsets, uint64_t seam_buffer_bytes,
+                             uint64_t *dev_seam_keys, uint64_t *dev_chunk_keys, int64_t *dev_best, int64_t *dev_scratch, int64_t *dev_rows,
+                             void *stream) {
+    if (!a || !dev_sieve || !dev_offsets || !dev_carry || !dev_seam_offsets || !dev_seam_keys || !dev_chunk_keys || !dev_best ||
+        !dev_scratch || !dev_rows || (total_bytes && !dev_bytes) || (seam_buffer_bytes && !dev_seam_bytes))
+        return fail(ACB_EINVAL, "null argument");
+    if (n_streams < 0 || n_streams > 0xfffffffell) return fail(ACB_EINVAL, "n_streams out of range (0 .. 2^32 - 2)");
+    if (total_bytes >= (1ull << 31) || seam_buffer_bytes >= (1ull << 31))
+        return fail(ACB_EINVAL, "total_bytes and seam_buffer_bytes must be below 2^31 (feed larger data in more chunks)");
+    SieveHeader sh;
+    if (int rc = sieve_header(a, sh)) return rc;
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CUDA_OK(cudaMemsetAsync(dev_scratch, 0, 2 * sizeof(uint64_t), st));
+    if (n_streams == 0) return ACB_OK;
+    const int64_t n = n_streams;
+    FirstArgs A;
+    A.B = Batch{dev_bytes, dev_offsets, n};
+    A.carry = dev_carry;
+    A.last = dev_last;
+    A.seam = dev_seam_bytes;
+    A.seam_offsets = dev_seam_offsets;
+    A.seam_keys = reinterpret_cast<unsigned long long *>(dev_seam_keys);
+    A.chunk_keys = reinterpret_cast<unsigned long long *>(dev_chunk_keys);
+    A.seam_rows = reinterpret_cast<long long *>(dev_scratch + 2);
+    A.chunk_rows = reinterpret_cast<long long *>(dev_scratch + 2 + 3 * n);
+    A.seam_cp = reinterpret_cast<long long *>(dev_scratch + 2 + 6 * n);
+    A.chunk_cp = reinterpret_cast<long long *>(dev_scratch + 2 + 9 * n);
+    A.best = reinterpret_cast<long long *>(dev_best);
+    A.rows = reinterpret_cast<long long *>(dev_rows);
+    A.stats = reinterpret_cast<unsigned long long *>(dev_scratch);
+    A.max_len = a->impl->hdr.max_pat_len;
+    A.kind = (int)a->impl->hdr.match_kind;
+    A.codepoints = codepoints ? 1 : 0;
+    int64_t blocks = (n + 127) / 128;
+    if (blocks > 16ll * d.sms) blocks = 16ll * d.sms;
+    stream_first_unmask_kernel<<<(unsigned)blocks, 128, 0, st>>>(A);
+    g_launches++;
+    CUDA_OK(cudaGetLastError());
+    const Batch seams{dev_seam_bytes, dev_seam_offsets, n};
+    if (int rc = acb_first_rows(a, dev_sieve, seams.bytes, seams.offsets, n, dev_seam_keys, dev_scratch + 2, stream)) return rc;
+    if (int rc = acb_first_rows(a, dev_sieve, dev_bytes, dev_offsets, n, dev_chunk_keys, dev_scratch + 2 + 3 * n, stream)) return rc;
+    if (codepoints) {
+        if (int rc = acb_rows_to_codepoints(seams.bytes, seams.offsets, n, seam_buffer_bytes, dev_scratch + 2, dev_scratch + 2 + 6 * n, stream))
+            return rc;
+        if (int rc = acb_rows_to_codepoints(dev_bytes, dev_offsets, n, total_bytes, dev_scratch + 2 + 3 * n, dev_scratch + 2 + 9 * n, stream))
+            return rc;
+    }
+    stream_first_resolve_kernel<<<(unsigned)blocks, 128, 0, st>>>(A);
+    g_launches++;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+int acb_stream_count(const acb_automaton *a, const uint8_t *dev_bytes, const int64_t *dev_offsets, int64_t n_streams, uint64_t total_bytes,
+                     const uint8_t *dev_last, int overlapping, int64_t *dev_carry, const int64_t *dev_seam_offsets,
+                     const acb_match *dev_seam_list, const uint64_t *dev_seam_match_offsets, const acb_match *dev_chunk_list,
+                     const uint64_t *dev_chunk_match_offsets, const uint64_t *dev_chunk_counts, int64_t *dev_running, int64_t *dev_counts,
+                     int64_t *dev_scratch, uint64_t scratch_words, void *stream) {
+    if (!a || !dev_offsets || !dev_carry || !dev_seam_offsets || !dev_seam_list || !dev_seam_match_offsets || !dev_running || !dev_counts ||
+        !dev_scratch || (total_bytes && !dev_bytes))
+        return fail(ACB_EINVAL, "null argument");
+    if (overlapping != 0 && overlapping != 1) return fail(ACB_EINVAL, "overlapping must be 0 or 1");
+    if (overlapping ? !dev_chunk_counts : (!dev_chunk_list || !dev_chunk_match_offsets)) return fail(ACB_EINVAL, "null argument");
+    if (n_streams < 0 || n_streams > 0xfffffffell) return fail(ACB_EINVAL, "n_streams out of range (0 .. 2^32 - 2)");
+    if (total_bytes >= (1ull << 31)) return fail(ACB_EINVAL, "total_bytes must be below 2^31 (feed larger data in more chunks)");
+    const uint64_t need = overlapping ? 4 : 4 + 6 * (uint64_t)n_streams;
+    if (scratch_words < need) return fail(ACB_EINVAL, "dev_scratch is too small");
+    const ImageHeader &h = a->impl->hdr;
+    const int kind = (int)h.match_kind;
+    if (overlapping && kind != ACB_STANDARD) return unsupported_overlapping(a);
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CUDA_OK(cudaMemsetAsync(dev_scratch, 0, 4 * sizeof(uint64_t), st));
+    if (n_streams == 0) return ACB_OK;
+    CountArgs A = {};
+    A.S.B = Batch{dev_bytes, dev_offsets, n_streams};
+    A.S.carry = dev_carry;
+    A.S.last = dev_last;
+    A.S.seam_offsets = dev_seam_offsets;
+    A.S.seam_list = reinterpret_cast<const uint4 *>(dev_seam_list);
+    A.S.chunk_list = reinterpret_cast<const uint4 *>(dev_chunk_list);
+    A.S.seam_mo = reinterpret_cast<const unsigned long long *>(dev_seam_match_offsets);
+    A.S.chunk_mo = reinterpret_cast<const unsigned long long *>(dev_chunk_match_offsets);
+    A.S.halo = h.max_pat_len ? h.max_pat_len - 1 : 0;
+    A.S.mode = overlapping ? kModeOverlap : (kind == ACB_STANDARD ? kModeStandard : kModeLeftmost);
+    A.S.longest = kind == ACB_LEFTMOST_LONGEST ? 1 : 0;
+    A.chunk_counts = reinterpret_cast<const unsigned long long *>(dev_chunk_counts);
+    A.running = reinterpret_cast<long long *>(dev_running);
+    A.out = reinterpret_cast<long long *>(dev_counts);
+    A.stats = reinterpret_cast<unsigned long long *>(dev_scratch);
+    if (overlapping) {
+        int64_t blocks = (n_streams + 127) / 128;
+        if (blocks > 16ll * d.sms) blocks = 16ll * d.sms;
+        stream_count_overlap_kernel<<<(unsigned)blocks, 128, 0, st>>>(A);
+        g_launches++;
+        CUDA_OK(cudaGetLastError());
+        return ACB_OK;
+    }
+    // records of both lists: each pair takes two words, each mark half of one
+    const uint64_t r_max = (scratch_words - need) / 4;
+    A.per = reinterpret_cast<long long *>(dev_scratch + 4);
+    A.long_list = reinterpret_cast<long long *>(dev_scratch + 4 + 4 * n_streams);
+    A.pairs = reinterpret_cast<uint4 *>(dev_scratch + need);
+    A.mark = reinterpret_cast<uint32_t *>(dev_scratch + need + 2 * r_max);
+    void *args[] = {&A};
+    const void *kern = A.S.mode == kModeStandard ? reinterpret_cast<const void *>(stream_count_kernel<kModeStandard>)
+                                                 : reinterpret_cast<const void *>(stream_count_kernel<kModeLeftmost>);
+    if (int rc = launch_cooperative(kern, args, d, st)) return rc;
     CUDA_OK(cudaGetLastError());
     return ACB_OK;
 }

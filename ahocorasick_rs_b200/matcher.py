@@ -1667,6 +1667,242 @@ class Stream:
         return self._feed(b"", True)
 
 
+class _QueryStreamBatch(StreamBatch):
+    """The stream forms of is_match, find_first and count_matches: one answer per stream after every feed, without the
+    rows.  They share StreamBatch's slots, limits, carry and seams (acb_stream_seams, then the kind's scans and resolve,
+    then acb_stream_advance; see include/acb200.h).  A feed with `last` returns those streams' final answers and
+    starts their slots again."""
+
+    MODE = ""
+    POSITIONS = False   # answers with positions (code points are carried for the str class)
+
+    def _feed_args(self, data, offsets, last):
+        torch = _torch()
+        n = self.n_streams
+        if not torch.is_tensor(data) or data.dtype != torch.uint8 or data.dim() != 1 or data.device.type != "cuda":
+            raise TypeError("data must be a 1-D uint8 CUDA tensor")
+        dev = self.device or data.device
+        if data.device != dev:
+            raise TypeError(f"data must be on {dev}, where this batch's streams live")
+        if not torch.is_tensor(offsets) or offsets.dtype != torch.int64 or offsets.shape != (n + 1,) or offsets.device != dev:
+            raise TypeError(f"offsets must be an int64 tensor of shape ({n + 1},) on {dev}")
+        if last is not None and (not torch.is_tensor(last) or last.dtype != torch.bool or last.shape != (n,) or last.device != dev):
+            raise TypeError(f"last must be None or a bool tensor of shape ({n},) on {dev}")
+        if data.numel() > self._ac.WINDOW_BYTES:
+            raise ValueError(f"one feed addresses at most {self._ac.WINDOW_BYTES} bytes (WINDOW_BYTES): feed larger data in more chunks")
+        _require_cuda()
+        return dev, data.contiguous(), offsets.contiguous(), (last.contiguous().view(torch.uint8) if last is not None else None)
+
+    def feed_device(self, data, offsets, last=None):
+        """One chunk per stream, as StreamBatch.feed_device takes them -> the answers after this feed (a CUDA tensor,
+        see the subclass)."""
+        torch = _torch()
+        dev, data, offsets, last_u8 = self._feed_args(data, offsets, last)
+        ac, L = self._ac, self._ac._L
+        with self._lock, ac._lock, torch.cuda.device(dev):
+            if self.device is None:
+                self._allocate(dev)
+                self._allocate_query(dev)
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            rc = L.acb_stream_seams(ac._h, data.data_ptr(), offsets.data_ptr(), self.n_streams, data.numel(), self._carry.data_ptr(),
+                                    self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(), stream)
+            if rc != _capi.ACB_OK:
+                raise RuntimeError(_capi.last_error())
+            out, stats = self._query(dev, data, offsets, last_u8, stream)
+            cp = self._codepoints and self.POSITIONS
+            scratch = torch.empty(6 * self.n_streams if cp else 1, dtype=torch.int64, device=dev)
+            rc = L.acb_stream_advance(ac._h, data.data_ptr(), offsets.data_ptr(), self.n_streams, data.numel(),
+                                      last_u8.data_ptr() if last_u8 is not None else None, int(cp), self._carry.data_ptr(),
+                                      self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(), scratch.data_ptr(), stream)
+            if rc != _capi.ACB_OK:
+                raise RuntimeError(_capi.last_error())
+            task_bytes = int(ac._plan(data, max(self.n_streams, 1)).task_bytes)
+            self.last_stats = {"engine": "sieve", "mode": self.MODE, **ac.sieve_geometry(dev, task_bytes),
+                               "seam_bytes": int(self._seam_offsets[self.n_streams].item()), **stats}
+        ac.last_stats = dict(self.last_stats)
+        return out
+
+    def _skips(self, scratch):
+        """tasks_skipped / windows_skipped of an acb_any_match or acb_find_first scratch (one synchronisation)."""
+        _, skipped, windows = scratch.tolist()
+        return {"tasks_skipped": skipped, "windows_skipped": windows}
+
+
+class IsMatchStreamBatch(_QueryStreamBatch):
+    """is_match per stream: feed_device returns a bool CUDA tensor (n_streams,), flag i = is_match(the stream's
+    concatenation so far).  A flag stays set until its stream ends; the chunks of a flagged stream are skipped by the
+    scan's task skip, so a stream that has matched costs almost nothing to keep feeding."""
+
+    MODE = "is_match_stream"
+
+    def _allocate_query(self, dev):
+        self._flags = _torch().zeros(self.n_streams, dtype=_torch().bool, device=dev)
+
+    def _query(self, dev, data, offsets, last_u8, stream):
+        torch = _torch()
+        ac, L, n = self._ac, self._ac._L, self.n_streams
+        sieve_t, _ = ac.sieve(dev)
+        scratch = torch.empty((2, 3), dtype=torch.int64, device=dev)
+        # the seams first: a stream whose match crosses the cut then has its chunk skipped
+        for k, (b, o) in enumerate(((self._seam, self._seam_offsets), (data, offsets))):
+            rc = L.acb_any_match(ac._h, sieve_t.data_ptr(), b.data_ptr(), o.data_ptr(), n, b.numel(), self._flags.data_ptr(),
+                                 scratch[k].data_ptr(), stream)
+            if rc != _capi.ACB_OK:
+                raise RuntimeError(_capi.last_error())
+        out = self._flags.clone()
+        if last_u8 is not None:
+            self._flags.masked_fill_(last_u8.view(torch.bool), False)
+        return out, {**self._skips(scratch[1]), "flagged": int(out.sum().item())}
+
+
+class FindFirstStreamBatch(_QueryStreamBatch):
+    """find_first per stream: feed_device returns an int64 CUDA tensor (n_streams, 3): row i is find_first of the
+    stream's whole concatenation, (pattern, start, end), as soon as no later data can change it -- Standard at once,
+    the leftmost kinds once start + max_pattern_len <= the bytes fed, every stream on `last` -- and (-1, -1, -1) before
+    that (or after `last` when the stream had no match).  Byte offsets, or code point indexes for the str class."""
+
+    MODE = "find_first_stream"
+    POSITIONS = True
+
+    def _allocate_query(self, dev):
+        torch = _torch()
+        n = self.n_streams
+        self._best = torch.zeros((n, 6), dtype=torch.int64, device=dev)
+        self._keys = torch.full((2, n), -1, dtype=torch.int64, device=dev)   # seam keys, chunk keys: ~0 = scan
+
+    def _query(self, dev, data, offsets, last_u8, stream):
+        torch = _torch()
+        ac, L, n = self._ac, self._ac._L, self.n_streams
+        ac.first_keys(self._seam, self._seam_offsets, self._keys[0])
+        chunk_scratch = ac.first_keys(data, offsets, self._keys[1])
+        scratch = torch.empty(2 + 12 * n, dtype=torch.int64, device=dev)
+        rows = torch.empty((n, 3), dtype=torch.int64, device=dev)
+        rc = L.acb_stream_first_resolve(ac._h, ac.sieve(dev)[0].data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
+                                        last_u8.data_ptr() if last_u8 is not None else None, int(self._codepoints), self._carry.data_ptr(),
+                                        self._seam.data_ptr(), self._seam_offsets.data_ptr(), self._seam.numel(), self._keys[0].data_ptr(),
+                                        self._keys[1].data_ptr(), self._best.data_ptr(), scratch.data_ptr(), rows.data_ptr(), stream)
+        if rc != _capi.ACB_OK:
+            raise RuntimeError(_capi.last_error())
+        return rows, {**self._skips(chunk_scratch), "pending": int(scratch[1].item())}
+
+
+class CountStreamBatch(_QueryStreamBatch):
+    """count_matches per stream: feed_device returns an int64 CUDA tensor (n_streams,), count i = the number of rows the
+    stream search (stream_batch, same `overlapping`) would have released so far; after `last`, count_matches of the
+    stream's concatenation.  Overlapping: the sieve's count mode on the chunks plus the seam records that cross the
+    cut, no rows.  Non-overlapping: the stream search's two lists, with the selection counted (one thread per stream, or
+    the whole grid for a stream with more than ACB_LONG_STRETCH records)."""
+
+    MODE = "count_stream"
+
+    def _allocate_query(self, dev):
+        self._running = _torch().zeros(self.n_streams, dtype=_torch().int64, device=dev)
+
+    def _query(self, dev, data, offsets, last_u8, stream):
+        torch = _torch()
+        ac, L, n = self._ac, self._ac._L, self.n_streams
+        m_s, mo_s, tot_s = ac.scan_device(self._seam, self._seam_offsets, 2, False, ws_slot=self._slots[1])
+        if self.overlapping:
+            chunk_counts = torch.zeros(n, dtype=torch.int64, device=dev)
+            scratch = torch.empty(3, dtype=torch.int64, device=dev)
+            rc = L.acb_count_overlapping(ac._h, ac.sieve(dev)[0].data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
+                                         chunk_counts.data_ptr(), scratch.data_ptr(), stream)
+            if rc != _capi.ACB_OK:
+                raise RuntimeError(_capi.last_error())
+            m_c = mo_c = None
+            words = 4
+        else:
+            m_c, mo_c, tot_c = ac.scan_device(data, offsets, 2, False, ws_slot=self._slots[0])
+            chunk_counts = None
+            words = 4 + 6 * n + 4 * (int(tot_c) + int(tot_s))
+        if m_s.dtype != torch.int32 or (m_c is not None and m_c.dtype != torch.int32):
+            raise RuntimeError("stream count: a list came back in the windowed int64 form acb_stream_count cannot read")
+
+        def ptr(t):   # an empty list is still a view of its workspace's buffer: pass that buffer's (non-null) address
+            return t.data_ptr() if t.numel() else t.untyped_storage().data_ptr() + t.storage_offset() * t.element_size()
+
+        scratch = torch.empty(words, dtype=torch.int64, device=dev)
+        counts = torch.empty(n, dtype=torch.int64, device=dev)
+        rc = L.acb_stream_count(ac._h, data.data_ptr(), offsets.data_ptr(), n, data.numel(), last_u8.data_ptr() if last_u8 is not None else None,
+                                int(self.overlapping), self._carry.data_ptr(), self._seam_offsets.data_ptr(), ptr(m_s), mo_s.data_ptr(),
+                                ptr(m_c) if m_c is not None else None, mo_c.data_ptr() if mo_c is not None else None,
+                                chunk_counts.data_ptr() if chunk_counts is not None else None, self._running.data_ptr(), counts.data_ptr(),
+                                scratch.data_ptr(), words, stream)
+        if rc != _capi.ACB_OK:
+            raise (ValueError if rc == _capi.ACB_EUNSUPPORTED else RuntimeError)(_capi.last_error())
+        records, held, long_stretches = scratch[:3].tolist()
+        return counts, {"records": records, "held": held, "long_stretches": long_stretches}
+
+
+class QueryStream:
+    """One query stream fed from the host (a query batch of one, with its own pinned staging buffer): feed(chunk) and
+    finish() return the answer after the feed (see the batch classes); finish() ends the stream."""
+
+    def __init__(self, batch: _QueryStreamBatch, answer):
+        self._batch = batch
+        self._answer = answer
+        self._codepoints = batch._codepoints
+        self._offs = None
+        self._pinned = None
+        self._lock = threading.Lock()
+        self._done = False
+
+    @property
+    def last_stats(self):
+        return self._batch.last_stats
+
+    def feed(self, chunk):
+        """The next chunk (a str for AhoCorasick, a bytes-like object for BytesAhoCorasick) -> the answer so far."""
+        if self._codepoints:
+            if not isinstance(chunk, str):
+                raise TypeError("argument 'chunk': 'str' expected")
+            return self._feed(chunk.encode("utf-8"), False)
+        return self._feed(_as_buffer_bytes(chunk), False)
+
+    def finish(self):
+        """The final answer; ends the stream."""
+        return self._feed(b"", True)
+
+    def _feed(self, chunk, last: bool):
+        if self._done:
+            raise RuntimeError("the stream is finished: feed after finish()")
+        n = len(chunk)
+        ac = self._batch._ac
+        if n > ac.WINDOW_BYTES:
+            raise ValueError(f"one feed addresses at most {ac.WINDOW_BYTES} bytes (WINDOW_BYTES): feed larger data in more chunks")
+        torch = _require_cuda()
+        dev = self._batch.device or torch.device("cuda", torch.cuda.current_device())
+        if self._offs is None:
+            self._offs = torch.zeros(2, dtype=torch.int64, device=dev)
+        with self._lock:   # the staging buffer is reused once the answer is on the host
+            if self._pinned is None or self._pinned.numel() < n:
+                self._pinned = torch.empty(max(n, 1 << 16), dtype=torch.uint8, pin_memory=True)
+            host = self._pinned
+            if n:
+                host.numpy()[:n] = np.frombuffer(chunk, dtype=np.uint8)
+            d = host[:n].to(dev, non_blocking=True)
+            self._offs[1] = n
+            out = self._batch.feed_device(d, self._offs, torch.ones(1, dtype=torch.bool, device=dev) if last else None)
+            ans = self._answer(out[0].tolist())
+        if last:
+            self._done = True
+        return ans
+
+
+def _first_answer(row):
+    return tuple(row) if row[0] >= 0 else None
+
+
+def _query_stream_batch(ac, kind: str, n_streams: int, overlapping: bool, codepoints: bool) -> _QueryStreamBatch:
+    cls = {"is_match": IsMatchStreamBatch, "find_first": FindFirstStreamBatch, "count": CountStreamBatch}[kind]
+    return cls(ac, n_streams, overlapping, codepoints)
+
+
+def _query_stream(ac, kind: str, overlapping: bool, codepoints: bool) -> QueryStream:
+    answer = {"is_match": bool, "find_first": _first_answer, "count": int}[kind]
+    return QueryStream(_query_stream_batch(ac, kind, 1, overlapping, codepoints), answer)
+
+
 def _as_buffer_bytes(obj) -> bytes:
     """reference PyBufferBytes::try_from (src/lib.rs:281-302): 1-D, C-contiguous u8 buffer."""
     if isinstance(obj, str):
@@ -1884,6 +2120,36 @@ class AhoCorasick:
         stream (it may cut a character); positions are code point indexes (see StreamBatch)."""
         return StreamBatch(self._ac, n_streams, overlapping, codepoints=True)
 
+    def is_match_stream_batch(self, n_streams: int) -> IsMatchStreamBatch:
+        """``n_streams`` is_match streams fed from the device: ``feed_device(data, offsets, last=None)`` -> bool CUDA
+        tensor (n,), is_match of each stream's concatenation so far (see IsMatchStreamBatch)."""
+        return _query_stream_batch(self._ac, "is_match", n_streams, False, codepoints=True)
+
+    def find_first_stream_batch(self, n_streams: int) -> FindFirstStreamBatch:
+        """``n_streams`` find_first streams fed from the device: ``feed_device(data, offsets, last=None)`` -> int64 CUDA
+        tensor (n, 3), each stream's first match once final, -1 rows while unknown (see FindFirstStreamBatch)."""
+        return _query_stream_batch(self._ac, "find_first", n_streams, False, codepoints=True)
+
+    def count_matches_stream_batch(self, n_streams: int, overlapping: bool = False) -> CountStreamBatch:
+        """``n_streams`` count streams fed from the device: ``feed_device(data, offsets, last=None)`` -> int64 CUDA tensor
+        (n,), the matches each stream's search has released so far (see CountStreamBatch)."""
+        return _query_stream_batch(self._ac, "count", n_streams, overlapping, codepoints=True)
+
+    def is_match_stream(self) -> QueryStream:
+        """One is_match stream: ``feed(chunk)`` and ``finish()`` -> bool, does the concatenation so far contain a pattern."""
+        return _query_stream(self._ac, "is_match", False, codepoints=True)
+
+    def find_first_stream(self) -> QueryStream:
+        """One find_first stream: ``feed(chunk)`` and ``finish()`` -> (pattern, start, end) once no later data can change
+        it, else None; ``finish()`` gives the final answer."""
+        return _query_stream(self._ac, "find_first", False, codepoints=True)
+
+    def count_matches_stream(self, overlapping: bool = False) -> QueryStream:
+        """One count stream: ``feed(chunk)`` -> the matches released so far, ``finish()`` -> count_matches of the
+        whole concatenation."""
+        self._ac.check_overlapping(overlapping)
+        return _query_stream(self._ac, "count", overlapping, codepoints=True)
+
     def scan_host(self, data, offsets, overlapping: bool = False, **kw):
         """Host-resident UTF-8 batch (uint8 array + int64 offsets) -> host arrays (matches (k, 4), match_offsets (n + 1));
         code point indexes.  Copies and scans are pipelined (see _Automaton.scan_host)."""
@@ -2019,6 +2285,36 @@ class BytesAhoCorasick:
         """``n_streams`` streams fed from the device: ``feed_device(data, offsets, last=None)`` takes one chunk per
         stream; positions are byte offsets (see StreamBatch)."""
         return StreamBatch(self._ac, n_streams, overlapping, codepoints=False)
+
+    def is_match_stream_batch(self, n_streams: int) -> IsMatchStreamBatch:
+        """``n_streams`` is_match streams fed from the device: ``feed_device(data, offsets, last=None)`` -> bool CUDA
+        tensor (n,), is_match of each stream's concatenation so far (see IsMatchStreamBatch)."""
+        return _query_stream_batch(self._ac, "is_match", n_streams, False, codepoints=False)
+
+    def find_first_stream_batch(self, n_streams: int) -> FindFirstStreamBatch:
+        """``n_streams`` find_first streams fed from the device: ``feed_device(data, offsets, last=None)`` -> int64 CUDA
+        tensor (n, 3), each stream's first match once final, -1 rows while unknown (see FindFirstStreamBatch)."""
+        return _query_stream_batch(self._ac, "find_first", n_streams, False, codepoints=False)
+
+    def count_matches_stream_batch(self, n_streams: int, overlapping: bool = False) -> CountStreamBatch:
+        """``n_streams`` count streams fed from the device: ``feed_device(data, offsets, last=None)`` -> int64 CUDA tensor
+        (n,), the matches each stream's search has released so far (see CountStreamBatch)."""
+        return _query_stream_batch(self._ac, "count", n_streams, overlapping, codepoints=False)
+
+    def is_match_stream(self) -> QueryStream:
+        """One is_match stream: ``feed(chunk)`` and ``finish()`` -> bool, does the concatenation so far contain a pattern."""
+        return _query_stream(self._ac, "is_match", False, codepoints=False)
+
+    def find_first_stream(self) -> QueryStream:
+        """One find_first stream: ``feed(chunk)`` and ``finish()`` -> (pattern, start, end) once no later data can change
+        it, else None; ``finish()`` gives the final answer."""
+        return _query_stream(self._ac, "find_first", False, codepoints=False)
+
+    def count_matches_stream(self, overlapping: bool = False) -> QueryStream:
+        """One count stream: ``feed(chunk)`` -> the matches released so far, ``finish()`` -> count_matches of the
+        whole concatenation."""
+        self._ac.check_overlapping(overlapping)
+        return _query_stream(self._ac, "count", overlapping, codepoints=False)
 
     def scan_host(self, data, offsets, overlapping: bool = False, **kw):
         """Host-resident batch (uint8 array + int64 offsets) -> host arrays (matches (k, 4), match_offsets (n + 1));

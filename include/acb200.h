@@ -469,6 +469,75 @@ int acb_stream_resolve(const acb_automaton *a, const void *dev_image, const uint
                        int64_t *dev_scratch, int64_t *dev_rows, int64_t *dev_row_offsets, void *stream);
 
 /*
+ * Stream queries: is_match, find_first and count_matches per stream, without the rows.  They keep the stream search's
+ * carry and tail (dev_carry, dev_tail above; word [1] is used by the non-overlapping count only) and its seams: a feed
+ * starts with acb_stream_seams and ends with acb_stream_advance.  Let C be a stream's concatenation so far, F = len(C).
+ *
+ * acb_stream_advance updates the carry without a selection: the new tail, F and T, and with codepoints != 0 the
+ * continuation bytes before the tail (dev_scratch = int64[6 * n_streams], else it may be null).  A stream with
+ * dev_last[i] != 0 gets a zero carry.  It reads the seams, so it runs after the feed's scans.  With code points a
+ * launch, acb_rows_to_codepoints' copy and launch, then one launch; without, one launch.
+ *
+ * is_match: acb_any_match on the seams and on the chunks, with the same persistent dev_flags (u8[n_streams], zero for
+ * a new stream): flag i is then is_match(C), and a stream already flagged has its chunk tasks skipped whole.  The
+ * caller reads the flags, and zeroes those of the streams that end.
+ *
+ * find_first: per stream, dev_best = int64[n_streams][6], zero for a new stream: [0] state (0 no candidate, 1 a pending
+ * one, 2 the final answer), [1] pattern, [2] start, [3] end (absolute byte offsets), [4] start, [5] end in code points
+ * (the byte offsets without codepoints).  dev_seam_keys and dev_chunk_keys = u64[n_streams], ~0 for a new stream, are
+ * the keys of acb_find_first on the seams and on the chunks; acb_stream_first_resolve leaves them ready for the next
+ * feed: 0 where that scan can be skipped (a final answer: both; a pending leftmost candidate: the chunk's, whose
+ * records all start after it), ~0 elsewhere.  A feed: acb_stream_seams, acb_find_first on the seams and on the
+ * chunks, acb_stream_first_resolve, acb_stream_advance.  The resolve decodes both keys (acb_first_rows; keys that
+ * were pre-set to 0 are ignored), converts them to code points (acb_rows_to_codepoints; the carried continuation
+ * count gives the part before the seam), takes the best of the carried candidate and the two under the kind's key
+ * order above, and applies the release rule: Standard is final at once (end <= F), the leftmost kinds once start +
+ * max_pattern_len <= F, every candidate on dev_last.  dev_rows = int64[n_streams][3] gets each final answer
+ * (pattern, start, end) -- code point indexes with codepoints != 0 -- and (-1, -1, -1) elsewhere; a stream that ends
+ * gets its final answer and a zero dev_best.  dev_seam_bytes, dev_seam_offsets are the seams' buffers,
+ * seam_buffer_bytes the length of dev_seam_bytes (below 2^31).  dev_scratch = int64[2 + 12 * n_streams]: it leaves
+ * [1] = streams with a pending candidate.  A memset and seven launches (eleven with code points: two copies and two
+ * launches of acb_rows_to_codepoints), no synchronisation.
+ *
+ * count_matches: dev_running = int64[n_streams], zero for a new stream.  acb_stream_count adds this feed's count and
+ * writes dev_counts = int64[n_streams]: the number of rows the stream search would have released so far (after a
+ * feed with dev_last[i], len(find_matches_as_indexes(C, overlapping))); it zeroes dev_running[i] of a stream that
+ * ends, and acb_stream_advance follows it.
+ *   overlapping = 1 (Standard only; a leftmost automaton returns ACB_EUNSUPPORTED): a feed is acb_stream_seams,
+ *     acb_scan_batch (overlapping = 2) on the seams, acb_count_overlapping on the chunks into zeroed dev_chunk_counts
+ *     = u64[n_streams], acb_stream_count, acb_stream_advance.  The count adds the chunk's and the seam records that
+ *     cross the tail / head join (start < T < end).  dev_chunk_list and its offsets may be null.  dev_scratch =
+ *     int64[4].  A memset and one launch.
+ *   overlapping = 0, every kind: the two scans of the stream search (acb_scan_batch, overlapping = 2, on the chunks
+ *     and on the seams), then acb_stream_count, which continues the selection from the carried restart point (word
+ *     [1]) and counts the picks the release rule allows.  A stream whose sequence has at most ACB_LONG_STRETCH
+ *     records is counted by one thread; a longer one by the whole grid (successors, pointer jumping, marks on the
+ *     selected chain, as acb_pattern_counts_non_overlapping).  dev_chunk_counts may be null.  dev_scratch =
+ *     int64[scratch_words], scratch_words >= 4 + 6 * n_streams + 4 * R, R = the two lists' lengths added.  A memset
+ *     and one cooperative launch.
+ *   dev_scratch leaves [0] = list records considered, [1] = streams holding a pick the release rule does not allow
+ *   yet, [2] = streams counted on the whole grid.
+ *
+ * All three return ACB_EINVAL, before any CUDA call, for a null pointer (dev_bytes may be null when total_bytes == 0,
+ * dev_tail and dev_seam_bytes when max_pattern_len == 1), n_streams outside [0, 2^32 - 2], total_bytes >= 2^31,
+ * overlapping other than 0 / 1 or a dev_scratch too small; acb_stream_first_resolve also for an automaton without a
+ * sieve image.  n_streams == 0 launches nothing.
+ */
+int acb_stream_advance(const acb_automaton *a, const uint8_t *dev_bytes, const int64_t *dev_offsets, int64_t n_streams, uint64_t total_bytes,
+                       const uint8_t *dev_last, int codepoints, int64_t *dev_carry, uint8_t *dev_tail, const uint8_t *dev_seam_bytes,
+                       const int64_t *dev_seam_offsets, int64_t *dev_scratch, void *stream);
+int acb_stream_first_resolve(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                             int64_t n_streams, uint64_t total_bytes, const uint8_t *dev_last, int codepoints, const int64_t *dev_carry,
+                             const uint8_t *dev_seam_bytes, const int64_t *dev_seam_offsets, uint64_t seam_buffer_bytes,
+                             uint64_t *dev_seam_keys, uint64_t *dev_chunk_keys, int64_t *dev_best, int64_t *dev_scratch, int64_t *dev_rows,
+                             void *stream);
+int acb_stream_count(const acb_automaton *a, const uint8_t *dev_bytes, const int64_t *dev_offsets, int64_t n_streams, uint64_t total_bytes,
+                     const uint8_t *dev_last, int overlapping, int64_t *dev_carry, const int64_t *dev_seam_offsets,
+                     const acb_match *dev_seam_list, const uint64_t *dev_seam_match_offsets, const acb_match *dev_chunk_list,
+                     const uint64_t *dev_chunk_match_offsets, const uint64_t *dev_chunk_counts, int64_t *dev_running, int64_t *dev_counts,
+                     int64_t *dev_scratch, uint64_t scratch_words, void *stream);
+
+/*
  * Multi-GPU: the fixed-size block a rank contributes to the gather of the per-shard match lists (the only exchange
  * of the sharded path; NCCL all-gather over NVLink).  dev_block holds (cap + 1) records of 16 bytes: record 0 =
  * (match count, hay_base, complete flag, 0), then the first `cap` matches of a finished scan (dev_total / dev_out of
