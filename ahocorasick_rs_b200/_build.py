@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libacb200.so")
 STAMP = LIB + ".cmd"
 SOURCES = ["capi.cu", "automaton.cpp", "sieve.cpp"]
-HEADERS = ["automaton.h", "scan_core.cuh", "scan_staged.cuh", "scan_global.cuh", "scan_sieve.cuh", "sieve.h", "repair.cuh", os.path.join("..", "..", "include", "acb200.h")]
+HEADERS = ["automaton.h", "scan_core.cuh", "scan_staged.cuh", "scan_global.cuh", "scan_sieve.cuh", "sieve.h", "repair.cuh", "tokens.cuh", os.path.join("..", "..", "include", "acb200.h")]
 FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-diag-suppress", "186",
          "-shared", "-Xcompiler", "-fPIC,-pthread"]
 

@@ -12,6 +12,8 @@ LIB_PATH = os.environ.get("ACB200_LIB") or os.path.join(HERE, "libacb200.so")
 
 ACB_OK = 0
 ACB_EINVAL, ACB_EBUILD, ACB_EUNSUPPORTED, ACB_ECUDA, ACB_ECAPACITY = -1, -2, -3, -4, -5
+ACB_TOKEN_ID_LIMIT = 1 << 21   # include/acb200.h: token ids lie in [0, ACB_TOKEN_ID_LIMIT)
+ACB_TOKEN_BYTES = 3            # ... and each becomes this many bytes (csrc/tokens.cuh)
 ACB_LONG_STRETCH = 4096   # include/acb200.h: longer per-haystack overlapping lists are counted by the whole grid
 
 
@@ -118,6 +120,8 @@ def lib():
                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64] + [C.c_void_p] * 6
         L.acb_stream_count.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64, C.c_void_p, C.c_int] + [C.c_void_p] * 10 + [
             C.c_uint64, C.c_void_p]
+        L.acb_tokens_encode.argtypes = [C.c_void_p, C.c_int, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.acb_tokens_encode_host.argtypes = [C.c_void_p, C.c_int, C.c_uint64, C.c_void_p, C.c_void_p]
         L.acb_pack_gather_block.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p, C.c_void_p]
         L.acb_scan_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(HotDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                      C.c_uint64, C.c_int, C.c_int, C.POINTER(Plan), C.POINTER(Workspace), C.c_void_p]
@@ -156,4 +160,5 @@ EXPORTS = [
     "acb_count_overlapping", "acb_count_non_overlapping", "acb_count_rows", "acb_stream_seams", "acb_stream_resolve",
     "acb_pattern_counts_overlapping", "acb_pattern_counts_non_overlapping", "acb_pattern_hits",
     "acb_pattern_hit_row_words", "acb_stream_advance", "acb_stream_first_resolve", "acb_stream_count",
+    "acb_tokens_encode", "acb_tokens_encode_host",
 ]

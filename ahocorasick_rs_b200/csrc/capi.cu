@@ -14,6 +14,7 @@
 #include "scan_staged.cuh"
 #include "scan_global.cuh"
 #include "scan_sieve.cuh"
+#include "tokens.cuh"
 
 namespace acb {
 
@@ -2881,6 +2882,54 @@ int acb_rows_to_codepoints(const uint8_t *dev_bytes, const int64_t *dev_offsets,
                                                                 reinterpret_cast<long long *>(dev_cp_rows));
     g_launches++;
     CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+}  // extern "C"
+
+template <typename T>
+static void tokens_launch(const void *ids, uint64_t n, uint8_t *out, uint64_t *bad, int sms, cudaStream_t st) {
+    const bool vec = (reinterpret_cast<uintptr_t>(ids) & 15u) == 0 && (reinterpret_cast<uintptr_t>(out) & 3u) == 0;
+    const uint64_t items = vec ? n / kTokGroup + n % kTokGroup : n;   // groups, then the tail's ids one per thread
+    uint64_t blocks = (items + kTokThreads - 1) / kTokThreads;
+    if (blocks > 8ull * (uint64_t)sms) blocks = 8ull * (uint64_t)sms;  // a full SM of 256-thread blocks, grid-stride beyond
+    if (blocks < 1) blocks = 1;
+    const T *p = static_cast<const T *>(ids);
+    auto *b = reinterpret_cast<unsigned long long *>(bad);
+    if (vec)
+        tokens_encode_kernel<T, true><<<(unsigned)blocks, kTokThreads, 0, st>>>(p, n, out, b);
+    else
+        tokens_encode_kernel<T, false><<<(unsigned)blocks, kTokThreads, 0, st>>>(p, n, out, b);
+    g_launches++;
+}
+
+extern "C" {
+
+static int tokens_check(const void *ids, int token_bytes, uint64_t n, const uint8_t *out, const uint64_t *bad) {
+    if (token_bytes != 2 && token_bytes != 4 && token_bytes != 8) return fail(ACB_EINVAL, "token_bytes must be 2, 4 or 8");
+    if (n >= (1ull << 60)) return fail(ACB_EINVAL, "n_tokens out of range (0 .. 2^60 - 1)");
+    if (!bad || (n && (!ids || !out))) return fail(ACB_EINVAL, "null argument");
+    return ACB_OK;
+}
+
+int acb_tokens_encode(const void *dev_tokens, int token_bytes, uint64_t n_tokens, uint8_t *dev_out, uint64_t *dev_bad, void *stream) {
+    if (int rc = tokens_check(dev_tokens, token_bytes, n_tokens, dev_out, dev_bad)) return rc;
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    if (n_tokens == 0) return ACB_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (token_bytes == 2) tokens_launch<uint16_t>(dev_tokens, n_tokens, dev_out, dev_bad, d.sms, st);
+    else if (token_bytes == 4) tokens_launch<int32_t>(dev_tokens, n_tokens, dev_out, dev_bad, d.sms, st);
+    else tokens_launch<int64_t>(dev_tokens, n_tokens, dev_out, dev_bad, d.sms, st);
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+int acb_tokens_encode_host(const void *host_tokens, int token_bytes, uint64_t n_tokens, uint8_t *host_out, uint64_t *host_bad) {
+    if (int rc = tokens_check(host_tokens, token_bytes, n_tokens, host_out, host_bad)) return rc;
+    if (token_bytes == 2) token_encode_host(static_cast<const uint16_t *>(host_tokens), n_tokens, host_out, host_bad);
+    else if (token_bytes == 4) token_encode_host(static_cast<const int32_t *>(host_tokens), n_tokens, host_out, host_bad);
+    else token_encode_host(static_cast<const int64_t *>(host_tokens), n_tokens, host_out, host_bad);
     return ACB_OK;
 }
 

@@ -16,6 +16,9 @@ are already device resident; ``is_match`` / ``is_match_batch`` /
 ``count_matches_device``, the length of each haystack's match list without the list;
 ``count_matches_by_pattern`` / ``count_matches_by_pattern_batch`` /
 ``count_matches_by_pattern_device``, how many matches each pattern has over a batch.
+
+``TokenAhoCorasick`` is the same API over token-id sequences (uint16 / int32 / int64): the ids are encoded into a
+self-synchronising 3-byte format (include/acb200.h) and searched as bytes, positions divided by 3.
 """
 from __future__ import annotations
 
@@ -2320,3 +2323,411 @@ class BytesAhoCorasick:
         """Host-resident batch (uint8 array + int64 offsets) -> host arrays (matches (k, 4), match_offsets (n + 1));
         byte offsets.  Copies and scans are pipelined (see _Automaton.scan_host)."""
         return self._ac.scan_host(data, offsets, overlapping, codepoints=False, **kw)
+
+
+# ---- token ids: TokenAhoCorasick -------------------------------------------------------------------------------------
+# Every id becomes ACB_TOKEN_BYTES bytes of a self-synchronising format (include/acb200.h, csrc/tokens.cuh: only a
+# token's first byte has its high bit set), so a byte search over the encoded ids is exactly the token search with
+# positions multiplied by 3.  Every query runs the byte path (codepoints=False) and divides the start and end columns.
+
+_TOKEN_WIDTHS = (np.dtype(np.uint16), np.dtype(np.int32), np.dtype(np.int64))   # what acb_tokens_encode(_host) read
+
+
+def _token_range_error(what: str, index: int, value) -> ValueError:
+    return ValueError(f"{what}: token {index} = {value} is outside [0, {_capi.ACB_TOKEN_ID_LIMIT}) (ACB_TOKEN_ID_LIMIT)")
+
+
+def _encode_host_tokens(seq, what: str) -> np.ndarray:
+    """One 1-D integer sequence (list, tuple, numpy array or memmap, CPU tensor) -> its encoded bytes, a uint8 numpy
+    array of 3 bytes per id (acb_tokens_encode_host).  TypeError for anything but integers, ValueError naming `what`,
+    the index and the value of the first id outside [0, 2^21)."""
+    torch = __import__("sys").modules.get("torch")
+    if torch is not None and torch.is_tensor(seq):
+        if seq.device.type != "cpu":
+            raise TypeError(f"{what}: a CUDA tensor goes to the *_device methods; this form takes host sequences")
+        seq = seq.detach().numpy()
+    try:
+        a = np.asarray(seq)
+    except ValueError as e:   # ragged nesting
+        raise TypeError(f"{what} must be a one-dimensional sequence of token ids") from e
+    if a.ndim != 1:
+        raise TypeError(f"{what} must be a one-dimensional sequence of token ids")
+    if a.size == 0:
+        return np.zeros(0, dtype=np.uint8)
+    if a.dtype == object:   # Python ints beyond int64, or mixed objects
+        for j, v in enumerate(a.tolist()):
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+                raise TypeError(f"{what}: token ids must be integers, not {type(v).__name__}")
+            if not 0 <= v < _capi.ACB_TOKEN_ID_LIMIT:
+                raise _token_range_error(what, j, v)
+        ids = np.asarray(a.tolist(), dtype=np.int64)
+    elif a.dtype.kind not in "iu":
+        raise TypeError(f"{what}: token ids must be integers, not {a.dtype}")
+    elif a.dtype in _TOKEN_WIDTHS:
+        ids = np.ascontiguousarray(a)
+    else:   # narrower ints widen to int32, uint32 / uint64 to int64 (an id past 2^63 wraps negative: still out of range)
+        ids = np.ascontiguousarray(a, dtype=np.int32 if a.itemsize < 4 else np.int64)
+    out = np.empty(_capi.ACB_TOKEN_BYTES * ids.size, dtype=np.uint8)
+    bad = np.full(1, np.iinfo(np.uint64).max, dtype=np.uint64)
+    if _capi.lib().acb_tokens_encode_host(ids.ctypes.data, ids.itemsize, ids.size, out.ctypes.data, bad.ctypes.data) != _capi.ACB_OK:
+        raise RuntimeError(_capi.last_error())
+    if bad[0] != np.iinfo(np.uint64).max:
+        j = int(bad[0])
+        raise _token_range_error(what, j, int(a[j]))
+    return out
+
+
+def _token_offsets(offsets, tokens):
+    """Token offsets -> byte offsets (x 3).  They must lie in [0, len(tokens)] (one synchronisation): a larger or
+    negative offset would wrap in the multiplication and could put a haystack boundary inside a token."""
+    torch = _torch()
+    if not torch.is_tensor(offsets) or offsets.dtype != torch.int64:
+        raise TypeError("offsets must be an int64 tensor of token offsets")
+    if torch.is_tensor(tokens) and offsets.numel():
+        n = tokens.numel()
+        if bool(((offsets < 0) | (offsets > n)).any().item()):
+            raise ValueError(f"offsets must lie in [0, {n}] (token offsets into the {n} ids)")
+    return offsets * _capi.ACB_TOKEN_BYTES
+
+
+def _token_rows(m, cols):
+    """A new tensor: the byte search's rows with their position columns `cols` (a slice) divided by 3.  Floor division
+    keeps the -1 of a row without a match at -1."""
+    out = m.clone()
+    out[:, cols] //= _capi.ACB_TOKEN_BYTES
+    return out
+
+
+class _TokenEncoder:
+    """acb_tokens_encode into one grow-only byte buffer per device.  Callers hold `lock` from the encode until every
+    scan that reads the buffer has been enqueued, then call done(): the next encode waits, on its own stream, for
+    those scans (a query that returns before its scan has finished may still be reading the buffer)."""
+
+    def __init__(self):
+        self.lock = threading.RLock()
+        self._bufs = {}      # device index -> uint8 tensor
+        self._readers = {}   # device index -> CUDA event after the last scan of the buffer
+
+    def encode(self, tokens):
+        """A 1-D uint16 / int32 / int64 CUDA tensor of ids -> a uint8 view of the buffer holding their bytes.  An id
+        outside [0, 2^21) raises ValueError with its index and value (the call waits for the kernel to know)."""
+        torch = _require_cuda()
+        if (not torch.is_tensor(tokens) or tokens.dim() != 1 or tokens.device.type != "cuda" or
+                tokens.dtype not in (torch.uint16, torch.int32, torch.int64)):
+            raise TypeError("tokens must be a 1-D CUDA tensor of uint16, int32 or int64 token ids")
+        tokens = tokens.contiguous()
+        dev = tokens.device
+        idx = dev.index if dev.index is not None else torch.cuda.current_device()
+        n = tokens.numel()
+        nbytes = _capi.ACB_TOKEN_BYTES * n
+        stream = torch.cuda.current_stream(dev)
+        reader = self._readers.get(idx)   # (dropped only once this encode is enqueued behind it)
+        buf = self._bufs.get(idx)
+        if buf is None or buf.numel() < nbytes:
+            if reader is not None:
+                reader.synchronize()   # the old buffer goes back to the allocator: no scan may still read it
+            buf = torch.empty(max(nbytes, 1 << 16), dtype=torch.uint8, device=dev)
+            self._bufs[idx] = buf
+        elif reader is not None:
+            stream.wait_event(reader)
+        bad = torch.full((1,), -1, dtype=torch.int64, device=dev)   # ~0: no bad id
+        with torch.cuda.device(dev):
+            rc = _capi.lib().acb_tokens_encode(tokens.data_ptr(), tokens.element_size(), n, buf.data_ptr(), bad.data_ptr(),
+                                               stream.cuda_stream)
+        if rc != _capi.ACB_OK:
+            raise RuntimeError(_capi.last_error())
+        self._readers.pop(idx, None)
+        j = int(bad.item())
+        if j != -1:
+            raise _token_range_error("tokens", j, int(tokens[j].item()))
+        return buf[:nbytes]
+
+    def done(self, dev):
+        torch = _torch()
+        idx = dev.index if dev.index is not None else torch.cuda.current_device()
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(dev))
+        self._readers[idx] = ev
+
+
+def _token_stream_limits(ac: "_Automaton", n_streams):
+    """The stream limits of StreamBatch, stated in tokens: the seams of one feed (2 x (max_pattern_len - 1) bytes per
+    stream) must fit WINDOW_BYTES.  Arguments StreamBatch refuses on their own are left to it."""
+    if isinstance(n_streams, bool) or not isinstance(n_streams, int) or n_streams < 0:
+        return
+    k = ac.max_pattern_len // _capi.ACB_TOKEN_BYTES
+    seam = 2 * n_streams * max(ac.max_pattern_len - 1, 0)
+    if seam > ac.WINDOW_BYTES:
+        raise ValueError(f"{n_streams} streams x 2 x (3 x {k} - 1) = {seam} seam bytes, with the longest pattern at {k} tokens: one "
+                         f"feed's seams must fit {ac.WINDOW_BYTES} bytes (WINDOW_BYTES); use fewer streams per batch")
+
+
+def _token_feed_limit(ac: "_Automaton", n_tokens: int):
+    limit = ac.WINDOW_BYTES // _capi.ACB_TOKEN_BYTES
+    if n_tokens > limit:
+        raise ValueError(f"one feed addresses at most {limit} tokens (WINDOW_BYTES / 3): feed larger data in more chunks")
+
+
+class TokenStreamBatch:
+    """A StreamBatch or a stream query batch over token ids: feed_device(tokens, offsets, last=None) takes one chunk of
+    ids per stream (a 1-D uint16 / int32 / int64 CUDA tensor, int64 offsets (n_streams + 1) in tokens) and returns
+    what the wrapped batch returns, positions in tokens: (rows (k, 4), row_offsets) for stream_batch, the answers for
+    the query batches."""
+
+    def __init__(self, batch, convert):
+        self._batch = batch
+        self._convert = convert
+        self._enc = _TokenEncoder()
+
+    n_streams = property(lambda self: self._batch.n_streams)
+    overlapping = property(lambda self: self._batch.overlapping)
+    device = property(lambda self: self._batch.device)
+    last_stats = property(lambda self: self._batch.last_stats)
+
+    def feed_device(self, tokens, offsets, last=None):
+        _require_cuda()
+        if _torch().is_tensor(tokens):
+            _token_feed_limit(self._batch._ac, tokens.numel())
+        offsets = _token_offsets(offsets, tokens)
+        # the wrapped feed_device reads the encoded chunk in place and synchronises before it returns (it reads its
+        # row counts), so the next feed may encode into the same buffer
+        with self._enc.lock:
+            data = self._enc.encode(tokens)
+            return self._convert(self._batch.feed_device(data, offsets, last))
+
+
+class TokenStream:
+    """A Stream or a query stream fed host chunks of token ids (1-D integer sequences): feed(chunk) and finish() return
+    what the wrapped stream returns, positions in tokens."""
+
+    def __init__(self, stream, convert):
+        self._stream = stream
+        self._convert = convert
+
+    last_stats = property(lambda self: self._stream.last_stats)
+
+    def feed(self, chunk):
+        data = _encode_host_tokens(chunk, "chunk")
+        _token_feed_limit(self._stream._batch._ac, data.size // _capi.ACB_TOKEN_BYTES)
+        return self._convert(self._stream._feed(data, False))
+
+    def finish(self):
+        return self._convert(self._stream._feed(b"", True))
+
+
+def _same(x):
+    return x
+
+
+def _token_first_answer(row):
+    return (row[0], row[1] // _capi.ACB_TOKEN_BYTES, row[2] // _capi.ACB_TOKEN_BYTES) if row[0] >= 0 else None
+
+
+def _token_tuples(m: np.ndarray):
+    return list(zip(m[:, 1].tolist(), (m[:, 2] // _capi.ACB_TOKEN_BYTES).tolist(), (m[:, 3] // _capi.ACB_TOKEN_BYTES).tolist()))
+
+
+class TokenAhoCorasick:
+    """Search for multiple token-id sequences against token-id sequences: tokenized corpora (uint16 / int32 arrays),
+    generation outputs (int64 tensors).  Positions are token indexes; everything else is BytesAhoCorasick's.
+
+    * ``patterns``: an iterable of non-empty 1-D integer sequences (lists, tuples, numpy arrays, CPU tensors) of ids
+      in [0, 2^21) (ACB_TOKEN_ID_LIMIT).
+    * ``matchkind``, ``implementation``: as for BytesAhoCorasick.
+
+    The ids are encoded into a self-synchronising 3-byte format (include/acb200.h) and searched by the byte engine:
+    host forms encode on the host, device forms with acb_tokens_encode into a grow-only buffer per device.
+    ``max_pattern_len`` is in bytes (3 x the longest pattern's tokens)."""
+
+    def __init__(self, patterns: Iterable, matchkind: MatchKind = MatchKind.Standard,
+                 implementation: Optional[Implementation] = None):
+        if not isinstance(matchkind, MatchKind):
+            raise TypeError("matchkind must be a MatchKind")
+        if implementation is not None and not isinstance(implementation, Implementation):
+            raise TypeError("implementation must be an Implementation or None")
+        encoded = []
+        for i, p in enumerate(iter(patterns)):
+            b = _encode_host_tokens(p, f"pattern {i}")
+            if b.size == 0:
+                raise ValueError("You passed in an empty pattern")
+            encoded.append(b.tobytes())
+        self._ac = _Automaton(encoded, matchkind, implementation)
+        self._enc = _TokenEncoder()
+
+    @property
+    def max_pattern_len(self) -> int:
+        return self._ac.max_pattern_len
+
+    @property
+    def last_stats(self):
+        return self._ac.last_stats
+
+    def _hays(self, haystacks):
+        return [_encode_host_tokens(h, f"haystack {i}") for i, h in enumerate(haystacks)]
+
+    def _on_device(self, query, tokens, offsets):
+        """query(data, byte offsets) on the encoded ids of a device batch, the encode buffer guarded until it is read."""
+        torch = _torch()
+        offsets = _token_offsets(offsets, tokens)
+        with self._enc.lock:
+            data = self._enc.encode(tokens)
+            with torch.cuda.device(data.device):
+                out = query(data, offsets)
+                self._enc.done(data.device)
+        return out
+
+    # ---- the match list ----------------------------------------------------------------------------------------------
+    def find_matches_as_indexes(self, haystack, overlapping: bool = False):
+        """-> list of (pattern index, start, end) in token indexes."""
+        hay = _encode_host_tokens(haystack, "haystack")
+        self._ac.check_overlapping(overlapping)
+        m, _ = self._ac.scan_host_batch([hay], overlapping, codepoints=False)
+        return _token_tuples(m)
+
+    def find_matches_as_indexes_batch(self, haystacks: Sequence, overlapping: bool = False):
+        """One list of (pattern, start, end) per haystack, each what ``find_matches_as_indexes`` returns for it."""
+        hays = self._hays(haystacks)
+        self._ac.check_overlapping(overlapping)
+        m, offs = self._ac.scan_host_batch(hays, overlapping, codepoints=False)
+        t = _token_tuples(m)
+        return [t[offs[i]:offs[i + 1]] for i in range(len(hays))]
+
+    def scan_device(self, tokens, offsets, overlapping: bool = False, capacity: Optional[int] = None):
+        """Device-resident batch of ids (1-D uint16 / int32 / int64 CUDA tensor, int64 offsets (n + 1) in tokens) ->
+        (matches, match_offsets, total) as BytesAhoCorasick.scan_device returns them (int32 rows, int64 above
+        WINDOW_BYTES encoded bytes), positions in tokens.  The tensors are the caller's own, not workspace views."""
+        self._ac.check_overlapping(overlapping)
+        torch = _torch()
+
+        def query(data, offs):
+            # the automaton's scan_device returns views of its workspace slot 0: the copies are enqueued under its
+            # lock, and the next scan on that slot (any thread, any stream) waits for them, as first_device's gather
+            with self._ac._lock:
+                m, mo, total = self._ac.scan_device(data, offs, overlapping, codepoints=False, capacity=capacity)
+                out = _token_rows(m, slice(2, 4)), mo.clone(), total
+                ws = self._ac._ws.get((data.device.index, 0))
+                if ws is not None:
+                    reader = torch.cuda.Event()
+                    reader.record(torch.cuda.current_stream(data.device))
+                    ws["reader"] = reader
+            return out
+        return self._on_device(query, tokens, offsets)
+
+    # ---- queries -----------------------------------------------------------------------------------------------------
+    def is_match(self, haystack) -> bool:
+        """Does any pattern occur in `haystack`?  The same for every match kind."""
+        return self._ac.any_host_batch(self._hays([haystack]))[0]
+
+    def is_match_batch(self, haystacks: Sequence) -> list:
+        return self._ac.any_host_batch(self._hays(haystacks))
+
+    def is_match_device(self, tokens, offsets):
+        """Device-resident batch of ids -> bool tensor (n,) (see _Automaton.any_device)."""
+        return self._on_device(lambda d, o: self._ac.any_device(d, o), tokens, offsets)
+
+    def find_first(self, haystack):
+        """-> (pattern index, start, end) in token indexes, or None: ``find_matches_as_indexes(haystack)[0]``."""
+        return self.find_first_batch([haystack])[0]
+
+    def find_first_batch(self, haystacks: Sequence) -> list:
+        rows = self._ac.first_host_batch(self._hays(haystacks), codepoints=False)
+        return [_token_first_answer(r) if r is not None else None for r in rows]
+
+    def find_first_device(self, tokens, offsets):
+        """Device-resident batch of ids -> int64 tensor (n, 3) of (pattern, start, end) in tokens, -1 rows where a
+        haystack has no match (see _Automaton.first_device)."""
+        return self._on_device(lambda d, o: _token_rows(self._ac.first_device(d, o), slice(1, 3)), tokens, offsets)
+
+    def count_matches(self, haystack, overlapping: bool = False) -> int:
+        """-> ``len(find_matches_as_indexes(haystack, overlapping))``, counted without building the list."""
+        return self.count_matches_batch([haystack], overlapping)[0]
+
+    def count_matches_batch(self, haystacks: Sequence, overlapping: bool = False) -> list:
+        hays = self._hays(haystacks)
+        self._ac.check_overlapping(overlapping)
+        return self._ac.count_host_batch(hays, overlapping)
+
+    def count_matches_device(self, tokens, offsets, overlapping: bool = False):
+        """Device-resident batch of ids -> int64 tensor (n,) of match counts (see _Automaton.count_device)."""
+        self._ac.check_overlapping(overlapping)
+        return self._on_device(lambda d, o: self._ac.count_device(d, o, overlapping), tokens, offsets)
+
+    def count_matches_by_pattern(self, haystack, overlapping: bool = False) -> list:
+        """-> entry i is how many of ``find_matches_as_indexes(haystack, overlapping)`` have pattern i."""
+        return self.count_matches_by_pattern_batch([haystack], overlapping)
+
+    def count_matches_by_pattern_batch(self, haystacks: Sequence, overlapping: bool = False) -> list:
+        hays = self._hays(haystacks)
+        self._ac.check_overlapping(overlapping)
+        return self._ac.pattern_counts_host_batch(hays, overlapping)
+
+    def count_matches_by_pattern_device(self, tokens, offsets, overlapping: bool = False):
+        """Device-resident batch of ids -> int64 tensor (n_patterns,) (see _Automaton.pattern_counts_device)."""
+        self._ac.check_overlapping(overlapping)
+        return self._on_device(lambda d, o: self._ac.pattern_counts_device(d, o, overlapping), tokens, offsets)
+
+    def matching_patterns(self, haystack, overlapping: bool = False) -> list:
+        """-> the distinct pattern ids of ``find_matches_as_indexes(haystack, overlapping)``, ascending."""
+        return self.matching_patterns_batch([haystack], overlapping)[0]
+
+    def matching_patterns_batch(self, haystacks: Sequence, overlapping: bool = False) -> list:
+        hays = self._hays(haystacks)
+        self._ac.check_overlapping(overlapping)
+        return self._ac.hits_host_batch(hays, overlapping)
+
+    def matching_patterns_device(self, tokens, offsets, overlapping: bool = False):
+        """Device-resident batch of ids -> (row_offsets, patterns, counts) (see _Automaton.hits_device)."""
+        self._ac.check_overlapping(overlapping)
+        return self._on_device(lambda d, o: self._ac.hits_device(d, o, overlapping), tokens, offsets)
+
+    # ---- streams: ids fed in chunks ----------------------------------------------------------------------------------
+    def stream(self, overlapping: bool = False) -> TokenStream:
+        """One stream fed host chunks of ids: ``feed(chunk)`` returns the rows (pattern, start, end) it releases, in
+        tokens of the whole stream; ``finish()`` returns the rest (see StreamBatch)."""
+        self._ac.check_overlapping(overlapping)
+        _token_stream_limits(self._ac, 1)
+        return TokenStream(Stream(self._ac, overlapping, codepoints=False), _token_tuples_of_rows)
+
+    def stream_batch(self, n_streams: int, overlapping: bool = False) -> TokenStreamBatch:
+        """``n_streams`` streams fed from the device: ``feed_device(tokens, offsets, last=None)`` -> (rows (k, 4) int64,
+        row_offsets), positions in tokens (see StreamBatch)."""
+        _token_stream_limits(self._ac, n_streams)
+        return TokenStreamBatch(StreamBatch(self._ac, n_streams, overlapping, codepoints=False),
+                                lambda r: (_token_rows(r[0], slice(2, 4)), r[1]))
+
+    def _query_batch(self, kind, n_streams, overlapping):
+        _token_stream_limits(self._ac, n_streams)
+        convert = (lambda rows: _token_rows(rows, slice(1, 3))) if kind == "find_first" else _same
+        return TokenStreamBatch(_query_stream_batch(self._ac, kind, n_streams, overlapping, codepoints=False), convert)
+
+    def _query_stream(self, kind, overlapping):
+        _token_stream_limits(self._ac, 1)
+        answer = {"is_match": bool, "find_first": _token_first_answer, "count": int}[kind]
+        return TokenStream(QueryStream(_query_stream_batch(self._ac, kind, 1, overlapping, codepoints=False), answer), _same)
+
+    def is_match_stream_batch(self, n_streams: int) -> TokenStreamBatch:
+        """``feed_device`` -> bool CUDA tensor (n,), is_match of each stream so far (see IsMatchStreamBatch)."""
+        return self._query_batch("is_match", n_streams, False)
+
+    def find_first_stream_batch(self, n_streams: int) -> TokenStreamBatch:
+        """``feed_device`` -> int64 CUDA tensor (n, 3), each stream's first match in tokens once final, -1 rows while
+        unknown (see FindFirstStreamBatch)."""
+        return self._query_batch("find_first", n_streams, False)
+
+    def count_matches_stream_batch(self, n_streams: int, overlapping: bool = False) -> TokenStreamBatch:
+        """``feed_device`` -> int64 CUDA tensor (n,), the matches each stream's search has released (see CountStreamBatch)."""
+        return self._query_batch("count", n_streams, overlapping)
+
+    def is_match_stream(self) -> TokenStream:
+        return self._query_stream("is_match", False)
+
+    def find_first_stream(self) -> TokenStream:
+        return self._query_stream("find_first", False)
+
+    def count_matches_stream(self, overlapping: bool = False) -> TokenStream:
+        self._ac.check_overlapping(overlapping)
+        return self._query_stream("count", overlapping)
+
+
+def _token_tuples_of_rows(rows):
+    return [(p, s // _capi.ACB_TOKEN_BYTES, e // _capi.ACB_TOKEN_BYTES) for p, s, e in rows]

@@ -538,6 +538,27 @@ int acb_stream_count(const acb_automaton *a, const uint8_t *dev_bytes, const int
                      int64_t *dev_scratch, uint64_t scratch_words, void *stream);
 
 /*
+ * Token ids: a byte format that makes a search over token-id sequences an exact byte search (csrc/tokens.cuh).  Id t,
+ * 0 <= t < ACB_TOKEN_ID_LIMIT, becomes ACB_TOKEN_BYTES bytes: 0x80 | (t >> 14), (t >> 7) & 0x7f, t & 0x7f.  Only a
+ * token's first byte has its high bit set, so every occurrence of an encoded pattern in an encoded haystack starts and
+ * ends on a token boundary: the byte search's rows, divided by ACB_TOKEN_BYTES, are the token search's, for every
+ * match kind, overlapping or not, and for every query and stream form.
+ *
+ * acb_tokens_encode writes ACB_TOKEN_BYTES * n_tokens bytes to dev_out from the ids at dev_tokens: token_bytes = 2
+ * (uint16), 4 (int32) or 8 (int64).  dev_bad = u64, which the caller presets to ~0: an id outside [0, 2^21) lowers
+ * it, with atomicMin, to that id's index, so after the call it holds the smallest bad index (or still ~0); the bytes of
+ * a bad id are undefined.  One launch (none for n_tokens == 0); 16-byte loads and 32-bit stores when dev_tokens is
+ * 16-byte aligned and dev_out 4-byte aligned, one id at a time otherwise.  No synchronisation.
+ * acb_tokens_encode_host is the same on host memory (host_bad preset by the caller too), on the calling thread.
+ * Both return ACB_EINVAL, before any CUDA call, for a token_bytes other than 2, 4 or 8, n_tokens >= 2^60 or a null
+ * pointer (the ids and the output may be null when n_tokens == 0).
+ */
+#define ACB_TOKEN_ID_LIMIT (1u << 21)
+#define ACB_TOKEN_BYTES 3
+int acb_tokens_encode(const void *dev_tokens, int token_bytes, uint64_t n_tokens, uint8_t *dev_out, uint64_t *dev_bad, void *stream);
+int acb_tokens_encode_host(const void *host_tokens, int token_bytes, uint64_t n_tokens, uint8_t *host_out, uint64_t *host_bad);
+
+/*
  * Multi-GPU: the fixed-size block a rank contributes to the gather of the per-shard match lists (the only exchange
  * of the sharded path; NCCL all-gather over NVLink).  dev_block holds (cap + 1) records of 16 bytes: record 0 =
  * (match count, hay_base, complete flag, 0), then the first `cap` matches of a finished scan (dev_total / dev_out of
