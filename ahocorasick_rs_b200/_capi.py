@@ -50,6 +50,11 @@ class HotDesc(C.Structure):
 _lib = None
 
 
+class PatternFilter(C.Structure):
+    """acb_pattern_filter: each haystack's pattern set (a packed bitset row per set, a set index per haystack)."""
+    _fields_ = [("dev_set_bits", C.c_void_p), ("n_sets", C.c_uint64), ("dev_set_index", C.c_void_p), ("index_bytes", C.c_int)]
+
+
 def lib():
     """The loaded library.  Fails loudly when it has not been built: there is no
     CPU fallback behind the matcher classes."""
@@ -125,6 +130,14 @@ def lib():
         L.acb_pack_gather_block.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p, C.c_void_p]
         L.acb_scan_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(HotDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                      C.c_uint64, C.c_int, C.c_int, C.POINTER(Plan), C.POINTER(Workspace), C.c_void_p]
+        F = C.POINTER(PatternFilter)
+        L.acb_scan_batch_filtered.argtypes = L.acb_scan_batch.argtypes[:-1] + [F, C.c_void_p]
+        L.acb_any_match_filtered.argtypes = L.acb_any_match.argtypes[:-1] + [F, C.c_void_p]
+        L.acb_find_first_filtered.argtypes = L.acb_find_first.argtypes[:-1] + [F, C.c_void_p]
+        L.acb_first_rows_filtered.argtypes = L.acb_first_rows.argtypes[:-1] + [F, C.c_void_p]
+        L.acb_count_overlapping_filtered.argtypes = L.acb_count_overlapping.argtypes[:-1] + [F, C.c_void_p]
+        L.acb_count_non_overlapping_filtered.argtypes = L.acb_count_non_overlapping.argtypes[:-1] + [F, C.c_void_p]
+        L.acb_stream_first_resolve_filtered.argtypes = L.acb_stream_first_resolve.argtypes[:-1] + [F, C.c_void_p]
         _lib = L
     return _lib
 
@@ -161,4 +174,6 @@ EXPORTS = [
     "acb_pattern_counts_overlapping", "acb_pattern_counts_non_overlapping", "acb_pattern_hits",
     "acb_pattern_hit_row_words", "acb_stream_advance", "acb_stream_first_resolve", "acb_stream_count",
     "acb_tokens_encode", "acb_tokens_encode_host",
+    "acb_scan_batch_filtered", "acb_any_match_filtered", "acb_find_first_filtered", "acb_first_rows_filtered",
+    "acb_count_overlapping_filtered", "acb_count_non_overlapping_filtered", "acb_stream_first_resolve_filtered",
 ]

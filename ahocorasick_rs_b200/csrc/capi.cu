@@ -1335,9 +1335,12 @@ __global__ void select_rows_kernel(const long long *rows, unsigned long long n, 
 // acb_first_rows: first-match keys (scan_sieve.cuh, FIRST) -> int64 rows (pattern, start, end), one thread per
 // haystack.  LeftmostFirst keys name (start, pattern): the end is start + the pattern's length.  The other two kinds
 // name (start, end): the pattern is the lowest pid of the reverse-trie node of those bytes -- the node stage 2 found --
-// reached by the same walk (hash of the W bytes before the end, then one child per byte towards the start).
+// reached by the same walk (hash of the W bytes before the end, then one child per byte towards the start).  With
+// pattern sets (first_rows_filtered_kernel) the pattern is that node's lowest pid the haystack's set admits.
 // ---------------------------------------------------------------------------
-__device__ uint32_t sieve_pid_of(const DevSieve &sv, const uint8_t *hay, uint32_t start, uint32_t end) {
+// FILT: the lowest pid of the node that `row` admits (see SieveFilter)
+template <bool FILT>
+__device__ __forceinline__ uint32_t sieve_pid_in(const DevSieve &sv, const uint8_t *hay, uint32_t start, uint32_t end, const uint32_t *row) {
     uint32_t lo = 0, hi = 0;  // the 8 bytes ending at end, little endian (the byte at end - 1 is the top byte of lo)
     for (uint32_t k = 1; k <= 8 && k <= end - start; k++) {
         const uint32_t b = hay[end - k];
@@ -1372,7 +1375,16 @@ __device__ uint32_t sieve_pid_of(const DevSieve &sv, const uint8_t *hay, uint32_
         v = l0 < nk && (sv.na[first + l0].meta & 0xffu) == b ? first + l0 : kSieveNoNode;
     }
     if (v == kSieveNoNode || sv.nb[v].own_cnt == 0) return 0xffffffffu;  // (a key always names a pattern)
+    if (FILT) {
+        for (uint32_t t = 0; t < sv.nb[v].own_cnt; t++)
+            if (filter_admits(row, sv.pids[sv.nb[v].own_off + t])) return sv.pids[sv.nb[v].own_off + t];
+        return 0xffffffffu;
+    }
     return sv.pids[sv.nb[v].own_off];  // ascending: the lowest index among patterns with these bytes
+}
+
+__device__ uint32_t sieve_pid_of(const DevSieve &sv, const uint8_t *hay, uint32_t start, uint32_t end) {
+    return sieve_pid_in<false>(sv, hay, start, end, nullptr);
 }
 
 __global__ void first_rows_kernel(DevSieve sv, const uint32_t *pat_len, Batch B, const unsigned long long *keys, long long *rows, int kind) {
@@ -1389,6 +1401,32 @@ __global__ void first_rows_kernel(DevSieve sv, const uint32_t *pat_len, Batch B,
                 end = kind == ACB_STANDARD ? hi : 0xffffffffu - lo;
                 start = kind == ACB_STANDARD ? end - (0xffffffffu - lo) : hi;
                 const uint32_t p = sieve_pid_of(sv, B.bytes + B.offsets[h], (uint32_t)start, (uint32_t)end);
+                pid = p == 0xffffffffu ? -1 : (long long)p;
+            }
+        }
+        rows[3 * h] = pid;
+        rows[3 * h + 1] = start;
+        rows[3 * h + 2] = end;
+    }
+}
+
+// acb_first_rows with pattern sets: LeftmostFirst keys already name an admitted pattern; the other kinds take the
+// node's lowest admitted pid
+__global__ void first_rows_filtered_kernel(DevSieve sv, const uint32_t *pat_len, Batch B, const unsigned long long *keys, long long *rows, int kind,
+                                           SieveFilter F) {
+    for (int64_t h = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; h < B.n_haystacks; h += (int64_t)gridDim.x * blockDim.x) {
+        const unsigned long long key = keys[h];
+        long long pid = -1, start = -1, end = -1;
+        if (key != ~0ull) {
+            const uint32_t hi = (uint32_t)(key >> 32), lo = (uint32_t)key;
+            if (kind == ACB_LEFTMOST_FIRST) {
+                start = hi;
+                pid = lo;
+                end = start + pat_len[lo];
+            } else {
+                end = kind == ACB_STANDARD ? hi : 0xffffffffu - lo;
+                start = kind == ACB_STANDARD ? end - (0xffffffffu - lo) : hi;
+                const uint32_t p = sieve_pid_in<true>(sv, B.bytes + B.offsets[h], (uint32_t)start, (uint32_t)end, filter_row(F, h));
                 pid = p == 0xffffffffu ? -1 : (long long)p;
             }
         }
@@ -2432,18 +2470,27 @@ DevSieve make_sieve_view(const SieveHeader &h, const void *dev_sieve) {
 
 // MODE kSieveAny (acb_any_match) / kSieveFirst + kind (acb_find_first): hay_cont carries the flags / keys and task_cont
 // the two skip counters, out goes unused
+// F: each haystack's pattern set (sieve_scan_filtered_kernel), or null
 template <bool CP, int MODE = kSieveList>
 int launch_sieve(const DevSieve &sv, const Batch &B, SievePlan &P, const Sink &out, uint32_t *task_cont, uint32_t *hay_cont,
-                 unsigned int *task_counter, const DeviceInfo &d, cudaStream_t st) {
+                 unsigned int *task_counter, const DeviceInfo &d, cudaStream_t st, const SieveFilter *F = nullptr) {
     const uint32_t ring = acb_sieve_ring(sv.bloom_words * 4, (uint32_t)d.max_smem_optin);
     if (ring == 0) return fail(ACB_ECUDA, "the sieve's filters do not fit in shared memory (rebuild them with a smaller bloom_bytes_max)");
     const uint32_t smem = sieve_smem_bytes(sv.bloom_words * 4, ring, CP);
     P.ring = ring;
-#define ACB_SIEVE_GO(WC)                                                                                  \
-    do {                                                                                                  \
-        auto kern = sieve_scan_kernel<CP, WC, MODE>;                                                      \
-        CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, d.max_smem_optin)); \
-        kern<<<d.sms, kSieveThreads, smem, st>>>(sv, B, P, out, task_cont, hay_cont, task_counter);       \
+#define ACB_SIEVE_GO(WC)                                                                                      \
+    do {                                                                                                      \
+        if constexpr (MODE != kSievePatterns) {                                                               \
+            if (F) {                                                                                          \
+                auto kern = sieve_scan_filtered_kernel<CP, WC, MODE>;                                         \
+                CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, d.max_smem_optin)); \
+                kern<<<d.sms, kSieveThreads, smem, st>>>(sv, B, P, out, task_cont, hay_cont, task_counter, *F); \
+                break;                                                                                        \
+            }                                                                                                 \
+        }                                                                                                     \
+        auto kern = sieve_scan_kernel<CP, WC, MODE>;                                                          \
+        CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, d.max_smem_optin));   \
+        kern<<<d.sms, kSieveThreads, smem, st>>>(sv, B, P, out, task_cont, hay_cont, task_counter);           \
     } while (0)
     if (sv.W < 4)
         ACB_SIEVE_GO(0);
@@ -2533,14 +2580,35 @@ int unsupported_overlapping(const acb_automaton *a) {
                                       " does not support overlapping searches");
 }
 
+// acb_pattern_filter -> the kernels' view; ACB_EINVAL (before any device work) for a malformed descriptor.  A null
+// descriptor is no filter (*out stays unset, *use false).
+int filter_view(const acb_automaton *a, const acb_pattern_filter *f, int64_t n_haystacks, SieveFilter &out, bool &use) {
+    use = f != nullptr;
+    if (!f) return ACB_OK;
+    if (f->n_sets == 0) return fail(ACB_EINVAL, "pattern filter: n_sets must be at least 1");
+    if (!f->dev_set_bits) return fail(ACB_EINVAL, "pattern filter: null dev_set_bits");
+    if (f->index_bytes != 4 && f->index_bytes != 8) return fail(ACB_EINVAL, "pattern filter: index_bytes must be 4 or 8");
+    if (!f->dev_set_index && n_haystacks > 0) return fail(ACB_EINVAL, "pattern filter: null dev_set_index");
+    out.bits = f->dev_set_bits;
+    out.index = f->dev_set_index;
+    out.n_sets = f->n_sets;
+    out.words = (uint32_t)((a->impl->hdr.n_patterns + 31) / 32);
+    out.index_bytes = (uint32_t)f->index_bytes;
+    return ACB_OK;
+}
+
 // acb_any_match (mode kSieveAny, out = u8 flags), acb_find_first (kSieveFirst + kind, out = u64 keys),
 // acb_count_overlapping (kSieveCount, out = u64 counts per haystack) and acb_pattern_counts_overlapping (kSievePatterns,
 // out = u64 counts per pattern): one launch of the sieve kernel in a mode that writes no list
 int sieve_early_scan(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
-                     int64_t n_haystacks, uint64_t total_bytes, void *dev_out, uint64_t *dev_scratch, void *stream, int mode) {
+                     int64_t n_haystacks, uint64_t total_bytes, void *dev_out, uint64_t *dev_scratch, void *stream, int mode,
+                     const acb_pattern_filter *filter = nullptr) {
     if (!a || !dev_sieve || !dev_offsets || !dev_out || !dev_scratch || (total_bytes && !dev_bytes)) return fail(ACB_EINVAL, "null argument");
     if (n_haystacks < 0 || n_haystacks > 0xfffffffell) return fail(ACB_EINVAL, "n_haystacks out of range (0 .. 2^32 - 2)");
     if (total_bytes >= (1ull << 31)) return fail(ACB_EINVAL, "total_bytes must be below 2^31 (scan larger inputs in windows)");
+    SieveFilter F;
+    bool filtered;
+    if (int rc = filter_view(a, filter, n_haystacks, F, filtered)) return rc;
     if ((mode == kSieveCount || mode == kSievePatterns) && a->impl->hdr.match_kind != ACB_STANDARD) return unsupported_overlapping(a);
     SieveHeader sh;
     if (int rc = sieve_header(a, sh)) return rc;
@@ -2565,12 +2633,13 @@ int sieve_early_scan(const acb_automaton *a, const void *dev_sieve, const uint8_
     uint32_t *skipped = reinterpret_cast<uint32_t *>(scr + 1), *out = static_cast<uint32_t *>(dev_out);
     unsigned int *counter = reinterpret_cast<unsigned int *>(scr);
     int rc;
+    const SieveFilter *Fp = filtered ? &F : nullptr;
     switch (mode) {
-        case kSieveAny: rc = launch_sieve<false, kSieveAny>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
-        case kSieveFirst + ACB_STANDARD: rc = launch_sieve<false, kSieveFirst + ACB_STANDARD>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
-        case kSieveFirst + ACB_LEFTMOST_FIRST: rc = launch_sieve<false, kSieveFirst + ACB_LEFTMOST_FIRST>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
-        case kSieveFirst + ACB_LEFTMOST_LONGEST: rc = launch_sieve<false, kSieveFirst + ACB_LEFTMOST_LONGEST>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
-        case kSieveCount: rc = launch_sieve<false, kSieveCount>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
+        case kSieveAny: rc = launch_sieve<false, kSieveAny>(sv, B, SP, Sink{}, skipped, out, counter, d, st, Fp); break;
+        case kSieveFirst + ACB_STANDARD: rc = launch_sieve<false, kSieveFirst + ACB_STANDARD>(sv, B, SP, Sink{}, skipped, out, counter, d, st, Fp); break;
+        case kSieveFirst + ACB_LEFTMOST_FIRST: rc = launch_sieve<false, kSieveFirst + ACB_LEFTMOST_FIRST>(sv, B, SP, Sink{}, skipped, out, counter, d, st, Fp); break;
+        case kSieveFirst + ACB_LEFTMOST_LONGEST: rc = launch_sieve<false, kSieveFirst + ACB_LEFTMOST_LONGEST>(sv, B, SP, Sink{}, skipped, out, counter, d, st, Fp); break;
+        case kSieveCount: rc = launch_sieve<false, kSieveCount>(sv, B, SP, Sink{}, skipped, out, counter, d, st, Fp); break;
         case kSievePatterns: rc = launch_sieve<false, kSievePatterns>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
         default: return fail(ACB_EINVAL, "unknown match kind");
     }
@@ -2594,7 +2663,7 @@ int check_ws(const acb_workspace *ws) {
 // dev_raw and are ordered into dev_out, so that dev_raw is free for the pairs.
 int sieve_list_scan(const acb_automaton *a, const void *dev_sieve, const Batch &B, uint64_t total_bytes, int mode, bool cp,
                     const uint32_t *pat_cplen, const acb_plan *plan, const acb_workspace *ws, const DeviceInfo &d, cudaStream_t st,
-                    unsigned long long *counts, bool by_pattern = false, const HitRows *hits = nullptr) {
+                    unsigned long long *counts, bool by_pattern = false, const HitRows *hits = nullptr, const SieveFilter *F = nullptr) {
     const ImageHeader &h = a->impl->hdr;
     const int kind = (int)h.match_kind;
     const uint8_t *dev_bytes = B.bytes;
@@ -2643,8 +2712,8 @@ int sieve_list_scan(const acb_automaton *a, const void *dev_sieve, const Batch &
     // code points: the continuation bytes each task saw before a haystack that starts in it, per haystack; lives in
     // the match_offsets buffer until the epilogue's last phases write the offsets there
     uint32_t *hay_cont = reinterpret_cast<uint32_t *>(match_offsets);
-    rc = cp ? launch_sieve<true>(sv, B, SP, out, cont_tail, hay_cont, task_counter, d, st)
-            : launch_sieve<false>(sv, B, SP, out, cont_tail, hay_cont, task_counter, d, st);
+    rc = cp ? launch_sieve<true>(sv, B, SP, out, cont_tail, hay_cont, task_counter, d, st, F)
+            : launch_sieve<false>(sv, B, SP, out, cont_tail, hay_cont, task_counter, d, st, F);
     if (rc) return rc;
     CUDA_OK(cudaGetLastError());
     if (e1) {
@@ -2698,10 +2767,14 @@ int sieve_list_scan(const acb_automaton *a, const void *dev_sieve, const Batch &
 // (by_pattern: counts per pattern, added to) and acb_pattern_hits (hits, dev_counts unused; either search)
 int non_overlapping_counts(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
                            int64_t n_haystacks, uint64_t total_bytes, const acb_plan *plan, const acb_workspace *ws,
-                           uint64_t *dev_counts, void *stream, bool by_pattern, const HitRows *hits = nullptr, bool overlapping = false) {
+                           uint64_t *dev_counts, void *stream, bool by_pattern, const HitRows *hits = nullptr, bool overlapping = false,
+                           const acb_pattern_filter *filter = nullptr) {
     if (!a || !dev_sieve || !dev_offsets || !plan || (!dev_counts && !hits) || (total_bytes && !dev_bytes)) return fail(ACB_EINVAL, "null argument");
     if (int rc = check_ws(ws)) return rc;
     if (n_haystacks < 0 || n_haystacks > 0xfffffffell) return fail(ACB_EINVAL, "n_haystacks out of range (0 .. 2^32 - 2)");
+    SieveFilter F;
+    bool filtered;
+    if (int rc = filter_view(a, filter, n_haystacks, F, filtered)) return rc;
     if (total_bytes >= (1ull << 31)) return fail(ACB_EINVAL, "total_bytes must be below 2^31 (scan larger inputs in windows)");
     if (overlapping && a->impl->hdr.match_kind != ACB_STANDARD) return unsupported_overlapping(a);
     acb_plan want;
@@ -2725,7 +2798,7 @@ int non_overlapping_counts(const acb_automaton *a, const void *dev_sieve, const 
     }
     const int mode = overlapping ? kModeOverlap : a->impl->hdr.match_kind == ACB_STANDARD ? kModeStandard : kModeLeftmost;
     return sieve_list_scan(a, dev_sieve, Batch{dev_bytes, dev_offsets, n_haystacks}, total_bytes, mode, false, nullptr, plan, ws, d, st,
-                           reinterpret_cast<unsigned long long *>(dev_counts), by_pattern, hits);
+                           reinterpret_cast<unsigned long long *>(dev_counts), by_pattern, hits, filtered ? &F : nullptr);
 }
 
 }  // namespace
@@ -2764,30 +2837,55 @@ int acb_select_non_overlapping(const acb_automaton *a, const int64_t *dev_rows, 
     return ACB_OK;
 }
 
+int acb_any_match_filtered(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                           int64_t n_haystacks, uint64_t total_bytes, uint8_t *dev_flags, uint64_t *dev_scratch,
+                           const acb_pattern_filter *filter, void *stream) {
+    if (!dev_flags) return fail(ACB_EINVAL, "null argument");
+    return sieve_early_scan(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, dev_flags, dev_scratch, stream, kSieveAny, filter);
+}
+
 int acb_any_match(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
                   int64_t n_haystacks, uint64_t total_bytes, uint8_t *dev_flags, uint64_t *dev_scratch, void *stream) {
-    if (!dev_flags) return fail(ACB_EINVAL, "null argument");
-    return sieve_early_scan(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, dev_flags, dev_scratch, stream, kSieveAny);
+    return acb_any_match_filtered(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, dev_flags, dev_scratch, nullptr, stream);
+}
+
+int acb_find_first_filtered(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                            int64_t n_haystacks, uint64_t total_bytes, uint64_t *dev_keys, uint64_t *dev_scratch,
+                            const acb_pattern_filter *filter, void *stream) {
+    if (!dev_keys) return fail(ACB_EINVAL, "null argument");
+    if (!a) return fail(ACB_EINVAL, "null argument");
+    return sieve_early_scan(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, dev_keys, dev_scratch, stream,
+                            kSieveFirst + (int)a->impl->hdr.match_kind, filter);
 }
 
 int acb_find_first(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
                    int64_t n_haystacks, uint64_t total_bytes, uint64_t *dev_keys, uint64_t *dev_scratch, void *stream) {
-    if (!dev_keys) return fail(ACB_EINVAL, "null argument");
-    if (!a) return fail(ACB_EINVAL, "null argument");
-    return sieve_early_scan(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, dev_keys, dev_scratch, stream,
-                            kSieveFirst + (int)a->impl->hdr.match_kind);
+    return acb_find_first_filtered(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, dev_keys, dev_scratch, nullptr, stream);
+}
+
+int acb_count_overlapping_filtered(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                                   int64_t n_haystacks, uint64_t total_bytes, uint64_t *dev_counts, uint64_t *dev_scratch,
+                                   const acb_pattern_filter *filter, void *stream) {
+    if (!dev_counts) return fail(ACB_EINVAL, "null argument");
+    return sieve_early_scan(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, dev_counts, dev_scratch, stream, kSieveCount, filter);
 }
 
 int acb_count_overlapping(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
                           int64_t n_haystacks, uint64_t total_bytes, uint64_t *dev_counts, uint64_t *dev_scratch, void *stream) {
-    if (!dev_counts) return fail(ACB_EINVAL, "null argument");
-    return sieve_early_scan(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, dev_counts, dev_scratch, stream, kSieveCount);
+    return acb_count_overlapping_filtered(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, dev_counts, dev_scratch, nullptr, stream);
+}
+
+int acb_count_non_overlapping_filtered(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                                       int64_t n_haystacks, uint64_t total_bytes, const acb_plan *plan, const acb_workspace *ws,
+                                       uint64_t *dev_counts, const acb_pattern_filter *filter, void *stream) {
+    return non_overlapping_counts(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, plan, ws, dev_counts, stream, false, nullptr,
+                                  false, filter);
 }
 
 int acb_count_non_overlapping(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
                               int64_t n_haystacks, uint64_t total_bytes, const acb_plan *plan, const acb_workspace *ws,
                               uint64_t *dev_counts, void *stream) {
-    return non_overlapping_counts(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, plan, ws, dev_counts, stream, false);
+    return acb_count_non_overlapping_filtered(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, plan, ws, dev_counts, nullptr, stream);
 }
 
 int acb_pattern_counts_overlapping(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
@@ -2842,10 +2940,13 @@ int acb_count_rows(const acb_automaton *a, const int64_t *dev_rows, uint64_t n_r
     return ACB_OK;
 }
 
-int acb_first_rows(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
-                   int64_t n_haystacks, const uint64_t *dev_keys, int64_t *dev_rows, void *stream) {
+int acb_first_rows_filtered(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                            int64_t n_haystacks, const uint64_t *dev_keys, int64_t *dev_rows, const acb_pattern_filter *filter, void *stream) {
     if (!a || !dev_sieve || !dev_offsets || !dev_keys || !dev_rows) return fail(ACB_EINVAL, "null argument");
     if (n_haystacks < 0 || n_haystacks > 0xfffffffell) return fail(ACB_EINVAL, "n_haystacks out of range (0 .. 2^32 - 2)");
+    SieveFilter F;
+    bool filtered;
+    if (int rc = filter_view(a, filter, n_haystacks, F, filtered)) return rc;
     SieveHeader sh;
     if (int rc = sieve_header(a, sh)) return rc;
     DeviceInfo d;
@@ -2855,12 +2956,22 @@ int acb_first_rows(const acb_automaton *a, const void *dev_sieve, const uint8_t 
     int64_t blocks = (n_haystacks + 127) / 128;
     if (blocks > 16ll * d.sms) blocks = 16ll * d.sms;  // grid-stride beyond that
     const uint32_t *pat_len = reinterpret_cast<const uint32_t *>(static_cast<const uint8_t *>(dev_sieve) + sh.off_pat_len);
-    first_rows_kernel<<<(unsigned)blocks, 128, 0, st>>>(make_sieve_view(sh, dev_sieve), pat_len, Batch{dev_bytes, dev_offsets, n_haystacks},
-                                                        reinterpret_cast<const unsigned long long *>(dev_keys),
-                                                        reinterpret_cast<long long *>(dev_rows), (int)a->impl->hdr.match_kind);
+    if (filtered)
+        first_rows_filtered_kernel<<<(unsigned)blocks, 128, 0, st>>>(make_sieve_view(sh, dev_sieve), pat_len, Batch{dev_bytes, dev_offsets, n_haystacks},
+                                                                     reinterpret_cast<const unsigned long long *>(dev_keys),
+                                                                     reinterpret_cast<long long *>(dev_rows), (int)a->impl->hdr.match_kind, F);
+    else
+        first_rows_kernel<<<(unsigned)blocks, 128, 0, st>>>(make_sieve_view(sh, dev_sieve), pat_len, Batch{dev_bytes, dev_offsets, n_haystacks},
+                                                            reinterpret_cast<const unsigned long long *>(dev_keys),
+                                                            reinterpret_cast<long long *>(dev_rows), (int)a->impl->hdr.match_kind);
     g_launches++;
     CUDA_OK(cudaGetLastError());
     return ACB_OK;
+}
+
+int acb_first_rows(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                   int64_t n_haystacks, const uint64_t *dev_keys, int64_t *dev_rows, void *stream) {
+    return acb_first_rows_filtered(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, dev_keys, dev_rows, nullptr, stream);
 }
 
 int acb_rows_to_codepoints(const uint8_t *dev_bytes, const int64_t *dev_offsets, int64_t n_haystacks, uint64_t total_bytes,
@@ -2948,11 +3059,17 @@ int acb_pack_gather_block(const uint64_t *dev_total, const acb_match *dev_out, u
     return ACB_OK;
 }
 
-int acb_scan_batch(const acb_automaton *a, const void *dev_image, const void *dev_hot, const acb_hot_desc *hot_desc,
-                   const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets, int64_t n_haystacks, uint64_t total_bytes,
-                   int overlapping, int codepoints, const acb_plan *plan, const acb_workspace *ws, void *stream) {
+int acb_scan_batch_filtered(const acb_automaton *a, const void *dev_image, const void *dev_hot, const acb_hot_desc *hot_desc,
+                            const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets, int64_t n_haystacks,
+                            uint64_t total_bytes, int overlapping, int codepoints, const acb_plan *plan, const acb_workspace *ws,
+                            const acb_pattern_filter *filter, void *stream) {
     if (!a || !dev_image || !dev_offsets || n_haystacks < 0 || !plan) return fail(ACB_EINVAL, "bad argument");
     if (n_haystacks > 0xfffffffell) return fail(ACB_EINVAL, "too many haystacks in one batch");
+    SieveFilter F;
+    bool filtered;
+    if (int rc = filter_view(a, filter, n_haystacks, F, filtered)) return rc;
+    // the table images hold every pattern: a filtered scan always runs the sieve
+    if (filtered && !dev_sieve) return fail(ACB_EINVAL, "a scan with pattern sets needs the sieve image");
     const ImageHeader &h = a->impl->hdr;
     const int kind = (int)h.match_kind;
     // overlapping == 2: the overlapping LIST, for any match kind -- the input of acb_select_non_overlapping; sieve only
@@ -3000,12 +3117,14 @@ int acb_scan_batch(const acb_automaton *a, const void *dev_image, const void *de
 
     int kernel = g_tuning.kernel;
     if (kernel == 0) kernel = dev_sieve ? 5 : 2;  // the caller uploads a sieve image when it wants the position-parallel scan
-    if (overlapping == 2) kernel = 5;
+    if (overlapping == 2 || filtered) kernel = 5;
     // the caller's profile says the hot rows do not cover this data: scan from the image in global memory / L2
     if (kernel == 2 && g_tuning.kernel == 0 && hot_desc && (hot_desc->reserved & 1u)) kernel = 4;
     if (kernel == 5 && !dev_sieve) return fail(ACB_EINVAL, "the sieve kernel needs a sieve image (acb_sieve_build / acb_sieve_write)");
     if ((!dev_hot || !hot_desc) && kernel != 4 && kernel != 5) kernel = 1;  // no hot image: the plain kernel (one thread per haystack)
-    if (kernel == 5) return sieve_list_scan(a, dev_sieve, B, total_bytes, mode, cp, im.pat_cplen, plan, ws, d, st, nullptr);
+    if (kernel == 5)
+        return sieve_list_scan(a, dev_sieve, B, total_bytes, mode, cp, im.pat_cplen, plan, ws, d, st, nullptr, false, nullptr,
+                               filtered ? &F : nullptr);
     const bool segments = kernel == 2 || kernel == 3 || kernel == 4;
     const int per_lane = kernel == 3 ? 2 : 1;  // segments per lane of the staged kernel (3: two interleaved chains)
     SegPlan P{};
@@ -3116,6 +3235,13 @@ int acb_scan_batch(const acb_automaton *a, const void *dev_image, const void *de
     if (rc) return rc;
     CUDA_OK(cudaGetLastError());
     return ACB_OK;
+}
+
+int acb_scan_batch(const acb_automaton *a, const void *dev_image, const void *dev_hot, const acb_hot_desc *hot_desc,
+                   const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets, int64_t n_haystacks, uint64_t total_bytes,
+                   int overlapping, int codepoints, const acb_plan *plan, const acb_workspace *ws, void *stream) {
+    return acb_scan_batch_filtered(a, dev_image, dev_hot, hot_desc, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, overlapping,
+                                   codepoints, plan, ws, nullptr, stream);
 }
 
 int acb_stream_seams(const acb_automaton *a, const uint8_t *dev_bytes, const int64_t *dev_offsets, int64_t n_streams, uint64_t total_bytes,
@@ -3265,15 +3391,20 @@ int acb_stream_advance(const acb_automaton *a, const uint8_t *dev_bytes, const i
     return ACB_OK;
 }
 
-int acb_stream_first_resolve(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
-                             int64_t n_streams, uint64_t total_bytes, const uint8_t *dev_last, int codepoints, const int64_t *dev_carry,
-                             const uint8_t *dev_seam_bytes, const int64_t *dev_seam_offsets, uint64_t seam_buffer_bytes,
-                             uint64_t *dev_seam_keys, uint64_t *dev_chunk_keys, int64_t *dev_best, int64_t *dev_scratch, int64_t *dev_rows,
-                             void *stream) {
+int acb_stream_first_resolve_filtered(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                                      int64_t n_streams, uint64_t total_bytes, const uint8_t *dev_last, int codepoints, const int64_t *dev_carry,
+                                      const uint8_t *dev_seam_bytes, const int64_t *dev_seam_offsets, uint64_t seam_buffer_bytes,
+                                      uint64_t *dev_seam_keys, uint64_t *dev_chunk_keys, int64_t *dev_best, int64_t *dev_scratch,
+                                      int64_t *dev_rows, const acb_pattern_filter *filter, void *stream) {
     if (!a || !dev_sieve || !dev_offsets || !dev_carry || !dev_seam_offsets || !dev_seam_keys || !dev_chunk_keys || !dev_best ||
         !dev_scratch || !dev_rows || (total_bytes && !dev_bytes) || (seam_buffer_bytes && !dev_seam_bytes))
         return fail(ACB_EINVAL, "null argument");
     if (n_streams < 0 || n_streams > 0xfffffffell) return fail(ACB_EINVAL, "n_streams out of range (0 .. 2^32 - 2)");
+    {
+        SieveFilter F;
+        bool filtered;
+        if (int rc = filter_view(a, filter, n_streams, F, filtered)) return rc;
+    }
     if (total_bytes >= (1ull << 31) || seam_buffer_bytes >= (1ull << 31))
         return fail(ACB_EINVAL, "total_bytes and seam_buffer_bytes must be below 2^31 (feed larger data in more chunks)");
     SieveHeader sh;
@@ -3308,8 +3439,9 @@ int acb_stream_first_resolve(const acb_automaton *a, const void *dev_sieve, cons
     g_launches++;
     CUDA_OK(cudaGetLastError());
     const Batch seams{dev_seam_bytes, dev_seam_offsets, n};
-    if (int rc = acb_first_rows(a, dev_sieve, seams.bytes, seams.offsets, n, dev_seam_keys, dev_scratch + 2, stream)) return rc;
-    if (int rc = acb_first_rows(a, dev_sieve, dev_bytes, dev_offsets, n, dev_chunk_keys, dev_scratch + 2 + 3 * n, stream)) return rc;
+    if (int rc = acb_first_rows_filtered(a, dev_sieve, seams.bytes, seams.offsets, n, dev_seam_keys, dev_scratch + 2, filter, stream)) return rc;
+    if (int rc = acb_first_rows_filtered(a, dev_sieve, dev_bytes, dev_offsets, n, dev_chunk_keys, dev_scratch + 2 + 3 * n, filter, stream))
+        return rc;
     if (codepoints) {
         if (int rc = acb_rows_to_codepoints(seams.bytes, seams.offsets, n, seam_buffer_bytes, dev_scratch + 2, dev_scratch + 2 + 6 * n, stream))
             return rc;
@@ -3320,6 +3452,16 @@ int acb_stream_first_resolve(const acb_automaton *a, const void *dev_sieve, cons
     g_launches++;
     CUDA_OK(cudaGetLastError());
     return ACB_OK;
+}
+
+int acb_stream_first_resolve(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                             int64_t n_streams, uint64_t total_bytes, const uint8_t *dev_last, int codepoints, const int64_t *dev_carry,
+                             const uint8_t *dev_seam_bytes, const int64_t *dev_seam_offsets, uint64_t seam_buffer_bytes,
+                             uint64_t *dev_seam_keys, uint64_t *dev_chunk_keys, int64_t *dev_best, int64_t *dev_scratch, int64_t *dev_rows,
+                             void *stream) {
+    return acb_stream_first_resolve_filtered(a, dev_sieve, dev_bytes, dev_offsets, n_streams, total_bytes, dev_last, codepoints, dev_carry,
+                                             dev_seam_bytes, dev_seam_offsets, seam_buffer_bytes, dev_seam_keys, dev_chunk_keys, dev_best,
+                                             dev_scratch, dev_rows, nullptr, stream);
 }
 
 int acb_stream_count(const acb_automaton *a, const uint8_t *dev_bytes, const int64_t *dev_offsets, int64_t n_streams, uint64_t total_bytes,

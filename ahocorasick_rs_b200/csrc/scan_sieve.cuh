@@ -184,6 +184,37 @@ __device__ __forceinline__ void add_per_pattern(unsigned long long *counts, uint
     if ((threadIdx.x & 31u) == (uint32_t)__ffs(peers) - 1u) atomicAdd(counts + pid, (unsigned long long)__popc(peers));
 }
 
+// Pattern sets (sieve_scan_filtered_kernel): each haystack h searches only for the pattern ids of ONE set, row
+// index[h] of a packed bitset (n_sets rows of `words` u32, bit p of a row = pattern p is in the set).  A pid is ADMITTED
+// when its bit is set in its haystack's row; an index outside [0, n_sets) admits nothing.  Stage 2 is the only place a
+// pid becomes a result, so the filter sits there alone; the deepest terminal node's chain is walked from the deepest
+// node (longest pattern) down, its pids ascending per node:
+//   LIST   the admitted pids of the chain (cnt = how many: the warp's reservation and the ranks stay dense)
+//   ANY    the flag, when the chain has an admitted pid
+//   FIRST  the deepest node with an admitted pid, and its lowest admitted pid: at one end position that is the smallest
+//          key of every kind (Standard: longest; LeftmostFirst: leftmost start, then lowest index; LeftmostLongest:
+//          leftmost start), exactly as the deepest terminal node is without a filter
+//   COUNT  the number of admitted pids
+// Every key and flag comes from admitted matches only, so the skips ("flag set", "cannot beat the key") stay exact.
+struct SieveFilter {
+    const uint32_t *bits;   // n_sets x words
+    const void *index;      // per haystack: int32 (index_bytes 4) or int64 (8)
+    uint64_t n_sets;
+    uint32_t words;         // ceil(n_patterns / 32)
+    uint32_t index_bytes;
+};
+
+// the bitset row of haystack h's set, or null (an index outside [0, n_sets): nothing is admitted)
+__device__ __forceinline__ const uint32_t *filter_row(const SieveFilter &F, int64_t h) {
+    const int64_t s = F.index_bytes == 4 ? (int64_t)__ldg(static_cast<const int32_t *>(F.index) + h)
+                                         : (int64_t)__ldg(static_cast<const long long *>(F.index) + h);
+    return s >= 0 && (uint64_t)s < F.n_sets ? F.bits + (uint64_t)s * F.words : nullptr;
+}
+
+__device__ __forceinline__ bool filter_admits(const uint32_t *row, uint32_t pid) {
+    return row != nullptr && ((__ldg(row + (pid >> 5)) >> (pid & 31u)) & 1u);
+}
+
 // WC: 0 = W < 4 (the window word is shifted down), 1 = W == 4, 2 = W in 6..8 (two words), 3 = W == 5 (a word and a byte)
 //
 // Positions inside a task are 32-bit offsets from the task's start (`rel`); the 64-bit stream position is t_lo + rel.
@@ -193,9 +224,13 @@ __device__ __forceinline__ void add_per_pattern(unsigned long long *counts, uint
 // hay_cont -> flags = u8[n_haystacks] (any), keys = u64[n_haystacks] (first), counts = u64[n_haystacks] (count) or
 // counts = u64[n_patterns] (patterns), task_cont -> skipped = u64[2] = [tasks skipped whole, windows not scanned] (see
 // acb_any_match, acb_find_first; count, patterns: unused).
-template <bool CP, int WC, int MODE = kSieveList>
-__global__ void __launch_bounds__(kSieveThreads, 1)
-sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_cont, uint32_t *hay_cont, unsigned int *task_counter) {
+//
+// FILT: stage 2 admits only the pids of each haystack's pattern set (see SieveFilter); the kernel body is shared by
+// sieve_scan_kernel (no filter) and sieve_scan_filtered_kernel.
+template <bool CP, int WC, int MODE, bool FILT>
+__device__ __forceinline__ void sieve_scan(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_cont,
+                                           uint32_t *hay_cont, unsigned int *task_counter, SieveFilter F) {
+    static_assert(!(FILT && MODE == kSievePatterns), "the pattern-count mode has no filtered form");
     constexpr bool ANY = MODE == kSieveAny, FIRST = MODE >= kSieveFirst && MODE < kSieveCount, EARLY = ANY || FIRST;  // EARLY: no list, work stops early
     constexpr bool COUNT = MODE == kSieveCount, PATTERNS = MODE == kSievePatterns, LIST = MODE == kSieveList;
     constexpr int KIND = MODE - kSieveFirst;  // (FIRST)
@@ -392,6 +427,7 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
             int32_t hs;
             const int64_t h = hay_of(active ? rel : max(wrel, lo_r), hs);
             uint32_t best = kSieveNoNode, cnt = 0, best_d = 0;  // best_d: the depth of best (FIRST)
+            const uint32_t *frow = nullptr;                      // FILT: haystack h's set (LIST: the records to write)
             if (active && (int32_t)rel - (int32_t)(W - 1) >= hs) {
                 const uint32_t klo = ent2.y, khi = ent2.z;
                 const uint32_t x = klo + khi * kMixHi;
@@ -453,7 +489,45 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
                     na = nc;
                     d++;
                 }
-                if (ANY) {
+                if (FILT) {
+                    // the chain from the deepest terminal node: cnt = its admitted pids; FIRST: the first admitted
+                    // (deepest node, lowest pid) becomes best / best_d / fpid
+                    frow = best != kSieveNoNode ? filter_row(F, h) : nullptr;
+                    const uint32_t *row = frow;
+                    uint32_t fpid = 0;
+                    for (uint32_t u = row ? best : kSieveNoNode; u != kSieveNoNode;) {
+                        const uint4 nb = __ldg(reinterpret_cast<const uint4 *>(sv.nb + u));  // own_off, own_cnt, term_link, depth
+                        for (uint32_t t = 0; t < nb.y; t++) {
+                            const uint32_t pid = __ldg(sv.pids + nb.x + t);
+                            if (!filter_admits(row, pid)) continue;
+                            if (cnt == 0) {
+                                fpid = pid;
+                                best_d = nb.w;
+                            }
+                            cnt++;
+                            if (EARLY) break;
+                        }
+                        if (EARLY && cnt) break;
+                        u = nb.z;
+                    }
+                    if (ANY) {
+                        if (cnt) flags[h] = 1;
+                        cnt = 0;
+                    } else if (FIRST) {
+                        if (cnt) {
+                            const uint32_t end_rel = rel + 1u - (uint32_t)hs, start_rel = end_rel - best_d;
+                            unsigned long long key;
+                            if (KIND == 0)
+                                key = (unsigned long long)end_rel << 32 | (0xffffffffu - best_d);
+                            else if (KIND == 1)
+                                key = (unsigned long long)start_rel << 32 | fpid;
+                            else
+                                key = (unsigned long long)start_rel << 32 | (0xffffffffu - end_rel);
+                            atomicMin(keys + h, key);
+                        }
+                        cnt = 0;
+                    }
+                } else if (ANY) {
                     if (best != kSieveNoNode) flags[h] = 1;  // a pattern ends here, inside haystack h
                 } else if (FIRST) {
                     if (best != kSieveNoNode) {  // the best match ending here: the deepest terminal node, its lowest pid
@@ -503,6 +577,24 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
                     unsigned long long idx = rbase + exc;
                     uint32_t seq = n_emitted + exc;
                     const uint32_t end_rel = (uint32_t)((int32_t)rel + 1 - hs);
+                    if (FILT) {
+                        for (uint32_t u = best; u != kSieveNoNode;) {
+                            const uint4 nb = __ldg(reinterpret_cast<const uint4 *>(sv.nb + u));
+                            for (uint32_t t = 0; t < nb.y; t++) {
+                                const uint32_t pid = __ldg(sv.pids + nb.x + t);
+                                if (!filter_admits(frow, pid)) continue;
+                                if (idx < out.cap) {
+                                    reinterpret_cast<uint4 *>(out.raw)[idx] = make_uint4((uint32_t)h, pid, end_rel - nb.w, end_rel);
+                                    out.raw_seq[idx] = seq;
+                                    out.raw_unit[idx] = task;
+                                    if (CP) out.raw_aux[idx] = aux;
+                                }
+                                idx++;
+                                seq++;
+                            }
+                            u = nb.z;
+                        }
+                    } else
                     for (uint32_t u = best; u != kSieveNoNode;) {
                         const uint4 nb = __ldg(reinterpret_cast<const uint4 *>(sv.nb + u));  // own_off, own_cnt, term_link, depth
                         for (uint32_t t = 0; t < nb.y; t++, idx++, seq++) {
@@ -754,6 +846,20 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
         if (tasks_skipped) atomicAdd(skipped, (unsigned long long)tasks_skipped);
         if (windows_skipped) atomicAdd(skipped + 1, (unsigned long long)windows_skipped);
     }
+}
+
+template <bool CP, int WC, int MODE = kSieveList>
+__global__ void __launch_bounds__(kSieveThreads, 1)
+sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_cont, uint32_t *hay_cont, unsigned int *task_counter) {
+    sieve_scan<CP, WC, MODE, false>(sv, B, P, out, task_cont, hay_cont, task_counter, SieveFilter{});
+}
+
+// the same scan with each haystack's pattern set (LIST, ANY, FIRST and COUNT)
+template <bool CP, int WC, int MODE = kSieveList>
+__global__ void __launch_bounds__(kSieveThreads, 1)
+sieve_scan_filtered_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_cont, uint32_t *hay_cont, unsigned int *task_counter,
+                           SieveFilter F) {
+    sieve_scan<CP, WC, MODE, true>(sv, B, P, out, task_cont, hay_cont, task_counter, F);
 }
 
 }  // namespace acb

@@ -126,6 +126,105 @@ PATH_SEARCH = 2      # per-haystack offsets by binary search (more than 4 record
 PATH_REPAIRED = 4    # some speculated segment start was wrong and the repair pass ran
 
 
+class PatternSets:
+    """Pattern sets of one automaton on one device: G subsets of its pattern ids, packed once into a bitset of G rows of
+    ceil(P / 32) u32 words (bit p % 32 of word p // 32 of row g = pattern p is in set g).  Made by ``pattern_sets`` of
+    the classes; a query given ``pattern_sets=ps, set_index=idx`` searches haystack i for the patterns of set idx[i]
+    only, and returns exactly what an automaton built from those patterns (same match kind, same relative order)
+    would return, with the full automaton's pattern ids."""
+
+    def __init__(self, ac: "_Automaton", sets, device=None):
+        torch = _torch()
+        P = ac.n_patterns
+        if device is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        device = torch.device(device)
+        if device.type == "cuda" and device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        if torch.is_tensor(sets):
+            if sets.dtype != torch.bool or sets.dim() != 2 or sets.shape[1] != P:
+                raise ValueError(f"a tensor of pattern sets must be a bool tensor of shape (G, {P})")
+            mask = sets.to(device)
+        else:
+            rows = [list(s) for s in sets]
+            mask = np.zeros((len(rows), P), dtype=bool)
+            for g, ids in enumerate(rows):
+                for p in ids:
+                    if isinstance(p, bool) or not isinstance(p, (int, np.integer)):
+                        raise ValueError(f"set {g}: pattern ids must be ints, not {type(p).__name__}")
+                    if not 0 <= int(p) < P:
+                        raise ValueError(f"set {g}: pattern id {int(p)} is outside [0, {P})")
+                    mask[g, int(p)] = True
+            mask = torch.from_numpy(mask).to(device)
+        if mask.shape[0] < 1:
+            raise ValueError("pattern sets: at least one set is needed")
+        self._ac = ac
+        self.device = device
+        self.n_sets = int(mask.shape[0])
+        self.words = max((P + 31) // 32, 1)
+        self.bits = self.pack(mask, self.words)
+
+    @staticmethod
+    def pack(mask, words: int):
+        """(G, P) bool tensor -> (G, words) int32 tensor, the u32 bitset rows (torch ops on the mask's device)."""
+        torch = _torch()
+        G, P = mask.shape
+        padded = torch.zeros((G, words * 32), dtype=torch.int64, device=mask.device)
+        padded[:, :P] = mask.to(torch.int64)
+        weights = torch.bitwise_left_shift(torch.ones(32, dtype=torch.int64, device=mask.device), torch.arange(32, device=mask.device))
+        w = (padded.view(G, words, 32) * weights).sum(dim=2)
+        return torch.where(w >= (1 << 31), w - (1 << 32), w).to(torch.int32).contiguous()
+
+
+def _filter_args(ac: "_Automaton", pattern_sets, set_index, n: int, dev):
+    """Checks a device call's (pattern_sets, set_index) -> the filter the internal paths carry: None, or
+    (PatternSets, contiguous int32 / int64 index tensor (n,))."""
+    torch = _torch()
+    if pattern_sets is None and set_index is None:
+        return None
+    if pattern_sets is None or set_index is None:
+        raise ValueError("pattern_sets and set_index go together: give both or neither")
+    if not isinstance(pattern_sets, PatternSets) or pattern_sets._ac is not ac:
+        raise ValueError("pattern_sets must come from this automaton's pattern_sets()")
+    if pattern_sets.device != dev:
+        raise ValueError(f"pattern_sets live on {pattern_sets.device}, the data on {dev}")
+    if (not torch.is_tensor(set_index) or set_index.dtype not in (torch.int32, torch.int64) or set_index.dim() != 1 or
+            set_index.shape[0] != n or set_index.device != dev):
+        raise ValueError(f"set_index must be an int32 or int64 tensor of shape ({n},) on {dev}")
+    if n:
+        lo, hi = (int(v) for v in torch.stack(torch.aminmax(set_index)).tolist())
+        if lo < 0 or hi >= pattern_sets.n_sets:
+            raise ValueError(f"set_index values must lie in [0, {pattern_sets.n_sets}); found [{lo}, {hi}]")
+    return pattern_sets, set_index.contiguous()
+
+
+def _filter_struct(flt):
+    """The acb_pattern_filter of an internal filter (None: no filter, a NULL pointer)."""
+    if flt is None:
+        return None
+    ps, idx = flt
+    f = _capi.PatternFilter()
+    f.dev_set_bits = ps.bits.data_ptr()
+    f.n_sets = ps.n_sets
+    f.dev_set_index = idx.data_ptr() if idx.numel() else ps.bits.data_ptr()
+    f.index_bytes = idx.element_size()
+    return C.byref(f)
+
+
+def _filter_slice(flt, a: int, b: int):
+    return None if flt is None else (flt[0], flt[1][a:b])
+
+
+def _host_sets(ac: "_Automaton", patterns, n: int, dev):
+    """A host call's patterns= -> an internal filter for its n haystacks: one set per haystack (n > 1: `patterns` holds
+    one iterable per haystack; n == 1 and single: the iterable itself)."""
+    torch = _torch()
+    ps = PatternSets(ac, patterns, dev)
+    if ps.n_sets != n:
+        raise ValueError(f"patterns= needs one set of pattern ids per haystack: {n} haystacks, {ps.n_sets} sets")
+    return ps, torch.arange(n, dtype=torch.int32, device=dev)
+
+
 class _Automaton:
     """Owns the host automaton handle, its device image and a growable device
     workspace.  Shared by both public classes."""
@@ -376,7 +475,7 @@ class _Automaton:
         hot = self.hot(dev, data, offsets, overlapping)
         return None if hot["rows"].reserved & 1 else hot
 
-    def any_device(self, data, offsets, out=None, sync: bool = True):
+    def any_device(self, data, offsets, out=None, sync: bool = True, flt=None):
         """Which haystacks of a device-resident batch contain an occurrence of any pattern -> bool CUDA tensor (n,).
         The answer does not depend on the match kind.  `out` (bool, (n,), contiguous, on the data's device): the
         answer is OR-ed into it, and haystacks already True there are not scanned.  With sync=False a call that runs
@@ -401,17 +500,18 @@ class _Automaton:
         if data.numel() > self.WINDOW_BYTES:
             if not sync:
                 raise ValueError(f"buffers above {self.WINDOW_BYTES} bytes are scanned in windows: sync=False is not available")
-            return self._any_device_windows(data, offsets, out if out is not None else torch.zeros(n, dtype=torch.bool, device=dev))
+            return self._any_device_windows(data, offsets, out if out is not None else torch.zeros(n, dtype=torch.bool, device=dev), flt)
         with self._lock, torch.cuda.device(dev):
-            use_sieve = self._pick_engine(dev, data, offsets, False) is None
+            use_sieve = flt is not None or self._pick_engine(dev, data, offsets, False) is None
             if use_sieve:
                 if out is None:
                     out = torch.zeros(n, dtype=torch.bool, device=dev)
                 sieve_t, _ = self.sieve(dev)
                 plan = self._plan(data, n)
                 scratch = torch.empty(3, dtype=torch.int64, device=dev)
-                rc = self._L.acb_any_match(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
-                                           out.data_ptr(), scratch.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+                rc = self._L.acb_any_match_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
+                                                    out.data_ptr(), scratch.data_ptr(), _filter_struct(flt),
+                                                    torch.cuda.current_stream(dev).cuda_stream)
                 if rc != _capi.ACB_OK:
                     raise RuntimeError(_capi.last_error())
             else:
@@ -435,10 +535,14 @@ class _Automaton:
             task_bytes = int(plan.task_bytes)
             tasks = (data.numel() + (data.data_ptr() & 511) + task_bytes - 1) // task_bytes
             self.last_stats = {"engine": "sieve", "mode": "any", **self.sieve_geometry(dev, task_bytes), "tasks": tasks,
-                               "tasks_skipped": skipped, "windows_skipped": windows}
+                               "tasks_skipped": skipped, "windows_skipped": windows, **self._set_stats(flt)}
         return out
 
-    def _any_device_windows(self, data, offsets, out):
+    def _set_stats(self, flt):
+        """last_stats entries of a call with pattern sets (none without)."""
+        return {} if flt is None else {"pattern_sets": flt[0].n_sets}
+
+    def _any_device_windows(self, data, offsets, out, flt=None):
         """any_device for buffers above WINDOW_BYTES: runs of whole haystacks that fit one call each get their slice
         of `out`; one haystack above the limit is scanned in windows that share max_pattern_len - 1 bytes (an
         occurrence lies inside one of them whole) and share its flag, stopping at the first window that sets it."""
@@ -457,7 +561,7 @@ class _Automaton:
                 w0 = 0
                 while not bool(flag.item()):
                     w1 = min(w0 + limit, hay.numel())
-                    self.any_device(hay[w0:w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=dev), flag)
+                    self.any_device(hay[w0:w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=dev), flag, flt=_filter_slice(flt, h, h + 1))
                     if w1 == hay.numel():
                         break
                     w0 += step
@@ -471,7 +575,7 @@ class _Automaton:
                 if big.numel():
                     h1 = h + int(big[0].item())
             end = int(offsets[h1].item())
-            self.any_device(data[start:end], offsets[h:h1 + 1] - start, out[h:h1])
+            self.any_device(data[start:end], offsets[h:h1 + 1] - start, out[h:h1], flt=_filter_slice(flt, h, h1))
             h = h1
         return out
 
@@ -486,7 +590,7 @@ class _Automaton:
             return (s, p)
         return (s, -e, p)
 
-    def first_keys(self, data, offsets, keys):
+    def first_keys(self, data, offsets, keys, flt=None):
         """acb_find_first on the sieve: lowers the u64 keys (an int64 CUDA tensor (n,), -1 = no match yet) of a batch
         below WINDOW_BYTES; returns the u64[3] scratch tensor (task counter, tasks skipped, windows not scanned)."""
         torch = _require_cuda()
@@ -494,21 +598,21 @@ class _Automaton:
         n = offsets.numel() - 1
         sieve_t, _ = self.sieve(dev)
         scratch = torch.empty(3, dtype=torch.int64, device=dev)
-        rc = self._L.acb_find_first(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
-                                    keys.data_ptr(), scratch.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        rc = self._L.acb_find_first_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
+                                             keys.data_ptr(), scratch.data_ptr(), _filter_struct(flt), torch.cuda.current_stream(dev).cuda_stream)
         if rc != _capi.ACB_OK:
             raise RuntimeError(_capi.last_error())
         return scratch
 
-    def first_rows(self, data, offsets, keys):
+    def first_rows(self, data, offsets, keys, flt=None):
         """acb_first_rows: keys -> int64 (n, 3) rows (pattern, start, end) in bytes, -1 rows where there is no match."""
         torch = _require_cuda()
         dev = data.device
         n = offsets.numel() - 1
         sieve_t, _ = self.sieve(dev)
         rows = torch.empty((n, 3), dtype=torch.int64, device=dev)
-        rc = self._L.acb_first_rows(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, keys.data_ptr(),
-                                    rows.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        rc = self._L.acb_first_rows_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, keys.data_ptr(),
+                                             rows.data_ptr(), _filter_struct(flt), torch.cuda.current_stream(dev).cuda_stream)
         if rc != _capi.ACB_OK:
             raise RuntimeError(_capi.last_error())
         return rows
@@ -522,7 +626,7 @@ class _Automaton:
             raise RuntimeError(_capi.last_error())
         return out
 
-    def first_device(self, data, offsets, codepoints: bool = False):
+    def first_device(self, data, offsets, codepoints: bool = False, flt=None):
         """Each haystack's first match for the match kind -> int64 CUDA tensor (n, 3) = (pattern, start, end), a row of
         -1 where a haystack has none; code point indexes with codepoints.  Row h is element 0 of haystack h's
         non-overlapping list (scan_device), for every match kind.
@@ -540,10 +644,10 @@ class _Automaton:
         if data.numel() == 0:
             return torch.full((n, 3), -1, dtype=torch.int64, device=dev)
         if data.numel() > self.WINDOW_BYTES:
-            rows = self._first_device_windows(data, offsets)
+            rows = self._first_device_windows(data, offsets, flt)
             return self._rows_to_codepoints(data, offsets, rows) if codepoints else rows
         with self._lock, torch.cuda.device(dev):
-            if self._pick_engine(dev, data, offsets, False) is not None:
+            if flt is None and self._pick_engine(dev, data, offsets, False) is not None:
                 m, mo, total = self.scan_device(data, offsets, False, codepoints)
                 rows = torch.full((n, 3), -1, dtype=torch.int64, device=dev)
                 if total:
@@ -556,15 +660,15 @@ class _Automaton:
                 self.last_stats = {"engine": self.last_stats.get("engine", "table"), "mode": "first"}
                 return rows
             keys = torch.full((n,), -1, dtype=torch.int64, device=dev)   # all ones: no match yet
-            scratch = self.first_keys(data, offsets, keys)
-            rows = self.first_rows(data, offsets, keys)
+            scratch = self.first_keys(data, offsets, keys, flt)
+            rows = self.first_rows(data, offsets, keys, flt)
             task_bytes = int(self._plan(data, n).task_bytes)
-            self.last_stats = {"engine": "sieve", "mode": "first", **self.sieve_geometry(dev, task_bytes),
+            self.last_stats = {"engine": "sieve", "mode": "first", **self.sieve_geometry(dev, task_bytes), **self._set_stats(flt),
                                "tasks": (data.numel() + (data.data_ptr() & 511) + task_bytes - 1) // task_bytes,
                                "skip_counters": scratch}   # device tensor: [task counter, tasks skipped, windows not scanned]
         return self._rows_to_codepoints(data, offsets, rows) if codepoints else rows
 
-    def _first_device_windows(self, data, offsets):
+    def _first_device_windows(self, data, offsets, flt=None):
         """first_device (bytes) for buffers above WINDOW_BYTES: runs of whole haystacks that fit one call each get
         their rows (positions are haystack-relative: nothing to rebase); one haystack above the limit goes to
         _first_one_large."""
@@ -579,7 +683,7 @@ class _Automaton:
         while h < n:
             start = int(offsets[h].item())
             if oversized and int(lens[h].item()) > limit:
-                best = self._first_one_large(data[start:start + int(lens[h].item())])
+                best = self._first_one_large(data[start:start + int(lens[h].item())], _filter_slice(flt, h, h + 1))
                 if best is not None:
                     rows[h] = torch.tensor(best, dtype=torch.int64, device=dev)
                 h += 1
@@ -592,11 +696,11 @@ class _Automaton:
                 if big.numel():
                     h1 = h + int(big[0].item())
             end = int(offsets[h1].item())
-            rows[h:h1] = self.first_device(data[start:end], offsets[h:h1 + 1] - start)
+            rows[h:h1] = self.first_device(data[start:end], offsets[h:h1 + 1] - start, flt=_filter_slice(flt, h, h1))
             h = h1
         return rows
 
-    def _first_one_large(self, hay):
+    def _first_one_large(self, hay, flt=None):
         """The first match (pattern, start, end) in bytes, or None, of one haystack above WINDOW_BYTES, scanned in
         windows that share max_pattern_len - 1 bytes, in order.  A window sees every match that ends inside it and does
         not end inside the bytes it shares with its predecessor.  Standard: the first window with a match holds the
@@ -610,7 +714,7 @@ class _Automaton:
         w0 = 0
         while True:
             w1 = min(w0 + limit, hay.numel())
-            p, s, e = self.first_device(hay[w0:w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=dev))[0].tolist()
+            p, s, e = self.first_device(hay[w0:w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=dev), flt=flt)[0].tolist()
             if p >= 0 and (best is None or self.first_order((p, s + w0, e + w0)) < self.first_order(best)):
                 best = (p, s + w0, e + w0)
             if w1 == hay.numel():
@@ -619,7 +723,7 @@ class _Automaton:
                 return best
             w0 += step
 
-    def first_host_batch(self, chunks: Sequence[bytes], codepoints: bool):
+    def first_host_batch(self, chunks: Sequence[bytes], codepoints: bool, patterns=None):
         """Host buffers (bytes-like objects, one per haystack) -> list of (pattern, start, end) or None: each one's first
         match.  The offsets and the haystacks are gathered into the pinned staging buffer and go to the device in one
         copy; the rows come back in one."""
@@ -641,10 +745,11 @@ class _Automaton:
             elif total_bytes:
                 hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
             d = host[:head + total_bytes].to(dev, non_blocking=True)
-            rows = self.first_device(d[head:], d[:8 * (n + 1)].view(torch.int64), codepoints).cpu().tolist()
+            flt = _host_sets(self, patterns, n, dev) if patterns is not None else None
+            rows = self.first_device(d[head:], d[:8 * (n + 1)].view(torch.int64), codepoints, flt).cpu().tolist()
         return [tuple(r) if r[0] >= 0 else None for r in rows]
 
-    def any_host_batch(self, chunks: Sequence[bytes]):
+    def any_host_batch(self, chunks: Sequence[bytes], patterns=None):
         """Host buffers (bytes-like objects, one per haystack) -> list of bool: does each contain any pattern.  The
         offsets and the haystacks are gathered into the pinned staging buffer and go to the device in one copy."""
         torch = _require_cuda()
@@ -665,11 +770,12 @@ class _Automaton:
             elif total_bytes:
                 hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
             d = host[:head + total_bytes].to(dev, non_blocking=True)
-            mask = self.any_device(d[head:], d[:8 * (n + 1)].view(torch.int64))
+            flt = _host_sets(self, patterns, n, dev) if patterns is not None else None
+            mask = self.any_device(d[head:], d[:8 * (n + 1)].view(torch.int64), flt=flt)
             return mask.cpu().tolist()
 
     # ---- match counts per haystack: len(find_matches_as_indexes(h, overlapping)) without the list ----------------
-    def count_device(self, data, offsets, overlapping=False, capacity: Optional[int] = None):
+    def count_device(self, data, offsets, overlapping=False, capacity: Optional[int] = None, flt=None):
         """How many matches each haystack of a device-resident batch has -> int64 CUDA tensor (n,): the length of
         its list in scan_device, for every match kind.  Counts are the same in bytes and in code points, so no code
         point work is ever done.  An overlapping search on a leftmost automaton raises ValueError, as scan_device does.
@@ -688,10 +794,10 @@ class _Automaton:
         if n <= 0 or data.numel() == 0:
             return torch.zeros(max(n, 0), dtype=torch.int64, device=dev)
         if data.numel() > self.WINDOW_BYTES:
-            return self._count_device_windows(data, offsets, overlapping)
+            return self._count_device_windows(data, offsets, overlapping, flt)
         with self._lock, torch.cuda.device(dev):
             stream = torch.cuda.current_stream(dev)
-            if self._pick_engine(dev, data, offsets, overlapping) is not None:
+            if flt is None and self._pick_engine(dev, data, offsets, overlapping) is not None:
                 _, mo, _ = self.scan_device(data, offsets, overlapping, False)
                 counts = mo[1:] - mo[:-1]
                 reader = torch.cuda.Event()
@@ -703,12 +809,13 @@ class _Automaton:
             counts = torch.zeros(n, dtype=torch.int64, device=dev)
             if overlapping:
                 scratch = torch.empty(3, dtype=torch.int64, device=dev)
-                rc = self._L.acb_count_overlapping(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
-                                                   counts.data_ptr(), scratch.data_ptr(), stream.cuda_stream)
+                rc = self._L.acb_count_overlapping_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n,
+                                                            data.numel(), counts.data_ptr(), scratch.data_ptr(), _filter_struct(flt),
+                                                            stream.cuda_stream)
                 if rc != _capi.ACB_OK:
                     raise RuntimeError(_capi.last_error())
                 self.last_stats = {"engine": "sieve", "mode": "count", **self.sieve_geometry(dev, self._plan(data, n).task_bytes),
-                                   "long_stretches": 0}
+                                   "long_stretches": 0, **self._set_stats(flt)}
                 return counts
             plan = self._plan(data, n)
             cap = capacity or max(1024, n * 2)
@@ -718,8 +825,9 @@ class _Automaton:
                 if reader is not None:   # a comparison of an earlier call (maybe on another stream) reads this workspace first
                     stream.wait_event(reader)
                 st = self._ws_struct(ws)
-                rc = self._L.acb_count_non_overlapping(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
-                                                       C.byref(plan), C.byref(st), counts.data_ptr(), stream.cuda_stream)
+                rc = self._L.acb_count_non_overlapping_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n,
+                                                                data.numel(), C.byref(plan), C.byref(st), counts.data_ptr(),
+                                                                _filter_struct(flt), stream.cuda_stream)
                 if rc != _capi.ACB_OK:
                     err = _capi.last_error()
                     ws["scratch"][:8].zero_()   # a scan that failed half way may have left its counters dirty
@@ -730,10 +838,10 @@ class _Automaton:
                     break
                 cap = max(total, raw_total) + max(total, raw_total) // 8 + 16
             self.last_stats = {"engine": "sieve", "mode": "count", **self.sieve_geometry(dev, plan.task_bytes), "list_records": raw_total,
-                               "long_stretches": long_stretches}
+                               "long_stretches": long_stretches, **self._set_stats(flt)}
             return counts
 
-    def _count_device_windows(self, data, offsets, overlapping):
+    def _count_device_windows(self, data, offsets, overlapping, flt=None):
         """count_device for buffers above WINDOW_BYTES: runs of whole haystacks that fit one call each get their slice
         of the counts; one haystack above the limit goes to _count_one_large.  last_stats["long_stretches"] sums the
         runs'."""
@@ -749,7 +857,7 @@ class _Automaton:
         while h < n:
             start = int(offsets[h].item())
             if oversized and int(lens[h].item()) > limit:
-                counts[h:h + 1] = self._count_one_large(data[start:start + int(lens[h].item())], overlapping)
+                counts[h:h + 1] = self._count_one_large(data[start:start + int(lens[h].item())], overlapping, _filter_slice(flt, h, h + 1))
                 h += 1
                 continue
             # the longest run of whole haystacks that fits one call (and stops before an oversized one)
@@ -760,14 +868,15 @@ class _Automaton:
                 if big.numel():
                     h1 = h + int(big[0].item())
             end = int(offsets[h1].item())
-            counts[h:h1] = self.count_device(data[start:end], offsets[h:h1 + 1] - start, overlapping)
+            counts[h:h1] = self.count_device(data[start:end], offsets[h:h1 + 1] - start, overlapping, flt=_filter_slice(flt, h, h1))
             long_stretches += self.last_stats.get("long_stretches", 0)
             h = h1
         torch.cuda.current_stream(dev).synchronize()
-        self.last_stats = {"engine": self.last_stats.get("engine"), "mode": "count", "long_stretches": long_stretches, "windows": True}
+        self.last_stats = {"engine": self.last_stats.get("engine"), "mode": "count", "long_stretches": long_stretches, "windows": True,
+                           **self._set_stats(flt)}
         return counts
 
-    def _count_one_large(self, hay, overlapping):
+    def _count_one_large(self, hay, overlapping, flt=None):
         """The count (an int64 CUDA tensor (1,)) of one haystack above WINDOW_BYTES.
         Overlapping: windows that share max_pattern_len - 1 bytes (the head of each window but the first).  A window
         counts every match inside it; a match that lies wholly inside a window's head was counted by the window before,
@@ -781,13 +890,13 @@ class _Automaton:
             w0 = 0
             while True:
                 w1 = min(w0 + limit, hay.numel())
-                total += self.count_device(hay[w0:w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=dev), True)
+                total += self.count_device(hay[w0:w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=dev), True, flt=flt)
                 if w0 and halo:
-                    total -= self.count_device(hay[w0:w0 + halo], torch.tensor([0, halo], dtype=torch.int64, device=dev), True)
+                    total -= self.count_device(hay[w0:w0 + halo], torch.tensor([0, halo], dtype=torch.int64, device=dev), True, flt=flt)
                 if w1 == hay.numel():
                     return total
                 w0 += limit - halo
-        rows = self._overlapping_rows_large(hay, False).contiguous()
+        rows = self._overlapping_rows_large(hay, False, flt).contiguous()
         count = torch.zeros(1, dtype=torch.int64, device=dev)
         if rows.shape[0]:
             scratch = torch.empty((rows.shape[0], 2), dtype=torch.int64, device=dev)   # 16 bytes per row
@@ -797,7 +906,7 @@ class _Automaton:
                 raise RuntimeError(_capi.last_error())
         return count
 
-    def count_host_batch(self, chunks: Sequence[bytes], overlapping):
+    def count_host_batch(self, chunks: Sequence[bytes], overlapping, patterns=None):
         """Host buffers (bytes-like objects, one per haystack) -> list of int: each one's match count.  The offsets and
         the haystacks are gathered into the pinned staging buffer and go to the device in one copy."""
         torch = _require_cuda()
@@ -819,7 +928,8 @@ class _Automaton:
             elif total_bytes:
                 hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
             d = host[:head + total_bytes].to(dev, non_blocking=True)
-            return self.count_device(d[head:], d[:8 * (n + 1)].view(torch.int64), overlapping).cpu().tolist()
+            flt = _host_sets(self, patterns, n, dev) if patterns is not None else None
+            return self.count_device(d[head:], d[:8 * (n + 1)].view(torch.int64), overlapping, flt=flt).cpu().tolist()
 
     # ---- match counts per pattern: bincount of find_matches_as_indexes' patterns, summed over a batch, without the list
     def pattern_counts_device(self, data, offsets, overlapping=False, capacity: Optional[int] = None):
@@ -1130,7 +1240,7 @@ class _Automaton:
         return [p[ro[i]:ro[i + 1]] for i in range(n)]
 
     def scan_device(self, data, offsets, overlapping=False, codepoints=False, capacity: Optional[int] = None,
-                    sync: bool = True, ws_slot: int = 0):
+                    sync: bool = True, ws_slot: int = 0, flt=None):
         """Scan a device-resident batch.  data: uint8 CUDA tensor, offsets: int64
         CUDA tensor (n+1).  One haystack of any size is simply n = 1.  Returns
         (matches, match_offsets, total): matches is an int32 CUDA tensor
@@ -1149,12 +1259,12 @@ class _Automaton:
         if data.numel() > self.WINDOW_BYTES:
             if not sync:
                 raise ValueError(f"buffers above {self.WINDOW_BYTES} bytes are scanned in windows: sync=False is not available")
-            return self._scan_device_windows(data, offsets, overlapping, codepoints)
+            return self._scan_device_windows(data, offsets, overlapping, codepoints, flt)
         img = self.image(dev)
         cap = capacity or max(1024, n * 2)
         stream = torch.cuda.current_stream(dev).cuda_stream
         with self._lock, torch.cuda.device(dev):
-            hot = self._pick_engine(dev, data, offsets, overlapping)
+            hot = self._pick_engine(dev, data, offsets, overlapping) if flt is None else None   # (pattern sets: the sieve)
             use_sieve = hot is None
             if use_sieve:
                 sieve_t, sieve_d = self.sieve(dev)
@@ -1165,11 +1275,12 @@ class _Automaton:
                 if reader is not None:   # any_device's comparison (maybe on another stream) reads this workspace first
                     torch.cuda.current_stream(dev).wait_event(reader)
                 st = self._ws_struct(ws)
-                rc = self._L.acb_scan_batch(self._h, img.data_ptr(),
-                                            hot["tensor"].data_ptr() if hot else None, C.byref(hot["rows"]) if hot else None,
-                                            sieve_t.data_ptr() if use_sieve else None,
-                                            data.data_ptr(), offsets.data_ptr(), n, data.numel(),
-                                            2 if overlapping == 2 else int(bool(overlapping)), int(bool(codepoints)), C.byref(plan), C.byref(st), stream)
+                rc = self._L.acb_scan_batch_filtered(self._h, img.data_ptr(),
+                                                     hot["tensor"].data_ptr() if hot else None, C.byref(hot["rows"]) if hot else None,
+                                                     sieve_t.data_ptr() if use_sieve else None,
+                                                     data.data_ptr(), offsets.data_ptr(), n, data.numel(),
+                                                     2 if overlapping == 2 else int(bool(overlapping)), int(bool(codepoints)), C.byref(plan),
+                                                     C.byref(st), _filter_struct(flt), stream)
                 if rc != _capi.ACB_OK:
                     err = _capi.last_error()
                     ws["scratch"][:8].zero_()   # a scan that failed half way may have left its counters dirty
@@ -1188,7 +1299,8 @@ class _Automaton:
                                        "segment_bytes": plan.segment_bytes, "lane_stride": plan.lane_stride}
                 else:
                     self.last_stats = {"engine": "sieve", **self.sieve_geometry(dev, plan.task_bytes), "nodes": sieve_d.nodes,
-                                       "keys": sieve_d.keys, "filter_entries": sieve_d.filter_entries, "list_records": raw_total}
+                                       "keys": sieve_d.keys, "filter_entries": sieve_d.filter_entries, "list_records": raw_total,
+                                       **self._set_stats(flt)}
                 if complete or (total == 0 and raw_total == 0):
                     return ws["out"][:total], ws["match_offsets"][: n + 1], total
                 cap = max(total, raw_total) + max(total, raw_total) // 8 + 16
@@ -1197,7 +1309,7 @@ class _Automaton:
     # runs of whole haystacks, a single haystack above the limit into overlapping windows.
     WINDOW_BYTES = (1 << 31) - (1 << 16)   # (below 2^31: every offset of one call is a non-negative int32)
 
-    def _scan_device_windows(self, data, offsets, overlapping, codepoints):
+    def _scan_device_windows(self, data, offsets, overlapping, codepoints, flt=None):
         """scan_device for buffers above WINDOW_BYTES.  Same results, as int64 tensors
         (offsets no longer fit 32 bits): (matches (k, 4) int64, match_offsets (n + 1) int64, total).
         Everything stays on the device; the host only learns where the runs of whole haystacks end."""
@@ -1214,7 +1326,7 @@ class _Automaton:
         while h < n:
             start = int(offsets[h].item())
             if oversized and int(lens[h].item()) > limit:
-                part = self._scan_one_large(data[start:start + int(lens[h].item())], overlapping, codepoints)
+                part = self._scan_one_large(data[start:start + int(lens[h].item())], overlapping, codepoints, _filter_slice(flt, h, h + 1))
                 part[:, 0] = h
                 parts.append(part)
                 base_count += int(part.shape[0])
@@ -1231,7 +1343,7 @@ class _Automaton:
             end = int(offsets[h1].item())
             sub_offs = offsets[h:h1 + 1] - start
             _t0 = __import__("time").perf_counter() if _TRACE else 0
-            m, mo_run, total = self.scan_device(data[start:end], sub_offs, overlapping, codepoints)
+            m, mo_run, total = self.scan_device(data[start:end], sub_offs, overlapping, codepoints, flt=_filter_slice(flt, h, h1))
             _t1 = __import__("time").perf_counter() if _TRACE else 0
             part = m.to(torch.int64)
             if h:
@@ -1248,7 +1360,7 @@ class _Automaton:
             out = torch.zeros((0, 4), dtype=torch.int64, device=dev)
         return out, mo, int(out.shape[0])
 
-    def _scan_one_large(self, hay, overlapping, codepoints):
+    def _scan_one_large(self, hay, overlapping, codepoints, flt=None):
         """One haystack above WINDOW_BYTES (BASELINE config 4: one 4 GiB haystack, overlapping).  The OVERLAPPING list
         is exact window by window: windows that share max_pattern_len - 1 bytes are independent (what ends at a position
         depends on no more than that), each keeps the matches that END beyond the shared bytes.  A non-overlapping
@@ -1256,7 +1368,7 @@ class _Automaton:
         overlapping list afterwards (acb_select_non_overlapping; SURVEY.md 8c), for all three match kinds."""
         torch = _require_cuda()
         dev = hay.device
-        rows = self._overlapping_rows_large(hay, codepoints)
+        rows = self._overlapping_rows_large(hay, codepoints, flt)
         if overlapping or rows.shape[0] == 0:
             return rows
         rows = rows.contiguous()
@@ -1268,7 +1380,7 @@ class _Automaton:
             raise RuntimeError(_capi.last_error())
         return out[: int(count.item())]
 
-    def _overlapping_rows_large(self, hay, codepoints):
+    def _overlapping_rows_large(self, hay, codepoints, flt=None):
         """The overlapping list of one haystack above WINDOW_BYTES, whatever the match kind, as int64 rows (haystack,
         pattern, start, end) in the reference's order (see _scan_one_large)."""
         torch = _require_cuda()
@@ -1276,17 +1388,17 @@ class _Automaton:
 
         def scan_window(window):
             one = torch.tensor([0, window.numel()], dtype=torch.int64, device=dev)
-            m, _, _ = self._scan_overlapping_list(window, one, codepoints)
+            m, _, _ = self._scan_overlapping_list(window, one, codepoints, flt)
             return m.to(torch.int64)
 
         parts = scan_in_windows(scan_window, hay, self.WINDOW_BYTES, max(self.max_pattern_len - 1, 0), codepoints)
         return torch.cat(parts, dim=0) if parts else torch.zeros((0, 4), dtype=torch.int64, device=dev)
 
-    def _scan_overlapping_list(self, data, offsets, codepoints):
+    def _scan_overlapping_list(self, data, offsets, codepoints, flt=None):
         """The overlapping match list whatever the automaton's match kind: the sieve's structures do not depend on the
         kind (overlapping = 2 is the library-internal form of the request; the public overlapping=True on a leftmost
         automaton stays an error, like the reference's)."""
-        return self.scan_device(data, offsets, 2, codepoints)
+        return self.scan_device(data, offsets, 2, codepoints, flt=flt)
 
     # ---- host-resident input (the reference's situation: src/lib.rs:229-249, 422-434 take host str / buffers) ----
     HOST_CHUNK_BYTES = 1 << 30     # inputs up to this size go in one piece (the scan is ~100x faster than PCIe: nothing to hide);
@@ -1480,13 +1592,15 @@ class _Automaton:
                 return hr[8:8 + 2 * total].view(np.uint32).reshape(total, 4).copy()
             return ctx["ws"]["out"][:total].cpu().numpy().view(np.uint32)
 
-    def scan_host_batch(self, chunks: Sequence[bytes], overlapping: bool, codepoints: bool):
+    def scan_host_batch(self, chunks: Sequence[bytes], overlapping: bool, codepoints: bool, patterns=None):
         """Host buffers (bytes-like objects, one per haystack) in, host numpy out: (matches uint32 (k,4),
         match_offsets int64 (n+1)).  The haystacks are gathered into this automaton's pinned staging buffer
         (for a single haystack: one copy straight out of the caller's buffer), then scan_host takes over."""
         torch = _require_cuda()
         self.check_overlapping(overlapping)
         n = len(chunks)
+        if patterns is not None:
+            return self._scan_host_batch_filtered(chunks, overlapping, codepoints, patterns)
         if n == 1 and len(chunks[0]) <= self.SMALL_CALL_BYTES and _capi.current_kernel() in (0, 5) and self.ENGINE != "table":
             m = self._small_call(chunks[0], overlapping, codepoints)
             if m is not None:
@@ -1503,6 +1617,36 @@ class _Automaton:
             elif total_bytes:
                 hv[:total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)  # one C-speed concatenation, one copy into pinned memory
             return self.scan_host(host[:total_bytes], offs, overlapping, codepoints)
+
+
+    def _scan_host_batch_filtered(self, chunks: Sequence[bytes], overlapping: bool, codepoints: bool, patterns):
+        """scan_host_batch with one pattern set per haystack: the haystacks are gathered into the pinned staging buffer
+        with their offsets, go to the device in one copy and are scanned by scan_device with the sets (the sieve)."""
+        torch = _require_cuda()
+        n = len(chunks)
+        dev = torch.device("cuda", torch.cuda.current_device())
+        offs = np.zeros(n + 1, dtype=np.int64)
+        if n:
+            np.cumsum(np.fromiter((len(c) for c in chunks), dtype=np.int64, count=n), out=offs[1:])
+        total_bytes = int(offs[-1])
+        if n == 0:
+            if len(list(patterns)) != 0:
+                raise ValueError("patterns= needs one set of pattern ids per haystack: 0 haystacks")
+            return np.zeros((0, 4), dtype=np.uint32), offs
+        head = (8 * (n + 1) + 511) & ~511   # the offsets, then the bytes at a 512-byte boundary of the buffer
+        with self._host_lock:
+            flt = _host_sets(self, patterns, n, dev)
+            host = self._pinned(head + total_bytes)
+            hv = host.numpy()
+            hv[:8 * (n + 1)].view(np.int64)[:] = offs
+            if n == 1:
+                hv[head:head + total_bytes] = np.frombuffer(chunks[0], dtype=np.uint8)
+            elif total_bytes:
+                hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
+            d = host[:head + total_bytes].to(dev, non_blocking=True)
+            m, mo, _ = self.scan_device(d[head:], d[:8 * (n + 1)].view(torch.int64), overlapping, codepoints, flt=flt)
+            m = m.cpu().numpy()
+            return (m.view(np.uint32) if m.dtype == np.int32 else m), mo.cpu().numpy().astype(np.int64)
 
 
 class StreamBatch:
@@ -1678,6 +1822,7 @@ class _QueryStreamBatch(StreamBatch):
 
     MODE = ""
     POSITIONS = False   # answers with positions (code points are carried for the str class)
+    _flt = None         # each stream's pattern set (is_match and find_first): (PatternSets, set index (n_streams,))
 
     def _feed_args(self, data, offsets, last):
         torch = _torch()
@@ -1693,6 +1838,8 @@ class _QueryStreamBatch(StreamBatch):
             raise TypeError(f"last must be None or a bool tensor of shape ({n},) on {dev}")
         if data.numel() > self._ac.WINDOW_BYTES:
             raise ValueError(f"one feed addresses at most {self._ac.WINDOW_BYTES} bytes (WINDOW_BYTES): feed larger data in more chunks")
+        if self._flt is not None and dev != self._flt[0].device:
+            raise TypeError(f"data must be on {self._flt[0].device}, where this batch's pattern sets live")
         _require_cuda()
         return dev, data.contiguous(), offsets.contiguous(), (last.contiguous().view(torch.uint8) if last is not None else None)
 
@@ -1721,7 +1868,7 @@ class _QueryStreamBatch(StreamBatch):
                 raise RuntimeError(_capi.last_error())
             task_bytes = int(ac._plan(data, max(self.n_streams, 1)).task_bytes)
             self.last_stats = {"engine": "sieve", "mode": self.MODE, **ac.sieve_geometry(dev, task_bytes),
-                               "seam_bytes": int(self._seam_offsets[self.n_streams].item()), **stats}
+                               "seam_bytes": int(self._seam_offsets[self.n_streams].item()), **stats, **ac._set_stats(self._flt)}
         ac.last_stats = dict(self.last_stats)
         return out
 
@@ -1748,8 +1895,8 @@ class IsMatchStreamBatch(_QueryStreamBatch):
         scratch = torch.empty((2, 3), dtype=torch.int64, device=dev)
         # the seams first: a stream whose match crosses the cut then has its chunk skipped
         for k, (b, o) in enumerate(((self._seam, self._seam_offsets), (data, offsets))):
-            rc = L.acb_any_match(ac._h, sieve_t.data_ptr(), b.data_ptr(), o.data_ptr(), n, b.numel(), self._flags.data_ptr(),
-                                 scratch[k].data_ptr(), stream)
+            rc = L.acb_any_match_filtered(ac._h, sieve_t.data_ptr(), b.data_ptr(), o.data_ptr(), n, b.numel(), self._flags.data_ptr(),
+                                          scratch[k].data_ptr(), _filter_struct(self._flt), stream)
             if rc != _capi.ACB_OK:
                 raise RuntimeError(_capi.last_error())
         out = self._flags.clone()
@@ -1776,14 +1923,15 @@ class FindFirstStreamBatch(_QueryStreamBatch):
     def _query(self, dev, data, offsets, last_u8, stream):
         torch = _torch()
         ac, L, n = self._ac, self._ac._L, self.n_streams
-        ac.first_keys(self._seam, self._seam_offsets, self._keys[0])
-        chunk_scratch = ac.first_keys(data, offsets, self._keys[1])
+        ac.first_keys(self._seam, self._seam_offsets, self._keys[0], self._flt)
+        chunk_scratch = ac.first_keys(data, offsets, self._keys[1], self._flt)
         scratch = torch.empty(2 + 12 * n, dtype=torch.int64, device=dev)
         rows = torch.empty((n, 3), dtype=torch.int64, device=dev)
-        rc = L.acb_stream_first_resolve(ac._h, ac.sieve(dev)[0].data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
-                                        last_u8.data_ptr() if last_u8 is not None else None, int(self._codepoints), self._carry.data_ptr(),
-                                        self._seam.data_ptr(), self._seam_offsets.data_ptr(), self._seam.numel(), self._keys[0].data_ptr(),
-                                        self._keys[1].data_ptr(), self._best.data_ptr(), scratch.data_ptr(), rows.data_ptr(), stream)
+        rc = L.acb_stream_first_resolve_filtered(ac._h, ac.sieve(dev)[0].data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
+                                                 last_u8.data_ptr() if last_u8 is not None else None, int(self._codepoints),
+                                                 self._carry.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(),
+                                                 self._seam.numel(), self._keys[0].data_ptr(), self._keys[1].data_ptr(), self._best.data_ptr(),
+                                                 scratch.data_ptr(), rows.data_ptr(), _filter_struct(self._flt), stream)
         if rc != _capi.ACB_OK:
             raise RuntimeError(_capi.last_error())
         return rows, {**self._skips(chunk_scratch), "pending": int(scratch[1].item())}
@@ -1896,14 +2044,26 @@ def _first_answer(row):
     return tuple(row) if row[0] >= 0 else None
 
 
-def _query_stream_batch(ac, kind: str, n_streams: int, overlapping: bool, codepoints: bool) -> _QueryStreamBatch:
+def _query_stream_batch(ac, kind: str, n_streams: int, overlapping: bool, codepoints: bool, pattern_sets=None,
+                        set_index=None) -> _QueryStreamBatch:
+    """A query batch; is_match and find_first take each stream's pattern set (fixed for the batch's life)."""
     cls = {"is_match": IsMatchStreamBatch, "find_first": FindFirstStreamBatch, "count": CountStreamBatch}[kind]
-    return cls(ac, n_streams, overlapping, codepoints)
+    batch = cls(ac, n_streams, overlapping, codepoints)
+    if pattern_sets is not None or set_index is not None:
+        dev = pattern_sets.device if isinstance(pattern_sets, PatternSets) else None
+        batch._flt = _filter_args(ac, pattern_sets, set_index, n_streams, dev)
+    return batch
 
 
-def _query_stream(ac, kind: str, overlapping: bool, codepoints: bool) -> QueryStream:
+def _query_stream(ac, kind: str, overlapping: bool, codepoints: bool, patterns=None) -> QueryStream:
+    """A host-fed query stream; `patterns`: the stream's pattern ids (is_match and find_first), or None."""
     answer = {"is_match": bool, "find_first": _first_answer, "count": int}[kind]
-    return QueryStream(_query_stream_batch(ac, kind, 1, overlapping, codepoints), answer)
+    if patterns is None:
+        return QueryStream(_query_stream_batch(ac, kind, 1, overlapping, codepoints), answer)
+    torch = _require_cuda()
+    ps = PatternSets(ac, [patterns])
+    return QueryStream(_query_stream_batch(ac, kind, 1, overlapping, codepoints, ps, torch.zeros(1, dtype=torch.int32, device=ps.device)),
+                       answer)
 
 
 def _as_buffer_bytes(obj) -> bytes:
@@ -1929,7 +2089,35 @@ def _tuples(m: np.ndarray):
     return list(zip(m[:, 1].tolist(), m[:, 2].tolist(), m[:, 3].tolist()))
 
 
-class AhoCorasick:
+def _one_set(patterns):
+    """A single-haystack host call's patterns= -> the per-haystack list the host batches take (None stays None)."""
+    return None if patterns is None else [patterns]
+
+
+def _batch_sets(patterns, n: int):
+    """A host batch's patterns= (one iterable of ids per haystack) -> a list of n of them (None stays None)."""
+    if patterns is None:
+        return None
+    sets = list(patterns)
+    if len(sets) != n:
+        raise ValueError(f"patterns= needs one set of pattern ids per haystack: {n} haystacks, {len(sets)} sets")
+    return sets
+
+
+class _PatternSetMethods:
+    """pattern_sets() and the device-call check of (pattern_sets, set_index), shared by the three classes."""
+
+    def pattern_sets(self, sets, device=None) -> PatternSets:
+        """Pattern sets for the pattern_sets= / set_index= arguments: `sets` is a list of iterables of pattern ids or a
+        (G, P) bool tensor; packed once into a bitset on `device` (default: the current CUDA device).  Ids outside
+        [0, P), G == 0 or a tensor of another shape raise ValueError."""
+        return PatternSets(self._ac, sets, device)
+
+    def _device_filter(self, data, offsets, pattern_sets, set_index):
+        return _filter_args(self._ac, pattern_sets, set_index, offsets.numel() - 1, data.device)
+
+
+class AhoCorasick(_PatternSetMethods):
     """Search for multiple pattern strings against a haystack string
     (reference: src/lib.rs:15-33, 134-273).
 
@@ -1972,98 +2160,104 @@ class AhoCorasick:
         self._patterns = strs if store else None
         self._ac = _Automaton(encoded, matchkind, implementation)
 
-    def find_matches_as_indexes(self, haystack: str, overlapping: bool = False):
-        """-> list of (pattern index, start, end) in code points (src/lib.rs:229-249)."""
+    def find_matches_as_indexes(self, haystack: str, overlapping: bool = False, patterns=None):
+        """-> list of (pattern index, start, end) in code points (src/lib.rs:229-249).  `patterns`: search only for
+        these pattern ids (as an automaton of those patterns would; ids stay the full automaton's)."""
         if not isinstance(haystack, str):
             raise TypeError("argument 'haystack': 'str' expected")
         self._ac.check_overlapping(overlapping)
-        m, _ = self._ac.scan_host_batch([haystack.encode("utf-8")], overlapping, codepoints=True)
+        m, _ = self._ac.scan_host_batch([haystack.encode("utf-8")], overlapping, codepoints=True, patterns=_one_set(patterns))
         return _tuples(m)
 
-    def find_matches_as_strings(self, haystack: str, overlapping: bool = False):
-        """-> list of matched patterns (src/lib.rs:253-272)."""
+    def find_matches_as_strings(self, haystack: str, overlapping: bool = False, patterns=None):
+        """-> list of matched patterns (src/lib.rs:253-272).  `patterns`: as for find_matches_as_indexes."""
         if not isinstance(haystack, str):
             raise TypeError("argument 'haystack': 'str' expected")
         self._ac.check_overlapping(overlapping)
-        m, _ = self._ac.scan_host_batch([haystack.encode("utf-8")], overlapping, codepoints=True)
+        m, _ = self._ac.scan_host_batch([haystack.encode("utf-8")], overlapping, codepoints=True, patterns=_one_set(patterns))
         if self._patterns is not None:
             pats = self._patterns
             return [pats[i] for i in m[:, 1].tolist()]
         return [haystack[s:e] for s, e in zip(m[:, 2].tolist(), m[:, 3].tolist())]
 
     # ---- additions: batches ------------------------------------------------------
-    def find_matches_as_indexes_batch(self, haystacks: Sequence[str], overlapping: bool = False):
+    def find_matches_as_indexes_batch(self, haystacks: Sequence[str], overlapping: bool = False, patterns=None):
         """One list of (pattern, start, end) per haystack, each exactly what
-        ``find_matches_as_indexes`` returns for it."""
+        ``find_matches_as_indexes`` returns for it (`patterns`: one iterable of ids per haystack)."""
         self._ac.check_overlapping(overlapping)
-        m, offs = self._ac.scan_host_batch([h.encode("utf-8") for h in haystacks], overlapping, codepoints=True)
+        m, offs = self._ac.scan_host_batch([h.encode("utf-8") for h in haystacks], overlapping, codepoints=True,
+                                           patterns=_batch_sets(patterns, len(haystacks)))
         t = _tuples(m)
         return [t[offs[i]:offs[i + 1]] for i in range(len(haystacks))]
 
-    def scan_device(self, data, offsets, overlapping: bool = False, **kw):
-        """Device-resident UTF-8 batch -> (matches, match_offsets, total); code point indexes."""
-        return self._ac.scan_device(data, offsets, overlapping, codepoints=True, **kw)
+    def scan_device(self, data, offsets, overlapping: bool = False, pattern_sets=None, set_index=None, **kw):
+        """Device-resident UTF-8 batch -> (matches, match_offsets, total); code point indexes.  pattern_sets= /
+        set_index=: haystack i searches only for the patterns of set set_index[i]."""
+        self._ac.check_overlapping(overlapping)
+        return self._ac.scan_device(data, offsets, overlapping, codepoints=True,
+                                    flt=self._device_filter(data, offsets, pattern_sets, set_index), **kw)
 
     # ---- additions: yes / no per haystack (the crate's AhoCorasick::is_match) ------------------------------
-    def is_match(self, haystack: str) -> bool:
+    def is_match(self, haystack: str, patterns=None) -> bool:
         """Does any pattern occur in `haystack`?  The same for every match kind, so there is no `overlapping`."""
         if not isinstance(haystack, str):
             raise TypeError("argument 'haystack': 'str' expected")
-        return self._ac.any_host_batch([haystack.encode("utf-8")])[0]
+        return self._ac.any_host_batch([haystack.encode("utf-8")], _one_set(patterns))[0]
 
-    def is_match_batch(self, haystacks: Sequence[str]) -> list:
+    def is_match_batch(self, haystacks: Sequence[str], patterns=None) -> list:
         """``is_match`` for each haystack, in one transfer and one scan."""
         hays = list(haystacks)
         for h in hays:
             if not isinstance(h, str):
                 raise TypeError("argument 'haystack': 'str' expected")
-        return self._ac.any_host_batch([h.encode("utf-8") for h in hays])
+        return self._ac.any_host_batch([h.encode("utf-8") for h in hays], _batch_sets(patterns, len(hays)))
 
-    def is_match_device(self, data, offsets, out=None, sync: bool = True):
+    def is_match_device(self, data, offsets, out=None, sync: bool = True, pattern_sets=None, set_index=None):
         """Device-resident UTF-8 batch -> bool tensor (n,) on its device (see _Automaton.any_device)."""
-        return self._ac.any_device(data, offsets, out, sync)
+        return self._ac.any_device(data, offsets, out, sync, flt=self._device_filter(data, offsets, pattern_sets, set_index))
 
     # ---- additions: the first match per haystack (the crate's AhoCorasick::find) ---------------------------------
-    def find_first(self, haystack: str):
+    def find_first(self, haystack: str, patterns=None):
         """-> (pattern index, start, end) in code points, or None: ``find_matches_as_indexes(haystack)[0]``, found
         without the rest of the list."""
         if not isinstance(haystack, str):
             raise TypeError("argument 'haystack': 'str' expected")
-        return self._ac.first_host_batch([haystack.encode("utf-8")], codepoints=True)[0]
+        return self._ac.first_host_batch([haystack.encode("utf-8")], codepoints=True, patterns=_one_set(patterns))[0]
 
-    def find_first_batch(self, haystacks: Sequence[str]) -> list:
+    def find_first_batch(self, haystacks: Sequence[str], patterns=None) -> list:
         """``find_first`` for each haystack, in one transfer and one scan."""
         hays = list(haystacks)
         for h in hays:
             if not isinstance(h, str):
                 raise TypeError("argument 'haystack': 'str' expected")
-        return self._ac.first_host_batch([h.encode("utf-8") for h in hays], codepoints=True)
+        return self._ac.first_host_batch([h.encode("utf-8") for h in hays], codepoints=True, patterns=_batch_sets(patterns, len(hays)))
 
-    def find_first_device(self, data, offsets):
+    def find_first_device(self, data, offsets, pattern_sets=None, set_index=None):
         """Device-resident UTF-8 batch -> int64 tensor (n, 3) of (pattern, start, end) in code points, -1 rows where a
         haystack has no match (see _Automaton.first_device)."""
-        return self._ac.first_device(data, offsets, codepoints=True)
+        return self._ac.first_device(data, offsets, codepoints=True, flt=self._device_filter(data, offsets, pattern_sets, set_index))
 
     # ---- additions: match counts per haystack ------------------------------------------------------------------
-    def count_matches(self, haystack: str, overlapping: bool = False) -> int:
+    def count_matches(self, haystack: str, overlapping: bool = False, patterns=None) -> int:
         """-> ``len(find_matches_as_indexes(haystack, overlapping))``, counted without building the list."""
         if not isinstance(haystack, str):
             raise TypeError("argument 'haystack': 'str' expected")
         self._ac.check_overlapping(overlapping)
-        return self._ac.count_host_batch([haystack.encode("utf-8")], overlapping)[0]
+        return self._ac.count_host_batch([haystack.encode("utf-8")], overlapping, _one_set(patterns))[0]
 
-    def count_matches_batch(self, haystacks: Sequence[str], overlapping: bool = False) -> list:
+    def count_matches_batch(self, haystacks: Sequence[str], overlapping: bool = False, patterns=None) -> list:
         """``count_matches`` for each haystack, in one transfer and one scan."""
         hays = list(haystacks)
         for h in hays:
             if not isinstance(h, str):
                 raise TypeError("argument 'haystack': 'str' expected")
         self._ac.check_overlapping(overlapping)
-        return self._ac.count_host_batch([h.encode("utf-8") for h in hays], overlapping)
+        return self._ac.count_host_batch([h.encode("utf-8") for h in hays], overlapping, _batch_sets(patterns, len(hays)))
 
-    def count_matches_device(self, data, offsets, overlapping: bool = False):
+    def count_matches_device(self, data, offsets, overlapping: bool = False, pattern_sets=None, set_index=None):
         """Device-resident UTF-8 batch -> int64 tensor (n,) of match counts (see _Automaton.count_device)."""
-        return self._ac.count_device(data, offsets, overlapping)
+        self._ac.check_overlapping(overlapping)
+        return self._ac.count_device(data, offsets, overlapping, flt=self._device_filter(data, offsets, pattern_sets, set_index))
 
     def count_matches_by_pattern(self, haystack: str, overlapping: bool = False) -> list:
         """-> list of length ``len(patterns)``: entry i is how many of ``find_matches_as_indexes(haystack,
@@ -2123,29 +2317,33 @@ class AhoCorasick:
         stream (it may cut a character); positions are code point indexes (see StreamBatch)."""
         return StreamBatch(self._ac, n_streams, overlapping, codepoints=True)
 
-    def is_match_stream_batch(self, n_streams: int) -> IsMatchStreamBatch:
+    def is_match_stream_batch(self, n_streams: int, pattern_sets=None, set_index=None) -> IsMatchStreamBatch:
         """``n_streams`` is_match streams fed from the device: ``feed_device(data, offsets, last=None)`` -> bool CUDA
-        tensor (n,), is_match of each stream's concatenation so far (see IsMatchStreamBatch)."""
-        return _query_stream_batch(self._ac, "is_match", n_streams, False, codepoints=True)
+        tensor (n,), is_match of each stream's concatenation so far (see IsMatchStreamBatch).  pattern_sets= /
+        set_index= (n_streams,): stream i searches only for the patterns of set set_index[i], for its whole life."""
+        return _query_stream_batch(self._ac, "is_match", n_streams, False, codepoints=True, pattern_sets=pattern_sets, set_index=set_index)
 
-    def find_first_stream_batch(self, n_streams: int) -> FindFirstStreamBatch:
+    def find_first_stream_batch(self, n_streams: int, pattern_sets=None, set_index=None) -> FindFirstStreamBatch:
         """``n_streams`` find_first streams fed from the device: ``feed_device(data, offsets, last=None)`` -> int64 CUDA
-        tensor (n, 3), each stream's first match once final, -1 rows while unknown (see FindFirstStreamBatch)."""
-        return _query_stream_batch(self._ac, "find_first", n_streams, False, codepoints=True)
+        tensor (n, 3), each stream's first match once final, -1 rows while unknown (see FindFirstStreamBatch).
+        pattern_sets= / set_index=: as for is_match_stream_batch."""
+        return _query_stream_batch(self._ac, "find_first", n_streams, False, codepoints=True, pattern_sets=pattern_sets,
+                                   set_index=set_index)
 
     def count_matches_stream_batch(self, n_streams: int, overlapping: bool = False) -> CountStreamBatch:
         """``n_streams`` count streams fed from the device: ``feed_device(data, offsets, last=None)`` -> int64 CUDA tensor
         (n,), the matches each stream's search has released so far (see CountStreamBatch)."""
         return _query_stream_batch(self._ac, "count", n_streams, overlapping, codepoints=True)
 
-    def is_match_stream(self) -> QueryStream:
-        """One is_match stream: ``feed(chunk)`` and ``finish()`` -> bool, does the concatenation so far contain a pattern."""
-        return _query_stream(self._ac, "is_match", False, codepoints=True)
+    def is_match_stream(self, patterns=None) -> QueryStream:
+        """One is_match stream: ``feed(chunk)`` and ``finish()`` -> bool, does the concatenation so far contain a pattern
+        (of `patterns`, when given)."""
+        return _query_stream(self._ac, "is_match", False, codepoints=True, patterns=patterns)
 
-    def find_first_stream(self) -> QueryStream:
+    def find_first_stream(self, patterns=None) -> QueryStream:
         """One find_first stream: ``feed(chunk)`` and ``finish()`` -> (pattern, start, end) once no later data can change
-        it, else None; ``finish()`` gives the final answer."""
-        return _query_stream(self._ac, "find_first", False, codepoints=True)
+        it, else None; ``finish()`` gives the final answer.  `patterns`: search only for these ids."""
+        return _query_stream(self._ac, "find_first", False, codepoints=True, patterns=patterns)
 
     def count_matches_stream(self, overlapping: bool = False) -> QueryStream:
         """One count stream: ``feed(chunk)`` -> the matches released so far, ``finish()`` -> count_matches of the
@@ -2159,7 +2357,7 @@ class AhoCorasick:
         return self._ac.scan_host(data, offsets, overlapping, codepoints=True, **kw)
 
 
-class BytesAhoCorasick:
+class BytesAhoCorasick(_PatternSetMethods):
     """Search for multiple pattern bytes against a bytes-like haystack
     (reference: src/lib.rs:342-363, 366-435).  No references to the patterns are kept."""
 
@@ -2177,67 +2375,75 @@ class BytesAhoCorasick:
             encoded.append(b)
         self._ac = _Automaton(encoded, matchkind, implementation)
 
-    def find_matches_as_indexes(self, haystack, overlapping: bool = False):
-        """-> list of (pattern index, start, end) in byte offsets (src/lib.rs:422-434)."""
+    def find_matches_as_indexes(self, haystack, overlapping: bool = False, patterns=None):
+        """-> list of (pattern index, start, end) in byte offsets (src/lib.rs:422-434).  `patterns`: search only for
+        these pattern ids (as an automaton of those patterns would; ids stay the full automaton's)."""
         hay = _as_buffer_bytes(haystack)
         self._ac.check_overlapping(overlapping)
-        m, _ = self._ac.scan_host_batch([hay], overlapping, codepoints=False)
+        m, _ = self._ac.scan_host_batch([hay], overlapping, codepoints=False, patterns=_one_set(patterns))
         return _tuples(m)
 
-    def find_matches_as_indexes_batch(self, haystacks: Sequence, overlapping: bool = False):
+    def find_matches_as_indexes_batch(self, haystacks: Sequence, overlapping: bool = False, patterns=None):
         self._ac.check_overlapping(overlapping)
-        m, offs = self._ac.scan_host_batch([_as_buffer_bytes(h) for h in haystacks], overlapping, codepoints=False)
+        m, offs = self._ac.scan_host_batch([_as_buffer_bytes(h) for h in haystacks], overlapping, codepoints=False,
+                                           patterns=_batch_sets(patterns, len(haystacks)))
         t = _tuples(m)
         return [t[offs[i]:offs[i + 1]] for i in range(len(haystacks))]
 
-    def scan_device(self, data, offsets, overlapping: bool = False, **kw):
-        """Device-resident batch -> (matches, match_offsets, total); byte offsets."""
-        return self._ac.scan_device(data, offsets, overlapping, codepoints=False, **kw)
+    def scan_device(self, data, offsets, overlapping: bool = False, pattern_sets=None, set_index=None, **kw):
+        """Device-resident batch -> (matches, match_offsets, total); byte offsets.  pattern_sets= / set_index=:
+        haystack i searches only for the patterns of set set_index[i]."""
+        self._ac.check_overlapping(overlapping)
+        return self._ac.scan_device(data, offsets, overlapping, codepoints=False,
+                                    flt=self._device_filter(data, offsets, pattern_sets, set_index), **kw)
 
     # ---- additions: yes / no per haystack (the crate's AhoCorasick::is_match) ------------------------------
-    def is_match(self, haystack) -> bool:
+    def is_match(self, haystack, patterns=None) -> bool:
         """Does any pattern occur in `haystack` (a bytes-like object)?  The same for every match kind."""
-        return self._ac.any_host_batch([_as_buffer_bytes(haystack)])[0]
+        return self._ac.any_host_batch([_as_buffer_bytes(haystack)], _one_set(patterns))[0]
 
-    def is_match_batch(self, haystacks: Sequence) -> list:
+    def is_match_batch(self, haystacks: Sequence, patterns=None) -> list:
         """``is_match`` for each haystack, in one transfer and one scan."""
-        return self._ac.any_host_batch([_as_buffer_bytes(h) for h in haystacks])
+        hays = [_as_buffer_bytes(h) for h in haystacks]
+        return self._ac.any_host_batch(hays, _batch_sets(patterns, len(hays)))
 
-    def is_match_device(self, data, offsets, out=None, sync: bool = True):
+    def is_match_device(self, data, offsets, out=None, sync: bool = True, pattern_sets=None, set_index=None):
         """Device-resident batch -> bool tensor (n,) on its device (see _Automaton.any_device)."""
-        return self._ac.any_device(data, offsets, out, sync)
+        return self._ac.any_device(data, offsets, out, sync, flt=self._device_filter(data, offsets, pattern_sets, set_index))
 
     # ---- additions: the first match per haystack (the crate's AhoCorasick::find) ---------------------------------
-    def find_first(self, haystack):
+    def find_first(self, haystack, patterns=None):
         """-> (pattern index, start, end) in bytes, or None: ``find_matches_as_indexes(haystack)[0]``, found without
         the rest of the list."""
-        return self._ac.first_host_batch([_as_buffer_bytes(haystack)], codepoints=False)[0]
+        return self._ac.first_host_batch([_as_buffer_bytes(haystack)], codepoints=False, patterns=_one_set(patterns))[0]
 
-    def find_first_batch(self, haystacks: Sequence) -> list:
+    def find_first_batch(self, haystacks: Sequence, patterns=None) -> list:
         """``find_first`` for each haystack, in one transfer and one scan."""
-        return self._ac.first_host_batch([_as_buffer_bytes(h) for h in haystacks], codepoints=False)
+        hays = [_as_buffer_bytes(h) for h in haystacks]
+        return self._ac.first_host_batch(hays, codepoints=False, patterns=_batch_sets(patterns, len(hays)))
 
-    def find_first_device(self, data, offsets):
+    def find_first_device(self, data, offsets, pattern_sets=None, set_index=None):
         """Device-resident batch -> int64 tensor (n, 3) of (pattern, start, end) in bytes, -1 rows where a haystack has
         no match (see _Automaton.first_device)."""
-        return self._ac.first_device(data, offsets, codepoints=False)
+        return self._ac.first_device(data, offsets, codepoints=False, flt=self._device_filter(data, offsets, pattern_sets, set_index))
 
     # ---- additions: match counts per haystack ------------------------------------------------------------------
-    def count_matches(self, haystack, overlapping: bool = False) -> int:
+    def count_matches(self, haystack, overlapping: bool = False, patterns=None) -> int:
         """-> ``len(find_matches_as_indexes(haystack, overlapping))``, counted without building the list."""
         hay = _as_buffer_bytes(haystack)
         self._ac.check_overlapping(overlapping)
-        return self._ac.count_host_batch([hay], overlapping)[0]
+        return self._ac.count_host_batch([hay], overlapping, _one_set(patterns))[0]
 
-    def count_matches_batch(self, haystacks: Sequence, overlapping: bool = False) -> list:
+    def count_matches_batch(self, haystacks: Sequence, overlapping: bool = False, patterns=None) -> list:
         """``count_matches`` for each haystack, in one transfer and one scan."""
         hays = [_as_buffer_bytes(h) for h in haystacks]
         self._ac.check_overlapping(overlapping)
-        return self._ac.count_host_batch(hays, overlapping)
+        return self._ac.count_host_batch(hays, overlapping, _batch_sets(patterns, len(hays)))
 
-    def count_matches_device(self, data, offsets, overlapping: bool = False):
+    def count_matches_device(self, data, offsets, overlapping: bool = False, pattern_sets=None, set_index=None):
         """Device-resident batch -> int64 tensor (n,) of match counts (see _Automaton.count_device)."""
-        return self._ac.count_device(data, offsets, overlapping)
+        self._ac.check_overlapping(overlapping)
+        return self._ac.count_device(data, offsets, overlapping, flt=self._device_filter(data, offsets, pattern_sets, set_index))
 
     def count_matches_by_pattern(self, haystack, overlapping: bool = False) -> list:
         """-> list of length ``len(patterns)``: entry i is how many of ``find_matches_as_indexes(haystack,
@@ -2289,29 +2495,33 @@ class BytesAhoCorasick:
         stream; positions are byte offsets (see StreamBatch)."""
         return StreamBatch(self._ac, n_streams, overlapping, codepoints=False)
 
-    def is_match_stream_batch(self, n_streams: int) -> IsMatchStreamBatch:
+    def is_match_stream_batch(self, n_streams: int, pattern_sets=None, set_index=None) -> IsMatchStreamBatch:
         """``n_streams`` is_match streams fed from the device: ``feed_device(data, offsets, last=None)`` -> bool CUDA
-        tensor (n,), is_match of each stream's concatenation so far (see IsMatchStreamBatch)."""
-        return _query_stream_batch(self._ac, "is_match", n_streams, False, codepoints=False)
+        tensor (n,), is_match of each stream's concatenation so far (see IsMatchStreamBatch).  pattern_sets= /
+        set_index= (n_streams,): stream i searches only for the patterns of set set_index[i], for its whole life."""
+        return _query_stream_batch(self._ac, "is_match", n_streams, False, codepoints=False, pattern_sets=pattern_sets, set_index=set_index)
 
-    def find_first_stream_batch(self, n_streams: int) -> FindFirstStreamBatch:
+    def find_first_stream_batch(self, n_streams: int, pattern_sets=None, set_index=None) -> FindFirstStreamBatch:
         """``n_streams`` find_first streams fed from the device: ``feed_device(data, offsets, last=None)`` -> int64 CUDA
-        tensor (n, 3), each stream's first match once final, -1 rows while unknown (see FindFirstStreamBatch)."""
-        return _query_stream_batch(self._ac, "find_first", n_streams, False, codepoints=False)
+        tensor (n, 3), each stream's first match once final, -1 rows while unknown (see FindFirstStreamBatch).
+        pattern_sets= / set_index=: as for is_match_stream_batch."""
+        return _query_stream_batch(self._ac, "find_first", n_streams, False, codepoints=False, pattern_sets=pattern_sets,
+                                   set_index=set_index)
 
     def count_matches_stream_batch(self, n_streams: int, overlapping: bool = False) -> CountStreamBatch:
         """``n_streams`` count streams fed from the device: ``feed_device(data, offsets, last=None)`` -> int64 CUDA tensor
         (n,), the matches each stream's search has released so far (see CountStreamBatch)."""
         return _query_stream_batch(self._ac, "count", n_streams, overlapping, codepoints=False)
 
-    def is_match_stream(self) -> QueryStream:
-        """One is_match stream: ``feed(chunk)`` and ``finish()`` -> bool, does the concatenation so far contain a pattern."""
-        return _query_stream(self._ac, "is_match", False, codepoints=False)
+    def is_match_stream(self, patterns=None) -> QueryStream:
+        """One is_match stream: ``feed(chunk)`` and ``finish()`` -> bool, does the concatenation so far contain a pattern
+        (of `patterns`, when given)."""
+        return _query_stream(self._ac, "is_match", False, codepoints=False, patterns=patterns)
 
-    def find_first_stream(self) -> QueryStream:
+    def find_first_stream(self, patterns=None) -> QueryStream:
         """One find_first stream: ``feed(chunk)`` and ``finish()`` -> (pattern, start, end) once no later data can change
-        it, else None; ``finish()`` gives the final answer."""
-        return _query_stream(self._ac, "find_first", False, codepoints=False)
+        it, else None; ``finish()`` gives the final answer.  `patterns`: search only for these ids."""
+        return _query_stream(self._ac, "find_first", False, codepoints=False, patterns=patterns)
 
     def count_matches_stream(self, overlapping: bool = False) -> QueryStream:
         """One count stream: ``feed(chunk)`` -> the matches released so far, ``finish()`` -> count_matches of the
@@ -2527,7 +2737,7 @@ def _token_tuples(m: np.ndarray):
     return list(zip(m[:, 1].tolist(), (m[:, 2] // _capi.ACB_TOKEN_BYTES).tolist(), (m[:, 3] // _capi.ACB_TOKEN_BYTES).tolist()))
 
 
-class TokenAhoCorasick:
+class TokenAhoCorasick(_PatternSetMethods):
     """Search for multiple token-id sequences against token-id sequences: tokenized corpora (uint16 / int32 arrays),
     generation outputs (int64 tensors).  Positions are token indexes; everything else is BytesAhoCorasick's.
 
@@ -2577,33 +2787,40 @@ class TokenAhoCorasick:
         return out
 
     # ---- the match list ----------------------------------------------------------------------------------------------
-    def find_matches_as_indexes(self, haystack, overlapping: bool = False):
-        """-> list of (pattern index, start, end) in token indexes."""
+    def _token_filter(self, tokens, offsets, pattern_sets, set_index):
+        if pattern_sets is None and set_index is None:
+            return None
+        n = (offsets.numel() if hasattr(offsets, "numel") else len(offsets)) - 1
+        return _filter_args(self._ac, pattern_sets, set_index, n, tokens.device if hasattr(tokens, "device") else None)
+
+    def find_matches_as_indexes(self, haystack, overlapping: bool = False, patterns=None):
+        """-> list of (pattern index, start, end) in token indexes.  `patterns`: search only for these pattern ids."""
         hay = _encode_host_tokens(haystack, "haystack")
         self._ac.check_overlapping(overlapping)
-        m, _ = self._ac.scan_host_batch([hay], overlapping, codepoints=False)
+        m, _ = self._ac.scan_host_batch([hay], overlapping, codepoints=False, patterns=_one_set(patterns))
         return _token_tuples(m)
 
-    def find_matches_as_indexes_batch(self, haystacks: Sequence, overlapping: bool = False):
+    def find_matches_as_indexes_batch(self, haystacks: Sequence, overlapping: bool = False, patterns=None):
         """One list of (pattern, start, end) per haystack, each what ``find_matches_as_indexes`` returns for it."""
         hays = self._hays(haystacks)
         self._ac.check_overlapping(overlapping)
-        m, offs = self._ac.scan_host_batch(hays, overlapping, codepoints=False)
+        m, offs = self._ac.scan_host_batch(hays, overlapping, codepoints=False, patterns=_batch_sets(patterns, len(hays)))
         t = _token_tuples(m)
         return [t[offs[i]:offs[i + 1]] for i in range(len(hays))]
 
-    def scan_device(self, tokens, offsets, overlapping: bool = False, capacity: Optional[int] = None):
+    def scan_device(self, tokens, offsets, overlapping: bool = False, capacity: Optional[int] = None, pattern_sets=None, set_index=None):
         """Device-resident batch of ids (1-D uint16 / int32 / int64 CUDA tensor, int64 offsets (n + 1) in tokens) ->
         (matches, match_offsets, total) as BytesAhoCorasick.scan_device returns them (int32 rows, int64 above
         WINDOW_BYTES encoded bytes), positions in tokens.  The tensors are the caller's own, not workspace views."""
         self._ac.check_overlapping(overlapping)
         torch = _torch()
+        flt = self._token_filter(tokens, offsets, pattern_sets, set_index)
 
         def query(data, offs):
             # the automaton's scan_device returns views of its workspace slot 0: the copies are enqueued under its
             # lock, and the next scan on that slot (any thread, any stream) waits for them, as first_device's gather
             with self._ac._lock:
-                m, mo, total = self._ac.scan_device(data, offs, overlapping, codepoints=False, capacity=capacity)
+                m, mo, total = self._ac.scan_device(data, offs, overlapping, codepoints=False, capacity=capacity, flt=flt)
                 out = _token_rows(m, slice(2, 4)), mo.clone(), total
                 ws = self._ac._ws.get((data.device.index, 0))
                 if ws is not None:
@@ -2614,43 +2831,48 @@ class TokenAhoCorasick:
         return self._on_device(query, tokens, offsets)
 
     # ---- queries -----------------------------------------------------------------------------------------------------
-    def is_match(self, haystack) -> bool:
+    def is_match(self, haystack, patterns=None) -> bool:
         """Does any pattern occur in `haystack`?  The same for every match kind."""
-        return self._ac.any_host_batch(self._hays([haystack]))[0]
+        return self._ac.any_host_batch(self._hays([haystack]), _one_set(patterns))[0]
 
-    def is_match_batch(self, haystacks: Sequence) -> list:
-        return self._ac.any_host_batch(self._hays(haystacks))
+    def is_match_batch(self, haystacks: Sequence, patterns=None) -> list:
+        hays = self._hays(haystacks)
+        return self._ac.any_host_batch(hays, _batch_sets(patterns, len(hays)))
 
-    def is_match_device(self, tokens, offsets):
+    def is_match_device(self, tokens, offsets, pattern_sets=None, set_index=None):
         """Device-resident batch of ids -> bool tensor (n,) (see _Automaton.any_device)."""
-        return self._on_device(lambda d, o: self._ac.any_device(d, o), tokens, offsets)
+        flt = self._token_filter(tokens, offsets, pattern_sets, set_index)
+        return self._on_device(lambda d, o: self._ac.any_device(d, o, flt=flt), tokens, offsets)
 
-    def find_first(self, haystack):
+    def find_first(self, haystack, patterns=None):
         """-> (pattern index, start, end) in token indexes, or None: ``find_matches_as_indexes(haystack)[0]``."""
-        return self.find_first_batch([haystack])[0]
+        return self.find_first_batch([haystack], _one_set(patterns))[0]
 
-    def find_first_batch(self, haystacks: Sequence) -> list:
-        rows = self._ac.first_host_batch(self._hays(haystacks), codepoints=False)
+    def find_first_batch(self, haystacks: Sequence, patterns=None) -> list:
+        hays = self._hays(haystacks)
+        rows = self._ac.first_host_batch(hays, codepoints=False, patterns=_batch_sets(patterns, len(hays)))
         return [_token_first_answer(r) if r is not None else None for r in rows]
 
-    def find_first_device(self, tokens, offsets):
+    def find_first_device(self, tokens, offsets, pattern_sets=None, set_index=None):
         """Device-resident batch of ids -> int64 tensor (n, 3) of (pattern, start, end) in tokens, -1 rows where a
         haystack has no match (see _Automaton.first_device)."""
-        return self._on_device(lambda d, o: _token_rows(self._ac.first_device(d, o), slice(1, 3)), tokens, offsets)
+        flt = self._token_filter(tokens, offsets, pattern_sets, set_index)
+        return self._on_device(lambda d, o: _token_rows(self._ac.first_device(d, o, flt=flt), slice(1, 3)), tokens, offsets)
 
-    def count_matches(self, haystack, overlapping: bool = False) -> int:
+    def count_matches(self, haystack, overlapping: bool = False, patterns=None) -> int:
         """-> ``len(find_matches_as_indexes(haystack, overlapping))``, counted without building the list."""
-        return self.count_matches_batch([haystack], overlapping)[0]
+        return self.count_matches_batch([haystack], overlapping, _one_set(patterns))[0]
 
-    def count_matches_batch(self, haystacks: Sequence, overlapping: bool = False) -> list:
+    def count_matches_batch(self, haystacks: Sequence, overlapping: bool = False, patterns=None) -> list:
         hays = self._hays(haystacks)
         self._ac.check_overlapping(overlapping)
-        return self._ac.count_host_batch(hays, overlapping)
+        return self._ac.count_host_batch(hays, overlapping, _batch_sets(patterns, len(hays)))
 
-    def count_matches_device(self, tokens, offsets, overlapping: bool = False):
+    def count_matches_device(self, tokens, offsets, overlapping: bool = False, pattern_sets=None, set_index=None):
         """Device-resident batch of ids -> int64 tensor (n,) of match counts (see _Automaton.count_device)."""
         self._ac.check_overlapping(overlapping)
-        return self._on_device(lambda d, o: self._ac.count_device(d, o, overlapping), tokens, offsets)
+        flt = self._token_filter(tokens, offsets, pattern_sets, set_index)
+        return self._on_device(lambda d, o: self._ac.count_device(d, o, overlapping, flt=flt), tokens, offsets)
 
     def count_matches_by_pattern(self, haystack, overlapping: bool = False) -> list:
         """-> entry i is how many of ``find_matches_as_indexes(haystack, overlapping)`` have pattern i."""
@@ -2695,34 +2917,43 @@ class TokenAhoCorasick:
         return TokenStreamBatch(StreamBatch(self._ac, n_streams, overlapping, codepoints=False),
                                 lambda r: (_token_rows(r[0], slice(2, 4)), r[1]))
 
-    def _query_batch(self, kind, n_streams, overlapping):
+    def _query_batch(self, kind, n_streams, overlapping, pattern_sets=None, set_index=None):
         _token_stream_limits(self._ac, n_streams)
         convert = (lambda rows: _token_rows(rows, slice(1, 3))) if kind == "find_first" else _same
-        return TokenStreamBatch(_query_stream_batch(self._ac, kind, n_streams, overlapping, codepoints=False), convert)
+        return TokenStreamBatch(_query_stream_batch(self._ac, kind, n_streams, overlapping, codepoints=False, pattern_sets=pattern_sets,
+                                                    set_index=set_index), convert)
 
-    def _query_stream(self, kind, overlapping):
+    def _query_stream(self, kind, overlapping, patterns=None):
         _token_stream_limits(self._ac, 1)
         answer = {"is_match": bool, "find_first": _token_first_answer, "count": int}[kind]
-        return TokenStream(QueryStream(_query_stream_batch(self._ac, kind, 1, overlapping, codepoints=False), answer), _same)
+        if patterns is None:
+            return TokenStream(QueryStream(_query_stream_batch(self._ac, kind, 1, overlapping, codepoints=False), answer), _same)
+        torch = _require_cuda()
+        ps = self.pattern_sets([patterns])
+        batch = _query_stream_batch(self._ac, kind, 1, overlapping, codepoints=False, pattern_sets=ps,
+                                    set_index=torch.zeros(1, dtype=torch.int32, device=ps.device))
+        return TokenStream(QueryStream(batch, answer), _same)
 
-    def is_match_stream_batch(self, n_streams: int) -> TokenStreamBatch:
-        """``feed_device`` -> bool CUDA tensor (n,), is_match of each stream so far (see IsMatchStreamBatch)."""
-        return self._query_batch("is_match", n_streams, False)
+    def is_match_stream_batch(self, n_streams: int, pattern_sets=None, set_index=None) -> TokenStreamBatch:
+        """``feed_device`` -> bool CUDA tensor (n,), is_match of each stream so far (see IsMatchStreamBatch);
+        pattern_sets= / set_index= (n_streams,) fix each stream's pattern set."""
+        return self._query_batch("is_match", n_streams, False, pattern_sets, set_index)
 
-    def find_first_stream_batch(self, n_streams: int) -> TokenStreamBatch:
+    def find_first_stream_batch(self, n_streams: int, pattern_sets=None, set_index=None) -> TokenStreamBatch:
         """``feed_device`` -> int64 CUDA tensor (n, 3), each stream's first match in tokens once final, -1 rows while
-        unknown (see FindFirstStreamBatch)."""
-        return self._query_batch("find_first", n_streams, False)
+        unknown (see FindFirstStreamBatch); pattern_sets= / set_index= (n_streams,) fix each stream's pattern set
+        (per-request stop sequences in batched generation)."""
+        return self._query_batch("find_first", n_streams, False, pattern_sets, set_index)
 
     def count_matches_stream_batch(self, n_streams: int, overlapping: bool = False) -> TokenStreamBatch:
         """``feed_device`` -> int64 CUDA tensor (n,), the matches each stream's search has released (see CountStreamBatch)."""
         return self._query_batch("count", n_streams, overlapping)
 
-    def is_match_stream(self) -> TokenStream:
-        return self._query_stream("is_match", False)
+    def is_match_stream(self, patterns=None) -> TokenStream:
+        return self._query_stream("is_match", False, patterns)
 
-    def find_first_stream(self) -> TokenStream:
-        return self._query_stream("find_first", False)
+    def find_first_stream(self, patterns=None) -> TokenStream:
+        return self._query_stream("find_first", False, patterns)
 
     def count_matches_stream(self, overlapping: bool = False) -> TokenStream:
         self._ac.check_overlapping(overlapping)

@@ -553,6 +553,53 @@ int acb_stream_count(const acb_automaton *a, const uint8_t *dev_bytes, const int
  * Both return ACB_EINVAL, before any CUDA call, for a token_bytes other than 2, 4 or 8, n_tokens >= 2^60 or a null
  * pointer (the ids and the output may be null when n_tokens == 0).
  */
+/*
+ * Pattern sets: each haystack (or stream) searches for its own subset of the automaton's patterns.  For haystack h with
+ * set S, every covered query returns exactly what it would return from an automaton built from only the patterns in S,
+ * with the same match kind and in the same relative order (LeftmostFirst priority is kept), reporting ids of the FULL
+ * automaton.  The descriptor:
+ *   dev_set_bits   u32[n_sets][words_per_set], words_per_set = ceil(n_patterns / 32): bit p % 32 of word p / 32 of
+ *                  row s = pattern p is in set s
+ *   dev_set_index  int32 (index_bytes 4) or int64 (8) [n_haystacks]: haystack h uses row dev_set_index[h]; an index
+ *                  outside [0, n_sets) admits no pattern (the kernels never read outside the bitset)
+ * The *_filtered entry points take it as their last argument before `stream` and are otherwise the calls they are
+ * named after; a NULL filter is exactly that call.  A filtered call always runs the sieve (the table images hold every
+ * pattern): acb_scan_batch_filtered takes kernel 5 whatever the tuning and needs dev_sieve.  acb_first_rows_filtered
+ * must get the filter its keys were found with (the node's lowest ADMITTED pid is reported), and
+ * acb_stream_first_resolve_filtered passes it on to the two acb_first_rows calls it makes.  ACB_EINVAL, before any
+ * device work: n_sets == 0, a null dev_set_bits, a null dev_set_index with n_haystacks > 0, index_bytes not 4 or 8.
+ * (The is_match stream needs no filtered resolve: it is acb_any_match_filtered on the seams and the chunks.)
+ */
+typedef struct acb_pattern_filter {
+    const uint32_t *dev_set_bits;
+    uint64_t n_sets;
+    const void *dev_set_index;
+    int index_bytes;
+} acb_pattern_filter;
+int acb_scan_batch_filtered(const acb_automaton *a, const void *dev_image, const void *dev_hot, const acb_hot_desc *hot_desc,
+                            const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets, int64_t n_haystacks,
+                            uint64_t total_bytes, int overlapping, int codepoints, const acb_plan *plan, const acb_workspace *ws,
+                            const acb_pattern_filter *filter, void *stream);
+int acb_any_match_filtered(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                           int64_t n_haystacks, uint64_t total_bytes, uint8_t *dev_flags, uint64_t *dev_scratch,
+                           const acb_pattern_filter *filter, void *stream);
+int acb_find_first_filtered(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                            int64_t n_haystacks, uint64_t total_bytes, uint64_t *dev_keys, uint64_t *dev_scratch,
+                            const acb_pattern_filter *filter, void *stream);
+int acb_first_rows_filtered(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                            int64_t n_haystacks, const uint64_t *dev_keys, int64_t *dev_rows, const acb_pattern_filter *filter, void *stream);
+int acb_count_overlapping_filtered(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                                   int64_t n_haystacks, uint64_t total_bytes, uint64_t *dev_counts, uint64_t *dev_scratch,
+                                   const acb_pattern_filter *filter, void *stream);
+int acb_count_non_overlapping_filtered(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                                       int64_t n_haystacks, uint64_t total_bytes, const acb_plan *plan, const acb_workspace *ws,
+                                       uint64_t *dev_counts, const acb_pattern_filter *filter, void *stream);
+int acb_stream_first_resolve_filtered(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                                      int64_t n_streams, uint64_t total_bytes, const uint8_t *dev_last, int codepoints, const int64_t *dev_carry,
+                                      const uint8_t *dev_seam_bytes, const int64_t *dev_seam_offsets, uint64_t seam_buffer_bytes,
+                                      uint64_t *dev_seam_keys, uint64_t *dev_chunk_keys, int64_t *dev_best, int64_t *dev_scratch,
+                                      int64_t *dev_rows, const acb_pattern_filter *filter, void *stream);
+
 #define ACB_TOKEN_ID_LIMIT (1u << 21)
 #define ACB_TOKEN_BYTES 3
 int acb_tokens_encode(const void *dev_tokens, int token_bytes, uint64_t n_tokens, uint8_t *dev_out, uint64_t *dev_bad, void *stream);
