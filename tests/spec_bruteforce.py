@@ -8,6 +8,10 @@ Let O = all occurrences (pid, a, e) with haystack[a:e] == patterns[pid]
 * non-overlapping: s = 0; repeat: among occurrences with a >= s take the
   minimum of  Standard (e, a, pid) | LeftmostFirst (a, pid) |
   LeftmostLongest (a, -e, pid); emit; s = e.
+
+* pattern sets: an automaton of only the patterns in S, in their original
+  relative order, with the full list's ids = the same rules over the
+  occurrences of the pids in S.
 """
 
 
@@ -22,9 +26,11 @@ def occurrences(patterns, haystack):
     return occ
 
 
-def spec_find(patterns, haystack, kind="Standard", overlapping=False):
-    """patterns/haystack: bytes (or str, for code point semantics). -> [(pid, a, e)]"""
+def spec_find(patterns, haystack, kind="Standard", overlapping=False, admitted=None):
+    """patterns/haystack: bytes (or str, for code point semantics); admitted: a set of pids (None: all). -> [(pid, a, e)]"""
     occ = occurrences(patterns, haystack)
+    if admitted is not None:
+        occ = [m for m in occ if m[0] in admitted]
     if overlapping:
         if kind != "Standard":
             raise ValueError(f"match kind {kind} does not support overlapping searches")

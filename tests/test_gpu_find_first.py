@@ -16,6 +16,7 @@ from ahocorasick_rs_b200 import workloads as W  # noqa: E402
 from oracle import Oracle  # noqa: E402
 
 from .gpu_helpers import KINDS, dev, dev_at, forced  # noqa: E402
+from .sieve_geometry_helpers import predicted_first_skips  # noqa: E402
 
 ENGINES = ["sieve", "sieve-small-tasks", "staged"]   # the first-match kernel with 16 KiB and 512-byte tasks, the table composition
 KIND_IDS = ["Standard", "LeftmostFirst", "LeftmostLongest"]
@@ -217,37 +218,6 @@ def test_utf8_str_haystacks(variant):
 
 
 # ---------------------------------------------------------------- skip counters and early exit
-def predicted_skips(ptr, offs, key_hi, T, kind, max_len):
-    """tasks skipped whole and windows not scanned, from the task grid (see acb_find_first in include/acb200.h), for
-    keys that do not change during the call (key_hi: the high words, 0xffffffff where there is no match)."""
-    origin = -(ptr & 511)
-    total = int(offs[-1])
-    n_tasks = (total - origin + T - 1) // T
-    tasks = windows = 0
-    for k in range(n_tasks):
-        t_lo = origin + k * T
-        lo, hi = max(t_lo, 0), min(t_lo + T, total)
-        if lo >= hi:
-            continue
-        tail = int(np.searchsorted(offs, hi - 1, side="right")) - 1
-        tail_s = int(offs[tail]) - t_lo
-        lo_r, hi_r = lo - t_lo, hi - t_lo
-
-        def cannot_win(rel):
-            e = rel - tail_s + 1
-            return (e if kind == MatchKind.Standard else max(e - max_len, 0)) > int(key_hi[tail])
-
-        if tail_s <= lo_r and cannot_win(lo_r):
-            tasks += 1
-            continue
-        wfirst, wlast = lo_r & ~511, (hi_r - 1) & ~511
-        for w in range(wfirst + 512, wlast + 1, 512):
-            if w >= tail_s and cannot_win(w):
-                windows += (wlast - w) // 512 + 1
-                break
-    return tasks, windows
-
-
 @pytest.mark.parametrize("variant", ["sieve", "sieve-small-tasks"])
 @pytest.mark.parametrize("kind", KINDS, ids=KIND_IDS)
 @pytest.mark.parametrize("shift", [0, 188, 511])
@@ -275,7 +245,7 @@ def test_entry_keys_skip_exactly(variant, kind, shift):
         T = ac._ac._plan(d, n).task_bytes
         assert T == (512 if variant == "sieve-small-tasks" else 16384)
         key_hi = keys.cpu().numpy().view(np.uint64) >> np.uint64(32)
-        tasks, windows = predicted_skips(d.data_ptr(), offs, key_hi, T, kind, ac._ac.max_pattern_len)
+        tasks, windows = predicted_first_skips(d.data_ptr(), offs, key_hi, T, kind, ac._ac.max_pattern_len)
         assert (scratch[1], scratch[2]) == (tasks, windows)
         assert tasks > 0
         if shift and T > 512:

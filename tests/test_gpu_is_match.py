@@ -18,6 +18,7 @@ from ahocorasick_rs_b200 import workloads as W  # noqa: E402
 from oracle import Oracle  # noqa: E402
 
 from .gpu_helpers import KINDS, dev, dev_at, forced  # noqa: E402
+from .sieve_geometry_helpers import predicted_any_skips  # noqa: E402
 
 ENGINES = ["sieve", "sieve-small-tasks", "staged"]   # the any-match kernel with 16 KiB and 512-byte tasks, the table composition
 SPEC_BYTES = 8192
@@ -289,34 +290,6 @@ def test_two_threads_on_the_table_walker_path(monkeypatch):
 
 
 # ---------------------------------------------------------------- accumulation and the skip counters
-def predicted_skips(ptr, offs, flags, T):
-    """tasks skipped whole and windows not scanned, from the task grid (see acb_any_match in include/acb200.h), for
-    flags that do not change during the call."""
-    origin = -(ptr & 511)
-    total = int(offs[-1])
-    n_tasks = (total - origin + T - 1) // T
-    tasks = windows = 0
-    for k in range(n_tasks):
-        t_lo = origin + k * T
-        lo, hi = max(t_lo, 0), min(t_lo + T, total)
-        if lo >= hi:
-            continue
-        tail = int(np.searchsorted(offs, hi - 1, side="right")) - 1
-        if not flags[tail]:
-            continue
-        tail_s = int(offs[tail]) - t_lo
-        lo_r, hi_r = lo - t_lo, hi - t_lo
-        if tail_s <= lo_r:
-            tasks += 1
-            continue
-        wfirst, wlast = lo_r & ~511, (hi_r - 1) & ~511
-        for w in range(wfirst + 512, wlast + 1, 512):
-            if w >= tail_s:
-                windows += (wlast - w) // 512 + 1
-                break
-    return tasks, windows
-
-
 @pytest.mark.parametrize("variant", ["sieve", "sieve-small-tasks"])
 @pytest.mark.parametrize("shift", [0, 188, 511])
 def test_preflagged_haystacks_are_skipped_exactly(variant, shift):
@@ -335,7 +308,7 @@ def test_preflagged_haystacks_are_skipped_exactly(variant, shift):
         st = ac._ac.last_stats
         T = st["task_bytes"]
         assert T == (512 if variant == "sieve-small-tasks" else 16384)
-        tasks, windows = predicted_skips(d.data_ptr(), offs, pre, T)
+        tasks, windows = predicted_any_skips(d.data_ptr(), offs, pre, T)
         assert (st["tasks_skipped"], st["windows_skipped"]) == (tasks, windows)
         assert tasks > 0 and st["tasks"] == (n * L + (d.data_ptr() & 511) + T - 1) // T
         if shift and T > 512:

@@ -5,9 +5,6 @@ filter whose primary bitmap is nearly full), and reverse-trie nodes with 1, 8, 9
 runs all four of the kernel's modes -- the match list (three kinds and overlapping), is_match, find_first and the
 counts -- against the CPU oracle, and asserts after every call that last_stats report the geometry it was built for
 (a changed default that stops an input from reaching its corner fails here instead of passing silently)."""
-import contextlib
-import functools
-
 import numpy as np
 import pytest
 
@@ -15,84 +12,21 @@ pytestmark = pytest.mark.gpu
 
 torch = pytest.importorskip("torch")
 
-from ahocorasick_rs_b200 import MatchKind, _capi, matcher  # noqa: E402
+from ahocorasick_rs_b200 import MatchKind, matcher  # noqa: E402
 from oracle import Oracle  # noqa: E402
 
 from .gpu_helpers import KINDS, check_batch, dev, dev_at, make_ac  # noqa: E402
-from .sieve_inputs import FANOUTS, TWO_LEVEL, dense_case, fanout_case, planted_case  # noqa: E402
-from .sieve_interp import SieveImage  # noqa: E402
+from .sieve_geometry_helpers import (assert_geometry, case_inputs, fanout, first_rows_of, geometry, host_geometry,  # noqa: E402
+                                     planted)
+from .sieve_inputs import FANOUTS, TWO_LEVEL  # noqa: E402
 
 RINGS = (1, 2, 4, 8)
 SHIFTS = (0, 1, 511)   # where the data starts after a 512-byte aligned address: moves the window and task grids
 DEFAULT_TASK = 16384
 
 
-@functools.lru_cache(maxsize=None)
-def planted(utf8, decoys=0):
-    return planted_case(utf8, decoys=decoys)
-
-
-@functools.lru_cache(maxsize=None)
-def dense(utf8):
-    return dense_case(utf8)
-
-
-@functools.lru_cache(maxsize=None)
-def fanout(f):
-    return fanout_case(f)
-
-
-@functools.lru_cache(maxsize=None)
-def host_geometry(case, budget, w):
-    """What the builder makes of a case at a filter budget, on the host (tests/sieve_interp.SieveImage: the same C
-    builder) -> (window, last_level, probes, bloom_bytes, primary bitmap fill)."""
-    pats = case_inputs(case)[0]
-    img = SieveImage(pats, 0, budget, w)
-    fill = float(np.unpackbits(img.bloom[:img.prim_words].view(np.uint8)).mean())
-    return img.W, img.last_level, img.n_probes, img.bloom_words * 4, fill
-
-
-def case_inputs(case):
-    name, utf8 = case
-    if name == "dense":
-        return dense(utf8)
-    return planted(utf8, 1000 if name == "decoys" else 0)
-
-
-@contextlib.contextmanager
-def geometry(monkeypatch, w, ring, task_bytes, budget=None):
-    """Sieve scans on this thread with primary window w (automata built inside: the image is built at the first
-    scan), ring depth `ring`, tasks of task_bytes and, when given, filters built for `budget` bytes."""
-    monkeypatch.setattr(matcher._Automaton, "SIEVE_W_MAX", w)
-    if budget is not None:
-        smem = matcher._Automaton._smem_optin(torch.cuda.current_device())
-        monkeypatch.setattr(matcher._Automaton, "SIEVE_SMEM_RESERVE", smem - budget)
-    _capi.set_tuning(5, 0, task_bytes, 0, sieve_ring=ring)
-    try:
-        yield
-    finally:
-        _capi.set_tuning(0)
-
-
-def assert_geometry(ac, want):
-    st = ac._ac.last_stats
-    assert st["engine"] == "sieve", st
-    for k, v in want.items():
-        assert st[k] == v, (k, v, st)
-
-
 def oracle(pats, kind, data, offs, overlapping=False, codepoints=False):
     return Oracle(pats, kind.name).scan_batch(data, offs, overlapping=overlapping, codepoints=codepoints)
-
-
-def first_rows(pats, kind, data, offs, codepoints):
-    """The oracle's first record per haystack, (n, 3) rows with -1 where there is none."""
-    _, counts, rec = oracle(pats, kind, data, offs, codepoints=codepoints)
-    rows = np.full((len(offs) - 1, 3), -1, dtype=np.int64)
-    at = np.concatenate([[0], np.cumsum(counts.astype(np.int64))[:-1]])
-    has = counts > 0
-    rows[has] = rec[at[has]][:, 1:4].astype(np.int64)
-    return rows
 
 
 def check_all_modes(pats, data, offs, want, codepoints=False, shift=0):
@@ -107,7 +41,7 @@ def check_all_modes(pats, data, offs, want, codepoints=False, shift=0):
         assert_geometry(ac, want)
         got = ac.find_first_device(d, o).cpu().numpy()
         assert_geometry(ac, want)
-        assert np.array_equal(got, first_rows(pats, kind, data, offs, codepoints)), kind
+        assert np.array_equal(got, first_rows_of(*oracle(pats, kind, data, offs, codepoints=codepoints)[1:])), kind
         _, counts, _ = oracle(pats, kind, data, offs)
         got = ac.count_matches_device(d, o).cpu().numpy()
         assert_geometry(ac, want)

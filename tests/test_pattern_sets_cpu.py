@@ -11,6 +11,7 @@ import torch
 from ahocorasick_rs_b200 import AhoCorasick, BytesAhoCorasick, MatchKind, TokenAhoCorasick, _capi
 from ahocorasick_rs_b200.matcher import PatternSets, _filter_args
 
+from .sieve_geometry_helpers import subset_scan_batch
 from .sieve_interp import SieveImage
 from .spec_bruteforce import spec_find
 
@@ -237,3 +238,38 @@ def test_model_duplicates_lowest_allowed_id():
     chains = _chain_rows(img, b"zab", 0, 3)
     assert model_first(chains, {2, 1}, "LeftmostFirst") == (1, 1, 3)
     assert model_list(chains, {0, 2}) == [(0, 1, 3), (2, 1, 3)]
+
+
+# ---- subset_scan_batch (the GPU tests' reference) against the brute-force statement --------------------------------
+@pytest.mark.parametrize("codepoints", [False, True], ids=["bytes", "str"])
+@pytest.mark.parametrize("seed", range(4))
+@pytest.mark.parametrize("search", ["Standard", "LeftmostFirst", "LeftmostLongest", "Overlapping"])
+def test_subset_scan_batch_matches_restricted_spec(search, seed, codepoints):
+    """subset_scan_batch groups haystacks by set and scans each group with an oracle of that set's patterns; the
+    semantics is spec_find on the full list with the occurrences restricted to S (the order is kept, so that is all a
+    subset changes).  Duplicates and a nested family; an index outside [0, G) admits nothing."""
+    kind, overlapping = ("Standard", True) if search == "Overlapping" else (search, False)
+    rng = random.Random(100 * seed + len(search) + codepoints)
+    alpha = ["a", "b", "c", "é", "€"] if codepoints else ["a", "b", "c"]
+    pats = ["".join(rng.choice(alpha) for _ in range(rng.randint(1, 5))) for _ in range(14)]
+    pats += [pats[2], pats[2], "abca", "bca", "ca", "a"]   # duplicates, a nested family
+    pb = [p.encode() for p in pats]
+    P = len(pats)
+    sets = [[], list(range(P)), [P - 3, P - 1], [3, 2, 15]] + [[p for p in range(P) if rng.random() < f] for f in (0.2, 0.6)]
+    hays = ["".join(rng.choice(alpha) for _ in range(rng.choice([0, 1, 7, 40, 120]))) for _ in range(30)]
+    idx = [rng.randrange(-1, len(sets) + 1) for _ in hays]
+    data = np.frombuffer("".join(hays).encode() or b"\0", dtype=np.uint8)[:len("".join(hays).encode())]
+    offs = np.zeros(len(hays) + 1, dtype=np.int64)
+    np.cumsum([len(h.encode()) for h in hays], out=offs[1:])
+    total, counts, rec = subset_scan_batch(pb, kind, data, offs, sets, idx, overlapping, codepoints)
+    assert rec.dtype == np.uint32 and rec.shape == (total, 4) and int(counts.sum()) == total
+    want_total = 0
+    for h, hay in enumerate(hays):
+        S = set(sets[idx[h]]) if 0 <= idx[h] < len(sets) else set()
+        want = spec_find(pats if codepoints else pb, hay if codepoints else hay.encode(), kind, overlapping, admitted=S)
+        got = [tuple(int(x) for x in r[1:]) for r in rec[rec[:, 0] == h]]
+        assert got == want, (h, S)
+        assert counts[h] == len(want)
+        want_total += len(want)
+    assert want_total == total and want_total > 0
+    assert np.array_equal(rec[:, 0], np.sort(rec[:, 0]))   # haystack order, as Oracle.scan_batch
