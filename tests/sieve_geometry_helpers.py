@@ -1,7 +1,8 @@
 """Helpers shared by the sieve geometry tests and the pattern-set tests: the cached seeded inputs of
 tests/sieve_inputs.py, forcing a sieve geometry (primary window, ring depth, task size, filter budget) and asserting it,
-the skip counters the task grid predicts for is_match and find_first, and `subset_scan_batch`, the CPU reference of a
-batch in which every haystack searches for its own subset of the patterns."""
+the skip counters the task grid predicts for is_match and find_first, `subset_scan_batch`, the CPU reference of a
+batch in which every haystack searches for its own subset of the patterns, and the references of
+count_matches_by_pattern and matching_patterns taken from the oracle's records."""
 import contextlib
 import functools
 
@@ -169,3 +170,38 @@ def first_rows_of(counts, rec):
     has = counts > 0
     rows[has] = rec[at[has]][:, 1:4].astype(np.int64)
     return rows
+
+
+# ---------------------------------------------------------------- count_matches_by_pattern and matching_patterns
+def hist_of(rec, n_patterns):
+    """count_matches_by_pattern from a batch's records -> int64 (n_patterns,): the bincount of the pattern column."""
+    return np.bincount(rec[:, 1].astype(np.int64), minlength=n_patterns)
+
+
+def hits_of(rec, n_haystacks, n_patterns):
+    """matching_patterns from a batch's records -> (row_offsets, patterns, counts) as int64 numpy arrays: each
+    haystack's distinct pattern ids, ascending, and how many of its records have each."""
+    keys, counts = np.unique(rec[:, 0].astype(np.int64) * n_patterns + rec[:, 1].astype(np.int64), return_counts=True)
+    row_offsets = np.searchsorted(keys, np.arange(n_haystacks + 1, dtype=np.int64) * n_patterns)
+    return row_offsets.astype(np.int64), keys % n_patterns, counts.astype(np.int64)
+
+
+def oracle_hist(pats, data, offs, kind, overlapping):
+    _, _, rec = Oracle(pats, kind.value).scan_batch(data, offs, overlapping=overlapping)
+    return hist_of(rec, len(pats))
+
+
+def oracle_hits(pats, data, offs, kind, overlapping):
+    """-> (row_offsets, patterns, counts) as int64 numpy arrays, from the oracle's records."""
+    _, _, rec = Oracle(pats, kind.value).scan_batch(data, offs, overlapping=overlapping)
+    return hits_of(rec, len(offs) - 1, len(pats))
+
+
+def hits_sums(hits, n_haystacks, n_patterns):
+    """The row sums (per haystack) and column sums (per pattern) of a hits triple -> two int64 arrays."""
+    ro, p, c = (np.asarray(t, dtype=np.int64) for t in hits)
+    rows = np.zeros(n_haystacks, dtype=np.int64)
+    np.add.at(rows, np.repeat(np.arange(n_haystacks), np.diff(ro)), c)
+    cols = np.zeros(n_patterns, dtype=np.int64)
+    np.add.at(cols, p, c)
+    return rows, cols

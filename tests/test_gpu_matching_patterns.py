@@ -19,15 +19,8 @@ from ahocorasick_rs_b200 import workloads as W  # noqa: E402
 from oracle import Oracle  # noqa: E402
 
 from .gpu_helpers import KINDS, SEARCH_IDS, SEARCHES, dev, forced  # noqa: E402
+from .sieve_geometry_helpers import oracle_hits  # noqa: E402
 from .test_gpu_count import ENGINES, KIND_IDS, L_STRETCH, VECTORS, batch, stretch_batch  # noqa: E402
-
-
-def oracle_hits(pats, data, offs, kind, overlapping):
-    """-> (row_offsets, patterns, counts) as int64 numpy arrays, from the oracle's records."""
-    _, _, rec = Oracle(pats, kind.value).scan_batch(data, offs, overlapping=overlapping)
-    keys, counts = np.unique(rec[:, 0].astype(np.int64) * len(pats) + rec[:, 1].astype(np.int64), return_counts=True)
-    row_offsets = np.searchsorted(keys, np.arange(len(offs), dtype=np.int64) * len(pats))
-    return row_offsets.astype(np.int64), keys % len(pats), counts.astype(np.int64)
 
 
 def check(pats, data, offs, kind, overlapping=False, ac=None, capacity=None, sums=True):

@@ -17,15 +17,10 @@ torch = pytest.importorskip("torch")
 
 from ahocorasick_rs_b200 import AhoCorasick, BytesAhoCorasick, Implementation, MatchKind, _capi, matcher  # noqa: E402
 from ahocorasick_rs_b200 import workloads as W  # noqa: E402
-from oracle import Oracle  # noqa: E402
 
 from .gpu_helpers import KINDS, SEARCH_IDS, SEARCHES, dev, forced  # noqa: E402
+from .sieve_geometry_helpers import oracle_hist  # noqa: E402
 from .test_gpu_count import ENGINES, KIND_IDS, L_STRETCH, VECTORS, batch, stretch_batch  # noqa: E402
-
-
-def oracle_hist(pats, data, offs, kind, overlapping):
-    _, _, rec = Oracle(pats, kind.value).scan_batch(data, offs, overlapping=overlapping)
-    return np.bincount(rec[:, 1].astype(np.int64), minlength=len(pats))
 
 
 def check(pats, data, offs, kind, overlapping=False, ac=None, capacity=None):

@@ -2,9 +2,10 @@
 primary window W (1..8) against every ring depth R (1, 2, 4, 8 windows of text per warp), 16 KiB and 512-byte tasks,
 code points, the filter budget (default, shallow: nothing on chip beyond the primary window, saturated: a 4 KiB
 filter whose primary bitmap is nearly full), and reverse-trie nodes with 1, 8, 9, 255 and 256 children.  Every case
-runs all four of the kernel's modes -- the match list (three kinds and overlapping), is_match, find_first and the
-counts -- against the CPU oracle, and asserts after every call that last_stats report the geometry it was built for
-(a changed default that stops an input from reaching its corner fails here instead of passing silently)."""
+runs all five of the kernel's modes -- the match list (three kinds and overlapping), is_match, find_first, the counts
+and the per-pattern counts -- and the two epilogues that read the ordered list for count_matches_by_pattern and
+matching_patterns, against the CPU oracle, and asserts after every call that last_stats report the geometry it was
+built for (a changed default that stops an input from reaching its corner fails here instead of passing silently)."""
 import numpy as np
 import pytest
 
@@ -16,8 +17,8 @@ from ahocorasick_rs_b200 import MatchKind, matcher  # noqa: E402
 from oracle import Oracle  # noqa: E402
 
 from .gpu_helpers import KINDS, check_batch, dev, dev_at, make_ac  # noqa: E402
-from .sieve_geometry_helpers import (assert_geometry, case_inputs, fanout, first_rows_of, geometry, host_geometry,  # noqa: E402
-                                     planted)
+from .sieve_geometry_helpers import (assert_geometry, case_inputs, fanout, first_rows_of, geometry, hist_of, hits_of,  # noqa: E402
+                                     hits_sums, host_geometry, planted)
 from .sieve_inputs import FANOUTS, TWO_LEVEL  # noqa: E402
 
 RINGS = (1, 2, 4, 8)
@@ -29,11 +30,30 @@ def oracle(pats, kind, data, offs, overlapping=False, codepoints=False):
     return Oracle(pats, kind.name).scan_batch(data, offs, overlapping=overlapping, codepoints=codepoints)
 
 
+def check_pattern_queries(ac, pats, d, o, want, counts, rec, overlapping=False):
+    """count_matches_by_pattern and matching_patterns of one search against the oracle's records, with the geometry
+    and the mode asserted after each call; the hits' row sums are the per-haystack counts and their column sums the
+    per-pattern counts."""
+    hist = ac.count_matches_by_pattern_device(d, o, overlapping).cpu().numpy()
+    assert_geometry(ac, want)
+    assert ac._ac.last_stats["mode"] == "pattern_counts"
+    assert np.array_equal(hist, hist_of(rec, len(pats))), (ac._ac.matchkind, overlapping)
+    got = [t.cpu().numpy() for t in ac.matching_patterns_device(d, o, overlapping)]
+    assert_geometry(ac, want)
+    assert ac._ac.last_stats["mode"] == "matching_patterns"
+    for t, exp in zip(got, hits_of(rec, len(counts), len(pats))):
+        assert np.array_equal(t, exp), (ac._ac.matchkind, overlapping)
+    rows, cols = hits_sums(got, len(counts), len(pats))
+    assert np.array_equal(rows, counts.astype(np.int64)) and np.array_equal(cols, hist)
+
+
 def check_all_modes(pats, data, offs, want, codepoints=False, shift=0):
-    """The four searches' lists, is_match, find_first for every kind and both counts, each against the oracle, with
-    the geometry asserted after every call.  -> overlapping matches in the batch."""
+    """The four searches' lists, is_match, find_first for every kind, both counts, count_matches_by_pattern (the
+    pattern mode for the overlapping search, the pattern epilogue for the others) and matching_patterns (the hits
+    epilogue), each against the oracle, with the geometry asserted after every call.  -> overlapping matches in the
+    batch."""
     d, o = dev_at(data, shift), dev(offs)
-    over_total, over_counts, _ = oracle(pats, MatchKind.Standard, data, offs, overlapping=True)
+    over_total, over_counts, over_rec = oracle(pats, MatchKind.Standard, data, offs, overlapping=True)
     assert over_total > 0
     for kind in KINDS:
         ac = make_ac(pats, kind, codepoints)
@@ -42,10 +62,11 @@ def check_all_modes(pats, data, offs, want, codepoints=False, shift=0):
         got = ac.find_first_device(d, o).cpu().numpy()
         assert_geometry(ac, want)
         assert np.array_equal(got, first_rows_of(*oracle(pats, kind, data, offs, codepoints=codepoints)[1:])), kind
-        _, counts, _ = oracle(pats, kind, data, offs)
+        _, counts, rec = oracle(pats, kind, data, offs)
         got = ac.count_matches_device(d, o).cpu().numpy()
         assert_geometry(ac, want)
         assert np.array_equal(got, counts.astype(np.int64)), kind
+        check_pattern_queries(ac, pats, d, o, want, counts, rec)
         if kind == MatchKind.Standard:
             check_batch(pats, kind, data, offs, overlapping=True, codepoints=codepoints, ac=ac, shift=shift)
             assert_geometry(ac, want)
@@ -55,6 +76,7 @@ def check_all_modes(pats, data, offs, want, codepoints=False, shift=0):
             got = ac.is_match_device(d, o).cpu().numpy()
             assert_geometry(ac, want)
             assert np.array_equal(got, over_counts > 0)
+            check_pattern_queries(ac, pats, d, o, want, over_counts, over_rec, overlapping=True)
     return over_total
 
 
