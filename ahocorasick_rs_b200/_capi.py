@@ -138,6 +138,14 @@ def lib():
         L.acb_count_overlapping_filtered.argtypes = L.acb_count_overlapping.argtypes[:-1] + [F, C.c_void_p]
         L.acb_count_non_overlapping_filtered.argtypes = L.acb_count_non_overlapping.argtypes[:-1] + [F, C.c_void_p]
         L.acb_stream_first_resolve_filtered.argtypes = L.acb_stream_first_resolve.argtypes[:-1] + [F, C.c_void_p]
+        L.acb_match_mask_overlapping.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64, C.c_void_p,
+                                                 C.c_uint64, C.c_void_p, C.c_void_p]
+        L.acb_match_mask_overlapping_filtered.argtypes = L.acb_match_mask_overlapping.argtypes[:-1] + [F, C.c_void_p]
+        L.acb_match_mask_non_overlapping.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64, C.POINTER(Plan),
+                                                     C.POINTER(Workspace), C.c_void_p, C.c_uint64, C.c_void_p]
+        L.acb_match_mask_non_overlapping_filtered.argtypes = L.acb_match_mask_non_overlapping.argtypes[:-1] + [F, C.c_void_p]
+        L.acb_mask_rows.argtypes = [C.c_void_p, C.c_int, C.c_uint64, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint64, C.c_void_p]
+        L.acb_mask_unpack.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
@@ -176,4 +184,6 @@ EXPORTS = [
     "acb_tokens_encode", "acb_tokens_encode_host",
     "acb_scan_batch_filtered", "acb_any_match_filtered", "acb_find_first_filtered", "acb_first_rows_filtered",
     "acb_count_overlapping_filtered", "acb_count_non_overlapping_filtered", "acb_stream_first_resolve_filtered",
+    "acb_match_mask_overlapping", "acb_match_mask_overlapping_filtered", "acb_match_mask_non_overlapping",
+    "acb_match_mask_non_overlapping_filtered", "acb_mask_rows", "acb_mask_unpack",
 ]

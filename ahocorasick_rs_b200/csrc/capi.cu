@@ -984,6 +984,83 @@ __global__ void __launch_bounds__(kScanThreads) sieve_pattern_epilogue_kernel(Si
     }
 }
 
+// The match-mask variant (acb_match_mask_non_overlapping): phases 1-3 place the overlapping list, select_stretches
+// finds each haystack's selection as in the pattern epilogue, and every selected record ORs the bits of its bytes,
+// bit_base + offsets[h] + [start, end), into `mask`.  totals[0] sums the selected records during the launch, totals[2]
+// = haystacks selected on the grid, totals[5] = the longest such stretch.  Nothing is OR-ed when the list did not fit.
+template <int MODE>
+__global__ void __launch_bounds__(kScanThreads) sieve_mask_epilogue_kernel(SieveEpiArgs E, uint32_t *mask, unsigned long long bit_base) {
+    namespace cg = cooperative_groups;
+    cg::grid_group grid = cg::this_grid();
+    if (blockIdx.x == 0 && threadIdx.x == 0) E.totals[0] = E.totals[2] = E.totals[5] = 0;  // (read and added to only after later barriers)
+    sieve_order_list<false>(E, grid);
+    grid.sync();
+    const unsigned long long list_total = E.totals[6];
+    const unsigned long long raw_total = E.totals[7];
+    const bool complete = list_total <= E.out_cap && raw_total <= E.raw_cap;  // (else the list has holes: nothing is OR-ed)
+    if (complete) {
+        const unsigned long long avail = list_total;
+        select_stretches<MODE>(E, grid, avail);
+        const uint32_t *const mark = E.raw_seq;
+        unsigned long long sum = 0;
+        for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < avail;
+             i += (unsigned long long)gridDim.x * blockDim.x) {
+            const uint4 r = reinterpret_cast<const uint4 *>(E.ordered)[i];  // haystack, pattern, start, end
+            const uint32_t c = E.unit_counts[r.x];
+            if (c == kLongMark ? mark[i] != 0 : i - E.unit_offsets[r.x] < c) {
+                or_bits(mask, bit_base + (unsigned long long)E.B.offsets[r.x] + r.z, r.w - r.z);
+                sum++;
+            }
+        }
+        block_add(E.totals, sum);
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        if (!complete) E.totals[0] = list_total;  // the caller retries with the room reported
+        E.totals[1] = complete ? 1 : 0;
+        E.totals[3] = E.totals[5] = E.totals[7] = 0;
+        E.totals[4] = raw_total > list_total ? raw_total : list_total;  // room the overlapping list needs
+        E.acc[kAccRaw] = E.acc[kAccGroups] = E.acc[kAccTraps] = E.acc[kAccRepairs] = 0;
+        E.acc[kAccQueue] = 0;
+    }
+}
+
+// acb_mask_rows: rows (haystack, pattern, start, end) of T = int32 (acb_match) or int64, haystack-relative; each ORs
+// bits bit_base + offsets[h] + [start, end).  Rows naming a haystack outside [0, n_haystacks) or an empty or negative
+// span are skipped.
+template <class T>
+__global__ void mask_rows_kernel(const T *rows, unsigned long long n, const int64_t *offsets, int64_t n_haystacks, uint32_t *mask,
+                                 unsigned long long bit_base) {
+    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
+        const long long h = (long long)rows[4 * i], s = (long long)rows[4 * i + 2], e = (long long)rows[4 * i + 3];
+        if (h < 0 || h >= n_haystacks || s < 0 || e <= s) continue;
+        or_bits(mask, bit_base + (unsigned long long)(offsets[h] + s), (uint32_t)(e - s));
+    }
+}
+
+// acb_mask_unpack: out[i] = bit bit_base + stride * i of mask, 16 outputs per thread (one 16-byte store when aligned)
+__global__ void __launch_bounds__(256) mask_unpack_kernel(const uint32_t *mask, unsigned long long bit_base, unsigned long long stride,
+                                                          unsigned long long n, uint8_t *out) {
+    for (unsigned long long i0 = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) * 16; i0 < n;
+         i0 += (unsigned long long)gridDim.x * blockDim.x * 16) {
+        uint32_t v[4] = {0, 0, 0, 0};
+        const unsigned long long m = n - i0 < 16 ? n - i0 : 16;
+#pragma unroll
+        for (int k = 0; k < 16; k++) {
+            if ((unsigned long long)k < m) {
+                const unsigned long long b = bit_base + stride * (i0 + k);
+                v[k >> 2] |= ((__ldg(mask + (b >> 5)) >> (b & 31u)) & 1u) << (8 * (k & 3));
+            }
+        }
+        if (m == 16 && (reinterpret_cast<uintptr_t>(out + i0) & 15u) == 0) {
+            *reinterpret_cast<uint4 *>(out + i0) = make_uint4(v[0], v[1], v[2], v[3]);
+        } else {
+#pragma unroll
+            for (int k = 0; k < 16; k++)
+                if ((unsigned long long)k < m) out[i0 + k] = (uint8_t)(v[k >> 2] >> (8 * (k & 3)));
+        }
+    }
+}
+
 // ---------------------------------------------------------------------------
 // HITS (acb_pattern_hits): each haystack's distinct patterns, with how many of its selected records have each one.
 // ---------------------------------------------------------------------------
@@ -2551,6 +2628,20 @@ int launch_sieve_pattern_epilogue(SieveEpiArgs &E, unsigned long long *pattern_c
     return launch_cooperative(reinterpret_cast<const void *>(sieve_pattern_epilogue_kernel<MODE>), args, d, st);
 }
 
+// acb_match_mask_*'s output: the u32 bitmask and the bit of the buffer's byte 0
+struct MaskBits {
+    uint32_t *mask;
+    unsigned long long bit_base;
+};
+
+template <int MODE>
+int launch_sieve_mask_epilogue(SieveEpiArgs &E, const MaskBits &mb, const DeviceInfo &d, cudaStream_t st) {
+    uint32_t *mask = mb.mask;
+    unsigned long long bit_base = mb.bit_base;
+    void *args[] = {&E, &mask, &bit_base};
+    return launch_cooperative(reinterpret_cast<const void *>(sieve_mask_epilogue_kernel<MODE>), args, d, st);
+}
+
 // acb_pattern_hits' counter rows
 struct HitRows {
     uint32_t *rows;
@@ -2598,18 +2689,20 @@ int filter_view(const acb_automaton *a, const acb_pattern_filter *f, int64_t n_h
 }
 
 // acb_any_match (mode kSieveAny, out = u8 flags), acb_find_first (kSieveFirst + kind, out = u64 keys),
-// acb_count_overlapping (kSieveCount, out = u64 counts per haystack) and acb_pattern_counts_overlapping (kSievePatterns,
-// out = u64 counts per pattern): one launch of the sieve kernel in a mode that writes no list
+// acb_count_overlapping (kSieveCount, out = u64 counts per haystack), acb_pattern_counts_overlapping (kSievePatterns,
+// out = u64 counts per pattern) and acb_match_mask_overlapping (kSieveCover, out = u32 mask words, from bit_base): one
+// launch of the sieve kernel in a mode that writes no list
 int sieve_early_scan(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
                      int64_t n_haystacks, uint64_t total_bytes, void *dev_out, uint64_t *dev_scratch, void *stream, int mode,
-                     const acb_pattern_filter *filter = nullptr) {
+                     const acb_pattern_filter *filter = nullptr, uint64_t bit_base = 0) {
     if (!a || !dev_sieve || !dev_offsets || !dev_out || !dev_scratch || (total_bytes && !dev_bytes)) return fail(ACB_EINVAL, "null argument");
     if (n_haystacks < 0 || n_haystacks > 0xfffffffell) return fail(ACB_EINVAL, "n_haystacks out of range (0 .. 2^32 - 2)");
     if (total_bytes >= (1ull << 31)) return fail(ACB_EINVAL, "total_bytes must be below 2^31 (scan larger inputs in windows)");
     SieveFilter F;
     bool filtered;
     if (int rc = filter_view(a, filter, n_haystacks, F, filtered)) return rc;
-    if ((mode == kSieveCount || mode == kSievePatterns) && a->impl->hdr.match_kind != ACB_STANDARD) return unsupported_overlapping(a);
+    if ((mode == kSieveCount || mode == kSievePatterns || mode == kSieveCover) && a->impl->hdr.match_kind != ACB_STANDARD)
+        return unsupported_overlapping(a);
     SieveHeader sh;
     if (int rc = sieve_header(a, sh)) return rc;
     DeviceInfo d;
@@ -2641,6 +2734,12 @@ int sieve_early_scan(const acb_automaton *a, const void *dev_sieve, const uint8_
         case kSieveFirst + ACB_LEFTMOST_LONGEST: rc = launch_sieve<false, kSieveFirst + ACB_LEFTMOST_LONGEST>(sv, B, SP, Sink{}, skipped, out, counter, d, st, Fp); break;
         case kSieveCount: rc = launch_sieve<false, kSieveCount>(sv, B, SP, Sink{}, skipped, out, counter, d, st, Fp); break;
         case kSievePatterns: rc = launch_sieve<false, kSievePatterns>(sv, B, SP, Sink{}, skipped, out, counter, d, st); break;
+        case kSieveCover: {
+            Sink cover{};
+            cover.cap = bit_base;  // (the list's capacity carries the mask's first bit in this mode)
+            rc = launch_sieve<false, kSieveCover>(sv, B, SP, cover, skipped, out, counter, d, st, Fp);
+            break;
+        }
         default: return fail(ACB_EINVAL, "unknown match kind");
     }
     if (rc) return rc;
@@ -2659,11 +2758,13 @@ int check_ws(const acb_workspace *ws) {
 // The sieve's list scan: the scan kernel, then the ordering epilogue -- acb_scan_batch's kernel 5 (counts == null:
 // the list, or its selection, in dev_out), acb_count_non_overlapping (counts: the count epilogue writes them) or
 // acb_pattern_counts_non_overlapping (counts, by_pattern: the pattern epilogue adds to them) or acb_pattern_hits (hits:
-// the hits epilogue, mode kModeOverlap for the overlapping search).  For the counts and the hits the raw records go to
+// the hits epilogue, mode kModeOverlap for the overlapping search) or acb_match_mask_non_overlapping (mb: the mask
+// epilogue ORs the selection's bytes into the mask).  For the counts, the hits and the mask the raw records go to
 // dev_raw and are ordered into dev_out, so that dev_raw is free for the pairs.
 int sieve_list_scan(const acb_automaton *a, const void *dev_sieve, const Batch &B, uint64_t total_bytes, int mode, bool cp,
                     const uint32_t *pat_cplen, const acb_plan *plan, const acb_workspace *ws, const DeviceInfo &d, cudaStream_t st,
-                    unsigned long long *counts, bool by_pattern = false, const HitRows *hits = nullptr, const SieveFilter *F = nullptr) {
+                    unsigned long long *counts, bool by_pattern = false, const HitRows *hits = nullptr, const SieveFilter *F = nullptr,
+                    const MaskBits *mb = nullptr) {
     const ImageHeader &h = a->impl->hdr;
     const int kind = (int)h.match_kind;
     const uint8_t *dev_bytes = B.bytes;
@@ -2700,7 +2801,7 @@ int sieve_list_scan(const acb_automaton *a, const void *dev_sieve, const Batch &
     uint32_t *cont_tail = reinterpret_cast<uint32_t *>(cont_cum + per_piece + 2);
     // a non-overlapping search orders the list into dev_raw's place and packs its selection into dev_out, so its
     // raw records go through dev_out first (a count packs nothing: dev_raw -> dev_out)
-    const bool in_raw = mode == kModeOverlap || counts || hits;
+    const bool in_raw = mode == kModeOverlap || counts || hits || mb;
     out.raw = in_raw ? ws->dev_raw : ws->dev_out;
     out.cap = cap;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
@@ -2746,7 +2847,9 @@ int sieve_list_scan(const acb_automaton *a, const void *dev_sieve, const Batch &
     E.totals = totals;
     E.acc = acc;
     E.match_offsets = match_offsets;
-    if (hits)
+    if (mb)
+        rc = mode == kModeStandard ? launch_sieve_mask_epilogue<kModeStandard>(E, *mb, d, st) : launch_sieve_mask_epilogue<kModeLeftmost>(E, *mb, d, st);
+    else if (hits)
         rc = mode == kModeStandard   ? launch_sieve_hits_epilogue<kModeStandard>(E, *hits, d, st)
              : mode == kModeLeftmost ? launch_sieve_hits_epilogue<kModeLeftmost>(E, *hits, d, st)
                                      : launch_sieve_hits_epilogue<kModeOverlap>(E, *hits, d, st);
@@ -2764,12 +2867,14 @@ int sieve_list_scan(const acb_automaton *a, const void *dev_sieve, const Batch &
 }
 
 // acb_count_non_overlapping (by_pattern = false: counts per haystack, written), acb_pattern_counts_non_overlapping
-// (by_pattern: counts per pattern, added to) and acb_pattern_hits (hits, dev_counts unused; either search)
+// (by_pattern: counts per pattern, added to), acb_pattern_hits (hits, dev_counts unused; either search) and
+// acb_match_mask_non_overlapping (mb, dev_counts unused: the selection's bytes OR-ed into the mask)
 int non_overlapping_counts(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
                            int64_t n_haystacks, uint64_t total_bytes, const acb_plan *plan, const acb_workspace *ws,
                            uint64_t *dev_counts, void *stream, bool by_pattern, const HitRows *hits = nullptr, bool overlapping = false,
-                           const acb_pattern_filter *filter = nullptr) {
-    if (!a || !dev_sieve || !dev_offsets || !plan || (!dev_counts && !hits) || (total_bytes && !dev_bytes)) return fail(ACB_EINVAL, "null argument");
+                           const acb_pattern_filter *filter = nullptr, const MaskBits *mb = nullptr) {
+    if (!a || !dev_sieve || !dev_offsets || !plan || (!dev_counts && !hits && !mb) || (mb && !mb->mask) || (total_bytes && !dev_bytes))
+        return fail(ACB_EINVAL, "null argument");
     if (int rc = check_ws(ws)) return rc;
     if (n_haystacks < 0 || n_haystacks > 0xfffffffell) return fail(ACB_EINVAL, "n_haystacks out of range (0 .. 2^32 - 2)");
     SieveFilter F;
@@ -2788,7 +2893,7 @@ int non_overlapping_counts(const acb_automaton *a, const void *dev_sieve, const 
     if (int rc = device_info(d)) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (n_haystacks == 0 || total_bytes == 0) {
-        if (n_haystacks && !by_pattern && !hits) CUDA_OK(cudaMemsetAsync(dev_counts, 0, (uint64_t)n_haystacks * sizeof(uint64_t), st));
+        if (n_haystacks && !by_pattern && !hits && !mb) CUDA_OK(cudaMemsetAsync(dev_counts, 0, (uint64_t)n_haystacks * sizeof(uint64_t), st));
         zero_outputs_kernel<<<(unsigned)((n_haystacks + 256) / 256), 256, 0, st>>>(
             reinterpret_cast<unsigned long long *>(ws->dev_unit_offsets), reinterpret_cast<unsigned long long *>(ws->dev_match_offsets),
             n_haystacks, reinterpret_cast<unsigned long long *>(ws->dev_total));
@@ -2798,7 +2903,7 @@ int non_overlapping_counts(const acb_automaton *a, const void *dev_sieve, const 
     }
     const int mode = overlapping ? kModeOverlap : a->impl->hdr.match_kind == ACB_STANDARD ? kModeStandard : kModeLeftmost;
     return sieve_list_scan(a, dev_sieve, Batch{dev_bytes, dev_offsets, n_haystacks}, total_bytes, mode, false, nullptr, plan, ws, d, st,
-                           reinterpret_cast<unsigned long long *>(dev_counts), by_pattern, hits, filtered ? &F : nullptr);
+                           reinterpret_cast<unsigned long long *>(dev_counts), by_pattern, hits, filtered ? &F : nullptr, mb);
 }
 
 }  // namespace
@@ -2913,6 +3018,75 @@ int acb_pattern_hits(const acb_automaton *a, const void *dev_sieve, const uint8_
     const HitRows hits{dev_rows, row_words, (uint32_t)a->impl->hdr.n_patterns};
     return non_overlapping_counts(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, plan, ws, nullptr, stream, false, &hits,
                                   overlapping != 0);
+}
+
+int acb_match_mask_overlapping_filtered(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                                        int64_t n_haystacks, uint64_t total_bytes, uint32_t *dev_mask, uint64_t bit_base,
+                                        uint64_t *dev_scratch, const acb_pattern_filter *filter, void *stream) {
+    if (!dev_mask) return fail(ACB_EINVAL, "null argument");
+    return sieve_early_scan(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, dev_mask, dev_scratch, stream, kSieveCover, filter,
+                            bit_base);
+}
+
+int acb_match_mask_overlapping(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                               int64_t n_haystacks, uint64_t total_bytes, uint32_t *dev_mask, uint64_t bit_base, uint64_t *dev_scratch,
+                               void *stream) {
+    return acb_match_mask_overlapping_filtered(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, dev_mask, bit_base, dev_scratch,
+                                               nullptr, stream);
+}
+
+int acb_match_mask_non_overlapping_filtered(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes,
+                                            const int64_t *dev_offsets, int64_t n_haystacks, uint64_t total_bytes, const acb_plan *plan,
+                                            const acb_workspace *ws, uint32_t *dev_mask, uint64_t bit_base,
+                                            const acb_pattern_filter *filter, void *stream) {
+    if (!dev_mask) return fail(ACB_EINVAL, "null argument");
+    const MaskBits mb{dev_mask, bit_base};
+    return non_overlapping_counts(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, plan, ws, nullptr, stream, false, nullptr,
+                                  false, filter, &mb);
+}
+
+int acb_match_mask_non_overlapping(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                                   int64_t n_haystacks, uint64_t total_bytes, const acb_plan *plan, const acb_workspace *ws,
+                                   uint32_t *dev_mask, uint64_t bit_base, void *stream) {
+    return acb_match_mask_non_overlapping_filtered(a, dev_sieve, dev_bytes, dev_offsets, n_haystacks, total_bytes, plan, ws, dev_mask, bit_base,
+                                                   nullptr, stream);
+}
+
+int acb_mask_rows(const void *dev_rows, int row_bytes, uint64_t n_rows, const int64_t *dev_offsets, int64_t n_haystacks, uint32_t *dev_mask,
+                  uint64_t bit_base, void *stream) {
+    if (!dev_mask || !dev_offsets || (n_rows && !dev_rows)) return fail(ACB_EINVAL, "null argument");
+    if (row_bytes != 4 && row_bytes != 8) return fail(ACB_EINVAL, "row_bytes must be 4 (acb_match records) or 8 (int64 rows)");
+    if (n_haystacks < 0 || n_haystacks > 0xfffffffell) return fail(ACB_EINVAL, "n_haystacks out of range (0 .. 2^32 - 2)");
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    if (n_rows == 0 || n_haystacks == 0) return ACB_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    uint64_t blocks = (n_rows + 255) / 256;
+    if (blocks > 16ull * d.sms) blocks = 16ull * d.sms;  // grid-stride beyond that
+    if (row_bytes == 4)
+        mask_rows_kernel<int32_t><<<(unsigned)blocks, 256, 0, st>>>(static_cast<const int32_t *>(dev_rows), n_rows, dev_offsets, n_haystacks,
+                                                                    dev_mask, bit_base);
+    else
+        mask_rows_kernel<long long><<<(unsigned)blocks, 256, 0, st>>>(static_cast<const long long *>(dev_rows), n_rows, dev_offsets, n_haystacks,
+                                                                      dev_mask, bit_base);
+    g_launches++;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+int acb_mask_unpack(const uint32_t *dev_mask, uint64_t bit_base, uint64_t stride, uint64_t n, uint8_t *dev_out, void *stream) {
+    if (n && (!dev_mask || !dev_out)) return fail(ACB_EINVAL, "null argument");
+    if (stride == 0) return fail(ACB_EINVAL, "stride must be at least 1");
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    if (n == 0) return ACB_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    uint64_t blocks = (n + 256 * 16 - 1) / (256 * 16);
+    if (blocks > 16ull * d.sms) blocks = 16ull * d.sms;  // grid-stride beyond that
+    mask_unpack_kernel<<<(unsigned)blocks, 256, 0, st>>>(dev_mask, bit_base, stride, n, dev_out);
+    g_launches++;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
 }
 
 int acb_count_rows(const acb_automaton *a, const int64_t *dev_rows, uint64_t n_rows, uint64_t *dev_scratch, uint64_t *dev_count,

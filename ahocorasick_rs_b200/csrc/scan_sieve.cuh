@@ -67,6 +67,12 @@
 // and adds 1 per pid instead of writing a record.  The chain is walked one pid per lane per step; lanes of a step that
 // hold the same pid (a short common pattern takes most hits) are summed first, and one lane per distinct pid adds.
 // Every position counts, so nothing is skipped.
+//
+// COVER (acb_match_mask_overlapping): the answer is the set of bytes that lie inside some overlapping match, as a u32
+// bitmask OR-ed into by the kernel (bit bit_base + p = byte p of the buffer).  Every match that ends at a position is a
+// suffix of the longest one ending there (the deepest terminal node, depth best_d, as FIRST finds it), so the union
+// of [e - best_d, e) over the matching end positions e is the cover: stage 2 ORs those bits, one atomicOr per word
+// the span touches, and walks no chain.  Every position counts, so nothing is skipped.
 #pragma once
 #include "scan_staged.cuh"
 #include "sieve.h"
@@ -153,6 +159,7 @@ constexpr int kSieveAny = 1;    // one flag per haystack (acb_any_match)
 constexpr int kSieveFirst = 2;  // one first-match key per haystack (acb_find_first): kSieveFirst + the match kind (ACB_*)
 constexpr int kSieveCount = 5;  // one overlapping match count per haystack (acb_count_overlapping)
 constexpr int kSievePatterns = 6;  // one overlapping match count per pattern (acb_pattern_counts_overlapping)
+constexpr int kSieveCover = 7;     // the bytes the overlapping matches cover, as a bitmask (acb_match_mask_overlapping)
 
 // continuation bytes among the first nbytes (0..16) of the 16-byte chunk at shared address a
 __device__ __forceinline__ uint32_t cont_prefix(uint32_t a, uint32_t nbytes) {
@@ -184,6 +191,16 @@ __device__ __forceinline__ void add_per_pattern(unsigned long long *counts, uint
     if ((threadIdx.x & 31u) == (uint32_t)__ffs(peers) - 1u) atomicAdd(counts + pid, (unsigned long long)__popc(peers));
 }
 
+// bits [b0, b0 + len) of the u32 bitmask `mask` are set: one atomicOr per word they touch
+__device__ __forceinline__ void or_bits(uint32_t *mask, unsigned long long b0, uint32_t len) {
+    const unsigned long long b1 = b0 + len;
+    for (unsigned long long w = b0 >> 5; (w << 5) < b1; w++) {
+        const unsigned long long lo = (w << 5) > b0 ? (w << 5) : b0, hi = (w << 5) + 32 < b1 ? (w << 5) + 32 : b1;
+        const uint32_t n = (uint32_t)(hi - lo), s = (uint32_t)(lo & 31u);
+        atomicOr(mask + w, (n == 32 ? 0xffffffffu : ((1u << n) - 1u)) << s);
+    }
+}
+
 // Pattern sets (sieve_scan_filtered_kernel): each haystack h searches only for the pattern ids of ONE set, row
 // index[h] of a packed bitset (n_sets rows of `words` u32, bit p of a row = pattern p is in the set).  A pid is ADMITTED
 // when its bit is set in its haystack's row; an index outside [0, n_sets) admits nothing.  Stage 2 is the only place a
@@ -195,6 +212,8 @@ __device__ __forceinline__ void add_per_pattern(unsigned long long *counts, uint
 //          key of every kind (Standard: longest; LeftmostFirst: leftmost start, then lowest index; LeftmostLongest:
 //          leftmost start), exactly as the deepest terminal node is without a filter
 //   COUNT  the number of admitted pids
+//   COVER  the depth of the deepest node with an admitted pid, as FIRST: every admitted match ending here is a suffix
+//          of that one
 // Every key and flag comes from admitted matches only, so the skips ("flag set", "cannot beat the key") stay exact.
 struct SieveFilter {
     const uint32_t *bits;   // n_sets x words
@@ -223,7 +242,8 @@ __device__ __forceinline__ bool filter_admits(const uint32_t *row, uint32_t pid)
 // code-point pointers carry the mode's outputs instead (so the list-mode instantiations keep their parameter block):
 // hay_cont -> flags = u8[n_haystacks] (any), keys = u64[n_haystacks] (first), counts = u64[n_haystacks] (count) or
 // counts = u64[n_patterns] (patterns), task_cont -> skipped = u64[2] = [tasks skipped whole, windows not scanned] (see
-// acb_any_match, acb_find_first; count, patterns: unused).
+// acb_any_match, acb_find_first; count, patterns: unused).  kSieveCover: hay_cont -> mask = u32 words, out.cap = the
+// mask's bit_base.
 //
 // FILT: stage 2 admits only the pids of each haystack's pattern set (see SieveFilter); the kernel body is shared by
 // sieve_scan_kernel (no filter) and sieve_scan_filtered_kernel.
@@ -233,6 +253,7 @@ __device__ __forceinline__ void sieve_scan(DevSieve sv, Batch B, SievePlan P, Si
     static_assert(!(FILT && MODE == kSievePatterns), "the pattern-count mode has no filtered form");
     constexpr bool ANY = MODE == kSieveAny, FIRST = MODE >= kSieveFirst && MODE < kSieveCount, EARLY = ANY || FIRST;  // EARLY: no list, work stops early
     constexpr bool COUNT = MODE == kSieveCount, PATTERNS = MODE == kSievePatterns, LIST = MODE == kSieveList;
+    constexpr bool COVER = MODE == kSieveCover;
     constexpr int KIND = MODE - kSieveFirst;  // (FIRST)
     static_assert(!(!LIST && CP), "the any-match, first-match and count modes have no positions to count");
     uint8_t *const flags = reinterpret_cast<uint8_t *>(hay_cont);
@@ -449,7 +470,7 @@ __device__ __forceinline__ void sieve_scan(DevSieve sv, Batch B, SievePlan P, Si
                 while (v != kSieveNoNode) {
                     if (na.y & kNodeTerminal) {
                         best = v;
-                        if (FIRST) best_d = d;
+                        if (FIRST || COVER) best_d = d;
                     }
                     const uint32_t nk = (na.y >> 8) & 0x1ffu;
                     if (nk == 0 || (int32_t)rel - (int32_t)d < hs) break;  // no longer pattern, or it would start before the haystack
@@ -505,9 +526,9 @@ __device__ __forceinline__ void sieve_scan(DevSieve sv, Batch B, SievePlan P, Si
                                 best_d = nb.w;
                             }
                             cnt++;
-                            if (EARLY) break;
+                            if (EARLY || COVER) break;
                         }
-                        if (EARLY && cnt) break;
+                        if ((EARLY || COVER) && cnt) break;
                         u = nb.z;
                     }
                     if (ANY) {
@@ -542,7 +563,7 @@ __device__ __forceinline__ void sieve_scan(DevSieve sv, Batch B, SievePlan P, Si
                         atomicMin(keys + h, key);
                     }
                 } else if (best != kSieveNoNode) {
-                    cnt = __ldg(&sv.nb[best].chain_cnt);
+                    cnt = COVER ? 1u : __ldg(&sv.nb[best].chain_cnt);
                 }
             }
             const uint32_t hits = EARLY ? 0u : __ballot_sync(0xffffffffu, cnt != 0);
@@ -567,6 +588,9 @@ __device__ __forceinline__ void sieve_scan(DevSieve sv, Batch B, SievePlan P, Si
                         if (u != kSieveNoNode) nb = __ldg(reinterpret_cast<const uint4 *>(sv.nb + u));
                     }
                 }
+            } else if (COVER) {
+                // the longest match ending here covers every shorter one: its bytes [e - best_d, e) of the buffer
+                if (cnt) or_bits(hay_cont, out.cap + (uint64_t)(t_lo + (int64_t)rel + 1) - best_d, best_d);
             } else if (hits) {
                 uint32_t total;
                 const uint32_t exc = warp_excl_scan(cnt, lane, &total);
@@ -854,7 +878,7 @@ sieve_scan_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_co
     sieve_scan<CP, WC, MODE, false>(sv, B, P, out, task_cont, hay_cont, task_counter, SieveFilter{});
 }
 
-// the same scan with each haystack's pattern set (LIST, ANY, FIRST and COUNT)
+// the same scan with each haystack's pattern set (LIST, ANY, FIRST, COUNT and COVER)
 template <bool CP, int WC, int MODE = kSieveList>
 __global__ void __launch_bounds__(kSieveThreads, 1)
 sieve_scan_filtered_kernel(DevSieve sv, Batch B, SievePlan P, Sink out, uint32_t *task_cont, uint32_t *hay_cont, unsigned int *task_counter,

@@ -1239,6 +1239,185 @@ class _Automaton:
             ro, p = ro.cpu().tolist(), p.cpu().tolist()
         return [p[ro[i]:ro[i + 1]] for i in range(n)]
 
+    # ---- match masks: which bytes lie inside a match of find_matches_as_indexes, without the list ----------------
+    def mask_device(self, data, offsets, overlapping=False, capacity: Optional[int] = None, flt=None, words=None, bit_base: int = 0):
+        """Which bytes of a device-resident batch lie inside one of its haystacks' matches -> the packed mask, an int32
+        CUDA tensor of u32 words: bit p % 32 of word p // 32 = byte p of `data` is covered (start <= p - offsets[h] < end
+        for a record of haystack h's list in scan_device).  With `words` given, the bits go to bit_base + p and are
+        OR-ed into it (runs and windows share one mask).  An overlapping search on a leftmost automaton raises
+        ValueError, as scan_device does.
+
+        Where the engine rule of scan_device picks the sieve (always with pattern sets): an overlapping search is the
+        sieve kernel's cover mode (acb_match_mask_overlapping: the longest match at each end position, no list) and
+        returns without waiting for the device; a non-overlapping search is the sieve's list scan and a mask epilogue
+        (acb_match_mask_non_overlapping), which waits for the device and scans again with more room when the list did
+        not fit (nothing was OR-ed then).  Where the rule picks a table walker, the rows of its full scan are OR-ed in
+        with acb_mask_rows; the next scan that reuses the workspace waits for that.  Batches above WINDOW_BYTES go in
+        runs of whole haystacks, and one haystack above it in windows.  `capacity`: as for scan_device."""
+        self.check_overlapping(overlapping)
+        torch = _require_cuda()
+        dev = data.device
+        n = offsets.numel() - 1
+        if words is None:
+            words = torch.zeros((data.numel() + 31) // 32, dtype=torch.int32, device=dev)
+        if n <= 0 or data.numel() == 0:
+            self.last_stats = {"engine": None, "mode": "match_mask", "long_stretches": 0, **self._set_stats(flt)}
+            return words
+        if data.numel() > self.WINDOW_BYTES:
+            self._mask_windows(words, bit_base, data, offsets, overlapping, flt)
+            return words
+        with self._lock, torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev)
+            if flt is None and self._pick_engine(dev, data, offsets, overlapping) is not None:
+                m, _, _ = self.scan_device(data, offsets, overlapping, False)
+                self._mask_rows(words, bit_base, m, offsets)
+                reader = torch.cuda.Event()
+                reader.record(stream)
+                self._ws[(dev.index if dev.index is not None else torch.cuda.current_device(), 0)]["reader"] = reader
+                self.last_stats = {"engine": self.last_stats.get("engine", "table"), "mode": "match_mask", "long_stretches": 0}
+                return words
+            sieve_t, _ = self.sieve(dev)
+            if overlapping:
+                scratch = torch.empty(3, dtype=torch.int64, device=dev)
+                rc = self._L.acb_match_mask_overlapping_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n,
+                                                                 data.numel(), words.data_ptr(), bit_base, scratch.data_ptr(),
+                                                                 _filter_struct(flt), stream.cuda_stream)
+                if rc != _capi.ACB_OK:
+                    raise RuntimeError(_capi.last_error())
+                self.last_stats = {"engine": "sieve", "mode": "match_mask", **self.sieve_geometry(dev, self._plan(data, n).task_bytes),
+                                   **self._set_stats(flt)}
+                return words
+            plan = self._plan(data, n)
+            cap = capacity or max(1024, n * 2)
+            while True:
+                ws = self._workspace(dev, plan, n, cap, 0)
+                reader = ws.pop("reader", None)
+                if reader is not None:   # a comparison of an earlier call (maybe on another stream) reads this workspace first
+                    stream.wait_event(reader)
+                st = self._ws_struct(ws)
+                rc = self._L.acb_match_mask_non_overlapping_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n,
+                                                                     data.numel(), C.byref(plan), C.byref(st), words.data_ptr(), bit_base,
+                                                                     _filter_struct(flt), stream.cuda_stream)
+                if rc != _capi.ACB_OK:
+                    err = _capi.last_error()
+                    ws["scratch"][:8].zero_()   # a scan that failed half way may have left its counters dirty
+                    raise RuntimeError(err)
+                tot = ws["total"].tolist()
+                total, complete, long_stretches, raw_total = tot[0], tot[1], tot[2], tot[4]
+                if complete or (total == 0 and raw_total == 0):
+                    break
+                cap = max(total, raw_total) + max(total, raw_total) // 8 + 16   # (nothing was OR-ed: the mask stays as it was)
+            self.last_stats = {"engine": "sieve", "mode": "match_mask", **self.sieve_geometry(dev, plan.task_bytes),
+                               "list_records": raw_total, "long_stretches": long_stretches, **self._set_stats(flt)}
+            return words
+
+    def _mask_rows(self, words, bit_base: int, rows, offsets):
+        """acb_mask_rows: OR the spans of selected rows (int32 acb_match records or int64 rows, haystack-relative) into
+        `words` at bit_base + offsets[h] + [start, end)."""
+        torch = _torch()
+        if rows.shape[0] == 0:
+            return
+        rows = rows.contiguous()
+        rc = self._L.acb_mask_rows(rows.data_ptr(), rows.element_size(), rows.shape[0], offsets.data_ptr(), offsets.numel() - 1,
+                                   words.data_ptr(), bit_base, torch.cuda.current_stream(rows.device).cuda_stream)
+        if rc != _capi.ACB_OK:
+            raise RuntimeError(_capi.last_error())
+
+    def _mask_windows(self, words, bit_base: int, data, offsets, overlapping, flt=None):
+        """mask_device above WINDOW_BYTES: runs of whole haystacks that fit one call each OR their bits, from the run's
+        first byte on; one haystack above the limit goes to _mask_one_large.  last_stats["long_stretches"] sums the
+        runs'."""
+        torch = _require_cuda()
+        dev = data.device
+        n = offsets.numel() - 1
+        limit = self.WINDOW_BYTES
+        lens = offsets[1:] - offsets[:-1]
+        oversized = bool((lens > limit).any().item())
+        long_stretches = 0
+        engine = None
+        h = 0
+        while h < n:
+            start = int(offsets[h].item())
+            if oversized and int(lens[h].item()) > limit:
+                self._mask_one_large(words, bit_base + start, data[start:start + int(lens[h].item())], overlapping, _filter_slice(flt, h, h + 1))
+                h += 1
+                continue
+            # the longest run of whole haystacks that fits one call (and stops before an oversized one)
+            h1 = int(torch.searchsorted(offsets, torch.tensor([start + limit], dtype=torch.int64, device=dev), right=True).item()) - 1
+            h1 = max(h + 1, min(h1, n))
+            if oversized:
+                big = torch.nonzero(lens[h:h1] > limit)
+                if big.numel():
+                    h1 = h + int(big[0].item())
+            end = int(offsets[h1].item())
+            if end > start:
+                self.mask_device(data[start:end], offsets[h:h1 + 1] - start, overlapping, flt=_filter_slice(flt, h, h1), words=words,
+                                 bit_base=bit_base + start)
+                long_stretches += self.last_stats.get("long_stretches", 0)
+                engine = self.last_stats.get("engine") or engine
+            h = h1
+        torch.cuda.current_stream(dev).synchronize()
+        self.last_stats = {"engine": engine, "mode": "match_mask", "long_stretches": long_stretches, "windows": True,
+                           **self._set_stats(flt)}
+
+    def _mask_one_large(self, words, bit_base: int, hay, overlapping, flt=None):
+        """OR the mask of one haystack above WINDOW_BYTES into `words` from bit_base on.
+        Overlapping: windows that share max_pattern_len - 1 bytes, each OR-ed at its own start.  Every match lies
+        inside some window whole, and a match seen by two windows sets the same bits twice: nothing is subtracted.
+        Non-overlapping: the selected rows of _scan_one_large, OR-ed with acb_mask_rows."""
+        torch = _require_cuda()
+        dev = hay.device
+        if overlapping:
+            limit, halo = self.WINDOW_BYTES, max(self.max_pattern_len - 1, 0)
+            w0 = 0
+            while True:
+                w1 = min(w0 + limit, hay.numel())
+                self.mask_device(hay[w0:w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=dev), True, flt=flt, words=words,
+                                 bit_base=bit_base + w0)
+                if w1 == hay.numel():
+                    return
+                w0 += limit - halo
+        rows = self._scan_one_large(hay, False, False, flt)
+        self._mask_rows(words, bit_base, rows, torch.tensor([0, hay.numel()], dtype=torch.int64, device=dev))
+
+    def unpack_mask(self, words, n: int, stride: int = 1):
+        """acb_mask_unpack: bool CUDA tensor (n,), entry i = bit stride * i of the packed mask."""
+        torch = _require_cuda()
+        out = torch.empty(n, dtype=torch.bool, device=words.device)
+        rc = self._L.acb_mask_unpack(words.data_ptr(), 0, stride, n, out.data_ptr(), torch.cuda.current_stream(words.device).cuda_stream)
+        if rc != _capi.ACB_OK:
+            raise RuntimeError(_capi.last_error())
+        return out
+
+    def spans_host_batch(self, chunks: Sequence[bytes], overlapping, codepoints: bool, patterns=None, unit: int = 1):
+        """Host buffers (bytes-like objects, one per haystack) -> one list of (start, end) per haystack: the maximal
+        runs of covered positions, haystack-relative, in code points with `codepoints`, else in bytes divided by `unit`.
+        The offsets and the haystacks are gathered into the pinned staging buffer and go to the device in one copy; the
+        packed mask (one bit per byte) comes back."""
+        torch = _require_cuda()
+        self.check_overlapping(overlapping)
+        n = len(chunks)
+        if n == 0:
+            return []
+        offs = np.zeros(n + 1, dtype=np.int64)
+        np.cumsum(np.fromiter((len(c) for c in chunks), dtype=np.int64, count=n), out=offs[1:])
+        total_bytes = int(offs[-1])
+        head = (8 * (n + 1) + 511) & ~511   # the offsets, then the bytes at a 512-byte boundary of the buffer
+        dev = torch.device("cuda", torch.cuda.current_device())
+        with self._host_lock:
+            host = self._pinned(head + total_bytes)
+            hv = host.numpy()
+            hv[:8 * (n + 1)].view(np.int64)[:] = offs
+            if n == 1:
+                hv[head:head + total_bytes] = np.frombuffer(chunks[0], dtype=np.uint8)
+            elif total_bytes:
+                hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
+            d = host[:head + total_bytes].to(dev, non_blocking=True)
+            flt = _host_sets(self, patterns, n, dev) if patterns is not None else None
+            words = self.mask_device(d[head:], d[:8 * (n + 1)].view(torch.int64), overlapping, flt=flt).cpu().numpy()
+            text = hv[head:head + total_bytes].copy() if codepoints else None
+        return spans_from_words(words, offs, text, unit)
+
     def scan_device(self, data, offsets, overlapping=False, codepoints=False, capacity: Optional[int] = None,
                     sync: bool = True, ws_slot: int = 0, flt=None):
         """Scan a device-resident batch.  data: uint8 CUDA tensor, offsets: int64
@@ -2089,6 +2268,36 @@ def _tuples(m: np.ndarray):
     return list(zip(m[:, 1].tolist(), m[:, 2].tolist(), m[:, 3].tolist()))
 
 
+def spans_from_words(words: np.ndarray, offs: np.ndarray, text: Optional[np.ndarray] = None, unit: int = 1):
+    """A packed mask (u32 words, bit p % 32 of word p // 32 = byte p; any 4-byte integer dtype) over the haystacks
+    [offs[h], offs[h + 1]) -> one list of (start, end) per haystack: its maximal runs of covered bytes, cut at haystack
+    boundaries, haystack-relative.  With `text` (the batch's UTF-8 bytes) positions are code points: a byte position
+    maps to the number of lead bytes before it.  Else they are bytes divided by `unit` (3 for token ids)."""
+    offs = np.asarray(offs, dtype=np.int64)
+    n, total = len(offs) - 1, int(offs[-1])
+    bits = np.unpackbits(np.ascontiguousarray(words).view(np.uint8), bitorder="little")[:total].astype(bool)
+    bits[:int(offs[0])] = False
+    # a run starts where a covered byte follows an uncovered one or a haystack start; it ends symmetrically
+    cut = np.zeros(total + 1, dtype=bool)
+    cut[offs] = True
+    prev = np.concatenate([[False], bits])
+    nxt = np.concatenate([bits, [False]])
+    starts = np.flatnonzero(nxt & (~prev | cut))
+    ends = np.flatnonzero(prev & (~nxt | cut))
+    hay = np.searchsorted(offs, starts, side="right") - 1
+    if text is not None:
+        lead = np.zeros(total + 1, dtype=np.int64)
+        np.cumsum((np.asarray(text[:total]) & 0xC0) != 0x80, out=lead[1:])
+        base = lead[offs[hay]]
+        s, e = lead[starts] - base, lead[ends] - base
+    else:
+        base = offs[hay]
+        s, e = (starts - base) // unit, (ends - base) // unit
+    bounds = np.searchsorted(hay, np.arange(n + 1), side="left")
+    pairs = list(zip(s.tolist(), e.tolist()))
+    return [pairs[bounds[h]:bounds[h + 1]] for h in range(n)]
+
+
 def _one_set(patterns):
     """A single-haystack host call's patterns= -> the per-haystack list the host batches take (None stays None)."""
     return None if patterns is None else [patterns]
@@ -2258,6 +2467,32 @@ class AhoCorasick(_PatternSetMethods):
         """Device-resident UTF-8 batch -> int64 tensor (n,) of match counts (see _Automaton.count_device)."""
         self._ac.check_overlapping(overlapping)
         return self._ac.count_device(data, offsets, overlapping, flt=self._device_filter(data, offsets, pattern_sets, set_index))
+
+    # ---- additions: which positions lie inside a match ---------------------------------------------------------
+    def match_spans(self, haystack: str, overlapping: bool = False, patterns=None) -> list:
+        """-> [(start, end), ...] in code points: the maximal runs of code points that lie inside some match of
+        ``find_matches_as_indexes(haystack, overlapping)``.  Overlapping or touching matches merge into one span."""
+        if not isinstance(haystack, str):
+            raise TypeError("argument 'haystack': 'str' expected")
+        self._ac.check_overlapping(overlapping)
+        return self._ac.spans_host_batch([haystack.encode("utf-8")], overlapping, True, _one_set(patterns))[0]
+
+    def match_spans_batch(self, haystacks: Sequence[str], overlapping: bool = False, patterns=None) -> list:
+        """``match_spans`` for each haystack, in one transfer and one scan; a span never crosses a haystack boundary."""
+        hays = list(haystacks)
+        for h in hays:
+            if not isinstance(h, str):
+                raise TypeError("argument 'haystack': 'str' expected")
+        self._ac.check_overlapping(overlapping)
+        return self._ac.spans_host_batch([h.encode("utf-8") for h in hays], overlapping, True, _batch_sets(patterns, len(hays)))
+
+    def match_mask_device(self, data, offsets, overlapping: bool = False, pattern_sets=None, set_index=None):
+        """Device-resident UTF-8 batch -> bool tensor of data's shape: byte p is True when it lies inside a match of its
+        haystack (every byte of a covered code point is covered; bytes outside every haystack are False).  See
+        _Automaton.mask_device."""
+        self._ac.check_overlapping(overlapping)
+        words = self._ac.mask_device(data, offsets, overlapping, flt=self._device_filter(data, offsets, pattern_sets, set_index))
+        return self._ac.unpack_mask(words, data.numel())
 
     def count_matches_by_pattern(self, haystack: str, overlapping: bool = False) -> list:
         """-> list of length ``len(patterns)``: entry i is how many of ``find_matches_as_indexes(haystack,
@@ -2444,6 +2679,27 @@ class BytesAhoCorasick(_PatternSetMethods):
         """Device-resident batch -> int64 tensor (n,) of match counts (see _Automaton.count_device)."""
         self._ac.check_overlapping(overlapping)
         return self._ac.count_device(data, offsets, overlapping, flt=self._device_filter(data, offsets, pattern_sets, set_index))
+
+    # ---- additions: which positions lie inside a match ---------------------------------------------------------
+    def match_spans(self, haystack, overlapping: bool = False, patterns=None) -> list:
+        """-> [(start, end), ...] in bytes: the maximal runs of bytes that lie inside some match of
+        ``find_matches_as_indexes(haystack, overlapping)``.  Overlapping or touching matches merge into one span."""
+        hay = _as_buffer_bytes(haystack)
+        self._ac.check_overlapping(overlapping)
+        return self._ac.spans_host_batch([hay], overlapping, False, _one_set(patterns))[0]
+
+    def match_spans_batch(self, haystacks: Sequence, overlapping: bool = False, patterns=None) -> list:
+        """``match_spans`` for each haystack, in one transfer and one scan; a span never crosses a haystack boundary."""
+        hays = [_as_buffer_bytes(h) for h in haystacks]
+        self._ac.check_overlapping(overlapping)
+        return self._ac.spans_host_batch(hays, overlapping, False, _batch_sets(patterns, len(hays)))
+
+    def match_mask_device(self, data, offsets, overlapping: bool = False, pattern_sets=None, set_index=None):
+        """Device-resident batch -> bool tensor of data's shape: byte p is True when it lies inside a match of its
+        haystack (bytes outside every haystack are False).  See _Automaton.mask_device."""
+        self._ac.check_overlapping(overlapping)
+        words = self._ac.mask_device(data, offsets, overlapping, flt=self._device_filter(data, offsets, pattern_sets, set_index))
+        return self._ac.unpack_mask(words, data.numel())
 
     def count_matches_by_pattern(self, haystack, overlapping: bool = False) -> list:
         """-> list of length ``len(patterns)``: entry i is how many of ``find_matches_as_indexes(haystack,
@@ -2873,6 +3129,26 @@ class TokenAhoCorasick(_PatternSetMethods):
         self._ac.check_overlapping(overlapping)
         flt = self._token_filter(tokens, offsets, pattern_sets, set_index)
         return self._on_device(lambda d, o: self._ac.count_device(d, o, overlapping, flt=flt), tokens, offsets)
+
+    def match_spans(self, haystack, overlapping: bool = False, patterns=None) -> list:
+        """-> [(start, end), ...] in tokens: the maximal runs of tokens that lie inside some match of
+        ``find_matches_as_indexes(haystack, overlapping)``."""
+        return self.match_spans_batch([haystack], overlapping, _one_set(patterns))[0]
+
+    def match_spans_batch(self, haystacks: Sequence, overlapping: bool = False, patterns=None) -> list:
+        hays = self._hays(haystacks)
+        self._ac.check_overlapping(overlapping)
+        return self._ac.spans_host_batch(hays, overlapping, False, _batch_sets(patterns, len(hays)), unit=_capi.ACB_TOKEN_BYTES)
+
+    def match_mask_device(self, tokens, offsets, overlapping: bool = False, pattern_sets=None, set_index=None):
+        """Device-resident batch of ids -> bool tensor (len(tokens),): token i is True when it lies inside a match of its
+        haystack (a per-token loss mask of banned sequences).  The mask is built over the encoded bytes and read at
+        every token's first byte: an occurrence starts and ends on a token boundary."""
+        self._ac.check_overlapping(overlapping)
+        flt = self._token_filter(tokens, offsets, pattern_sets, set_index)
+        n = tokens.numel() if hasattr(tokens, "numel") else 0
+        return self._on_device(lambda d, o: self._ac.unpack_mask(self._ac.mask_device(d, o, overlapping, flt=flt), n, _capi.ACB_TOKEN_BYTES),
+                               tokens, offsets)
 
     def count_matches_by_pattern(self, haystack, overlapping: bool = False) -> list:
         """-> entry i is how many of ``find_matches_as_indexes(haystack, overlapping)`` have pattern i."""

@@ -600,6 +600,56 @@ int acb_stream_first_resolve_filtered(const acb_automaton *a, const void *dev_si
                                       uint64_t *dev_seam_keys, uint64_t *dev_chunk_keys, int64_t *dev_best, int64_t *dev_scratch,
                                       int64_t *dev_rows, const acb_pattern_filter *filter, void *stream);
 
+/*
+ * Match masks: which bytes of a device-resident batch lie inside a match.  For haystack h, with R_h the reference's
+ * result find_matches_as_indexes(h, overlapping) (with a filter: R_h for h's set), byte offsets[h] + p is COVERED when
+ * start <= p < end for some record of R_h.  Bytes outside every haystack are not covered.  The mask is a u32 bitmask
+ * that every call OR-accumulates into: bit bit_base + q (bit q % 32 of word q / 32) stands for byte q of dev_bytes,
+ * and the caller zeroes the mask once.  So runs of haystacks, windows of one haystack and several code paths can fill
+ * one mask.  The list is never handed back.
+ *
+ * acb_match_mask_overlapping covers the overlapping matches: one launch of the sieve kernel in its cover mode -- at
+ * each end position the longest match ending there covers every shorter one, so its bytes are OR-ed in and no chain
+ * is walked.  No records, no epilogue, no synchronisation, nothing skipped.  Standard automata only: any other kind
+ * returns ACB_EUNSUPPORTED before any byte is read.  dev_scratch = u64[3], as for acb_count_overlapping.
+ *
+ * acb_match_mask_non_overlapping covers the non-overlapping matches for every match kind: the sieve's list scan (plan
+ * and workspace as for acb_count_non_overlapping), then an epilogue that places the overlapping list, selects each
+ * haystack's matches as acb_pattern_counts_non_overlapping does (stretches of more than ACB_LONG_STRETCH records on the
+ * whole grid) and ORs the selected records' bytes.  ws->dev_total is that call's: [0] = records selected, [1] = 1 when
+ * the mask was written (0: the workspace was too small, NOTHING was OR-ed, and [0] / [4] say how much room a second
+ * call needs), [2] = haystacks selected by the whole grid, [4] = records of the overlapping list.  Two launches, no
+ * synchronisation.
+ *
+ * acb_mask_rows ORs the bytes of rows that are already selected: row_bytes 4 = acb_match records, 8 = int64 rows
+ * (haystack, pattern, start, end), positions haystack-relative bytes; row r covers bits bit_base + dev_offsets[h] +
+ * [start, end).  Rows naming a haystack outside [0, n_haystacks) or an empty span are skipped.  One launch.
+ *
+ * acb_mask_unpack turns bits into bytes: dev_out[i] = bit bit_base + stride * i of dev_mask (0 or 1), i < n.  stride 1
+ * for bytes, ACB_TOKEN_BYTES for token ids (an occurrence starts and ends on a token boundary).  One launch.
+ *
+ * ACB_EINVAL, before any CUDA call: a null pointer (dev_bytes may be null when total_bytes == 0, dev_rows when n_rows
+ * == 0, dev_mask and dev_out when n == 0), n_haystacks outside [0, 2^32 - 2], total_bytes >= 2^31, a malformed filter,
+ * a workspace with a null buffer or a plan acb_plan_scan does not give for these arguments, row_bytes not 4 or 8,
+ * stride 0.
+ */
+int acb_match_mask_overlapping(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                               int64_t n_haystacks, uint64_t total_bytes, uint32_t *dev_mask, uint64_t bit_base, uint64_t *dev_scratch,
+                               void *stream);
+int acb_match_mask_overlapping_filtered(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                                        int64_t n_haystacks, uint64_t total_bytes, uint32_t *dev_mask, uint64_t bit_base,
+                                        uint64_t *dev_scratch, const acb_pattern_filter *filter, void *stream);
+int acb_match_mask_non_overlapping(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes, const int64_t *dev_offsets,
+                                   int64_t n_haystacks, uint64_t total_bytes, const acb_plan *plan, const acb_workspace *ws,
+                                   uint32_t *dev_mask, uint64_t bit_base, void *stream);
+int acb_match_mask_non_overlapping_filtered(const acb_automaton *a, const void *dev_sieve, const uint8_t *dev_bytes,
+                                            const int64_t *dev_offsets, int64_t n_haystacks, uint64_t total_bytes, const acb_plan *plan,
+                                            const acb_workspace *ws, uint32_t *dev_mask, uint64_t bit_base,
+                                            const acb_pattern_filter *filter, void *stream);
+int acb_mask_rows(const void *dev_rows, int row_bytes, uint64_t n_rows, const int64_t *dev_offsets, int64_t n_haystacks, uint32_t *dev_mask,
+                  uint64_t bit_base, void *stream);
+int acb_mask_unpack(const uint32_t *dev_mask, uint64_t bit_base, uint64_t stride, uint64_t n, uint8_t *dev_out, void *stream);
+
 #define ACB_TOKEN_ID_LIMIT (1u << 21)
 #define ACB_TOKEN_BYTES 3
 int acb_tokens_encode(const void *dev_tokens, int token_bytes, uint64_t n_tokens, uint8_t *dev_out, uint64_t *dev_bad, void *stream);
