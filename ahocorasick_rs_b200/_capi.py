@@ -146,6 +146,8 @@ def lib():
         L.acb_match_mask_non_overlapping_filtered.argtypes = L.acb_match_mask_non_overlapping.argtypes[:-1] + [F, C.c_void_p]
         L.acb_mask_rows.argtypes = [C.c_void_p, C.c_int, C.c_uint64, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint64, C.c_void_p]
         L.acb_mask_unpack.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]
+        L.acb_stream_mask_rows.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 7
+        L.acb_stream_mask_emit.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_uint64] + [C.c_void_p] * 10
         _lib = L
     return _lib
 
@@ -185,5 +187,5 @@ EXPORTS = [
     "acb_scan_batch_filtered", "acb_any_match_filtered", "acb_find_first_filtered", "acb_first_rows_filtered",
     "acb_count_overlapping_filtered", "acb_count_non_overlapping_filtered", "acb_stream_first_resolve_filtered",
     "acb_match_mask_overlapping", "acb_match_mask_overlapping_filtered", "acb_match_mask_non_overlapping",
-    "acb_match_mask_non_overlapping_filtered", "acb_mask_rows", "acb_mask_unpack",
+    "acb_match_mask_non_overlapping_filtered", "acb_mask_rows", "acb_mask_unpack", "acb_stream_mask_rows", "acb_stream_mask_emit",
 ]

@@ -2125,6 +2125,115 @@ __global__ void __launch_bounds__(kScanThreads) stream_count_kernel(CountArgs A)
     }
 }
 
+// ---------------------------------------------------------------------------
+// Match-mask streams (acb_stream_mask_rows, acb_stream_mask_emit): which positions of each stream lie inside a match,
+// released once no later data can change them.  After a feed a stream has released [0, R), R = F - T (R = F on
+// `last`); a match covering p < R starts at most p and ends by start + max_pattern_len <= F, so the rows stream has
+// released it for every kind.  The caller keeps the stream search's carry, tail and seams, and the HELD flags: one u8
+// per byte of the tail, the flags of [R, F).  A feed ORs its coverage into two bit spaces, one over the chunk buffer
+// and one over the seam buffer; the emit then writes the flags of [R_old, R_new) and the held flags of [R_new, F_new).
+// Both read the carry as it was before the feed.
+// ---------------------------------------------------------------------------
+struct MaskStreamArgs {
+    const int64_t *offsets;         // [n + 1] the chunks
+    int64_t n;
+    const int64_t *carry;           // [n][kCarryWords] before this feed
+    const int64_t *seam_offsets;    // [n + 1]
+    const uint8_t *last;            // [n] or null
+    uint32_t *chunk_mask, *seam_mask;  // bit q: byte q of the chunk buffer / of the seam buffer
+    const uint8_t *held_in;         // [n][halo]: byte k = the flag of R_old + k, k < T_old
+    uint8_t *held_out;              // [n][halo]: byte k = the flag of R_new + k, k < T_new
+    uint8_t *flags;                 // the released flags, packed by stream
+    int64_t *flag_offsets;          // [n + 1]
+    int64_t *flag_starts;           // [n] the index of each stream's first released position (in units of stride)
+    unsigned long long stride;      // 1: a flag per byte; ACB_TOKEN_BYTES: a flag per token (at its first byte)
+    uint32_t halo;
+    int overlapping;
+};
+
+// stream i's positions: r_old = F_old - T_old, f_new = F_old + chunk length, r_new = what this feed releases up to
+__device__ __forceinline__ void mask_stream_range(const MaskStreamArgs &A, int64_t i, long long &r_old, long long &r_new, long long &f_new) {
+    const int64_t *c = A.carry + kCarryWords * i;
+    r_old = c[kCarryFed] - c[kCarryTail];
+    f_new = c[kCarryFed] + (A.offsets[i + 1] - A.offsets[i]);
+    r_new = (A.last && A.last[i]) ? f_new : f_new - min(f_new, (long long)A.halo);
+}
+
+__device__ __forceinline__ uint32_t mask_bit(const uint32_t *m, unsigned long long q) { return (m[q >> 5] >> (q & 31u)) & 1u; }
+
+// the flag of byte p of stream i, r_old <= p < f_new: in the old tail the held flag OR the seam's bit; in the chunk
+// the chunk's bit, OR (overlapping) the seam's bit when p lies in the head (a match that crosses the cut)
+__device__ __forceinline__ uint32_t mask_stream_flag(const MaskStreamArgs &A, int64_t i, long long p) {
+    const int64_t *c = A.carry + kCarryWords * i;
+    const long long fed = c[kCarryFed], t = c[kCarryTail];
+    if (p < fed) {
+        const long long k = p - (fed - t);
+        return A.held_in[(unsigned long long)i * A.halo + k] | mask_bit(A.seam_mask, (unsigned long long)(A.seam_offsets[i] + k));
+    }
+    const long long k = p - fed;
+    uint32_t f = mask_bit(A.chunk_mask, (unsigned long long)(A.offsets[i] + k));
+    if (A.overlapping && k < (long long)A.halo) f |= mask_bit(A.seam_mask, (unsigned long long)(A.seam_offsets[i] + t + k));
+    return f;
+}
+
+// Non-overlapping: every released row (stream, pattern, start, end; absolute bytes) ORs its bytes into the bit spaces,
+// the part in the old tail [F - T, F) into the seam's and the rest into the chunk's.  A row this feed releases was not
+// released before, so it starts at or after F - T: it lies in tail || chunk.  Grid-stride over all rows.
+__global__ void stream_mask_rows_kernel(MaskStreamArgs A, const long long *rows, const int64_t *row_offsets) {
+    const int64_t total = row_offsets[A.n];
+    for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < total; g += (int64_t)gridDim.x * blockDim.x) {
+        const long long *r = rows + 4 * g;
+        const int64_t i = r[0];
+        const long long s = r[2], e = r[3];
+        const long long fed = A.carry[kCarryWords * i + kCarryFed], t = A.carry[kCarryWords * i + kCarryTail];
+        if (s < fed) or_bits(A.seam_mask, (unsigned long long)(A.seam_offsets[i] + s - (fed - t)), (uint32_t)(min(e, fed) - s));
+        if (e > fed) {
+            const long long c0 = max(s, fed);
+            or_bits(A.chunk_mask, (unsigned long long)(A.offsets[i] + c0 - fed), (uint32_t)(e - c0));
+        }
+    }
+}
+
+// flag_offsets[i + 1] = the positions stream i releases (multiples of stride in [r_old, r_new)), flag_starts[i] = the
+// first one's index
+__global__ void stream_mask_count_kernel(MaskStreamArgs A) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < A.n; i += (int64_t)gridDim.x * blockDim.x) {
+        long long r_old, r_new, f_new;
+        mask_stream_range(A, i, r_old, r_new, f_new);
+        const long long s = (long long)A.stride, first = (r_old + s - 1) / s, end = (r_new + s - 1) / s;
+        A.flag_offsets[i + 1] = end - first;
+        A.flag_starts[i] = first;
+    }
+}
+
+// Every released flag, grid-stride over all of them (one stream with a 256 MiB feed is spread over the whole grid);
+// the stream of flag g by a binary search in flag_offsets, as stream_rows_kernel.  Then the held flags of [r_new,
+// f_new), grid-stride over n * halo.  held_in and held_out are different buffers: a chunk shorter than the tail
+// shifts it.
+__global__ void stream_mask_emit_kernel(MaskStreamArgs A) {
+    const int64_t n = A.n, total = A.flag_offsets[n];
+    const int64_t step = (int64_t)gridDim.x * blockDim.x, first_g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    for (int64_t g = first_g; g < total; g += step) {
+        int64_t i = 0, hi = n - 1;  // the last stream whose flags start at or before g: its flags hold g
+        while (i < hi) {
+            const int64_t mid = (i + hi + 1) >> 1;
+            if (A.flag_offsets[mid] <= g)
+                i = mid;
+            else
+                hi = mid - 1;
+        }
+        const long long p = (A.flag_starts[i] + (g - A.flag_offsets[i])) * (long long)A.stride;
+        A.flags[g] = (uint8_t)mask_stream_flag(A, i, p);
+    }
+    const int64_t held = n * (int64_t)A.halo;
+    for (int64_t q = first_g; q < held; q += step) {
+        const int64_t i = q / A.halo, k = q - i * A.halo;
+        long long r_old, r_new, f_new;
+        mask_stream_range(A, i, r_old, r_new, f_new);
+        if (k < f_new - r_new) A.held_out[q] = (uint8_t)mask_stream_flag(A, i, r_new + k);
+    }
+}
+
 }  // namespace acb
 
 // ===========================================================================
@@ -3694,6 +3803,78 @@ int acb_stream_count(const acb_automaton *a, const uint8_t *dev_bytes, const int
     const void *kern = A.S.mode == kModeStandard ? reinterpret_cast<const void *>(stream_count_kernel<kModeStandard>)
                                                  : reinterpret_cast<const void *>(stream_count_kernel<kModeLeftmost>);
     if (int rc = launch_cooperative(kern, args, d, st)) return rc;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+int acb_stream_mask_rows(const int64_t *dev_offsets, int64_t n_streams, const int64_t *dev_carry_before, const int64_t *dev_seam_offsets,
+                         const int64_t *dev_rows, const int64_t *dev_row_offsets, uint32_t *dev_chunk_mask, uint32_t *dev_seam_mask,
+                         void *stream) {
+    if (!dev_offsets || !dev_carry_before || !dev_seam_offsets || !dev_rows || !dev_row_offsets || !dev_chunk_mask || !dev_seam_mask)
+        return fail(ACB_EINVAL, "null argument");
+    if (n_streams < 0 || n_streams > 0xfffffffell) return fail(ACB_EINVAL, "n_streams out of range (0 .. 2^32 - 2)");
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    if (n_streams == 0) return ACB_OK;
+    MaskStreamArgs A = {};
+    A.offsets = dev_offsets;
+    A.n = n_streams;
+    A.carry = dev_carry_before;
+    A.seam_offsets = dev_seam_offsets;
+    A.chunk_mask = dev_chunk_mask;
+    A.seam_mask = dev_seam_mask;
+    // the row count is on the device only: a grid of 8 blocks per SM, grid-stride over the rows
+    stream_mask_rows_kernel<<<(unsigned)(8 * d.sms), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        A, reinterpret_cast<const long long *>(dev_rows), dev_row_offsets);
+    g_launches++;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+int acb_stream_mask_emit(const acb_automaton *a, const int64_t *dev_offsets, int64_t n_streams, const uint8_t *dev_last, int overlapping,
+                         uint64_t stride, const int64_t *dev_carry_before, const int64_t *dev_seam_offsets, const uint32_t *dev_chunk_mask,
+                         const uint32_t *dev_seam_mask, const uint8_t *dev_held_in, uint8_t *dev_held_out, uint8_t *dev_flags,
+                         int64_t *dev_flag_offsets, int64_t *dev_flag_starts, void *stream) {
+    if (!a || !dev_offsets || !dev_carry_before || !dev_seam_offsets || !dev_chunk_mask || !dev_seam_mask || !dev_flags || !dev_flag_offsets ||
+        !dev_flag_starts)
+        return fail(ACB_EINVAL, "null argument");
+    const uint32_t halo = a->impl->hdr.max_pat_len ? a->impl->hdr.max_pat_len - 1 : 0;
+    if (halo && (!dev_held_in || !dev_held_out)) return fail(ACB_EINVAL, "null argument");
+    if (halo && dev_held_in == dev_held_out) return fail(ACB_EINVAL, "dev_held_in and dev_held_out must be different buffers");
+    if (overlapping != 0 && overlapping != 1) return fail(ACB_EINVAL, "overlapping must be 0 or 1");
+    if (stride == 0 || stride > 0xffffffffull) return fail(ACB_EINVAL, "stride out of range (1 .. 2^32 - 1)");
+    if (n_streams < 0 || n_streams > 0xfffffffell) return fail(ACB_EINVAL, "n_streams out of range (0 .. 2^32 - 2)");
+    if (overlapping && (int)a->impl->hdr.match_kind != ACB_STANDARD) return unsupported_overlapping(a);
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (n_streams == 0) {
+        CUDA_OK(cudaMemsetAsync(dev_flag_offsets, 0, sizeof(int64_t), st));
+        return ACB_OK;
+    }
+    MaskStreamArgs A = {};
+    A.offsets = dev_offsets;
+    A.n = n_streams;
+    A.carry = dev_carry_before;
+    A.seam_offsets = dev_seam_offsets;
+    A.last = dev_last;
+    A.chunk_mask = const_cast<uint32_t *>(dev_chunk_mask);
+    A.seam_mask = const_cast<uint32_t *>(dev_seam_mask);
+    A.held_in = dev_held_in;
+    A.held_out = dev_held_out;
+    A.flags = dev_flags;
+    A.flag_offsets = dev_flag_offsets;
+    A.flag_starts = dev_flag_starts;
+    A.stride = stride;
+    A.halo = halo;
+    A.overlapping = overlapping;
+    int64_t blocks = (n_streams + 255) / 256;
+    if (blocks > 8ll * d.sms) blocks = 8ll * d.sms;
+    stream_mask_count_kernel<<<(unsigned)blocks, 256, 0, st>>>(A);
+    stream_prefix_kernel<<<1, kScanThreads, 0, st>>>(dev_flag_offsets, n_streams);
+    // the flag count is on the device only: a grid of 8 blocks per SM, grid-stride over the flags and the held bytes
+    stream_mask_emit_kernel<<<(unsigned)(8 * d.sms), 256, 0, st>>>(A);
+    g_launches += 3;
     CUDA_OK(cudaGetLastError());
     return ACB_OK;
 }

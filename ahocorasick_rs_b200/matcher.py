@@ -2164,6 +2164,106 @@ class CountStreamBatch(_QueryStreamBatch):
         return counts, {"records": records, "held": held, "long_stretches": long_stretches}
 
 
+class MaskStreamBatch(_QueryStreamBatch):
+    """Match masks per stream: after each feed, the flags of the positions no later data can change.  With halo =
+    max_pattern_len - 1 and F the bytes stream i has been fed, it has released the positions whose first byte lies below
+    R = max(0, F - halo) (all of them on `last`, after which the slot starts again at 0).  A released flag is final: it
+    equals match_mask_device of the whole concatenation at that position (overlapping or not; with pattern sets, the
+    stream's set).  feed_device returns (flags bool (k,), flag_offsets int64 (n_streams + 1), flag_starts int64
+    (n_streams,)): stream i's flags are flags[flag_offsets[i]:flag_offsets[i + 1]], for its positions flag_starts[i],
+    flag_starts[i] + 1, ...  A flag per byte, or per token id (stride = ACB_TOKEN_BYTES) for TokenAhoCorasick.
+
+    Overlapping: the sieve's cover mode on the chunks and on the seams, no list.  Non-overlapping: the stream search's
+    two list scans and resolve, then acb_stream_mask_rows.  Then acb_stream_mask_emit (include/acb200.h)."""
+
+    MODE = "match_mask_stream"
+
+    def __init__(self, ac: "_Automaton", n_streams: int, overlapping: bool, stride: int = 1):
+        super().__init__(ac, n_streams, overlapping, codepoints=False)
+        self._stride = stride
+
+    def _allocate_query(self, dev):
+        torch = _torch()
+        size = max(self.n_streams * self._halo, 1)
+        self._held = (torch.zeros(size, dtype=torch.uint8, device=dev), torch.zeros(size, dtype=torch.uint8, device=dev))
+
+    def feed_device(self, data, offsets, last=None):
+        torch = _torch()
+        dev, data, offsets, last_u8 = self._feed_args(data, offsets, last)
+        ac, L, n = self._ac, self._ac._L, self.n_streams
+        flt = _filter_struct(self._flt)
+        with self._lock, ac._lock, torch.cuda.device(dev):
+            if self.device is None:
+                self._allocate(dev)
+                self._allocate_query(dev)
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            last_p = last_u8.data_ptr() if last_u8 is not None else None
+            rc = L.acb_stream_seams(ac._h, data.data_ptr(), offsets.data_ptr(), n, data.numel(), self._carry.data_ptr(),
+                                    self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(), stream)
+            if rc != _capi.ACB_OK:
+                raise RuntimeError(_capi.last_error())
+            chunk_bits = torch.zeros(max((data.numel() + 31) // 32, 1), dtype=torch.int32, device=dev)
+            seam_bits = torch.zeros(max((self._seam.numel() + 31) // 32, 1), dtype=torch.int32, device=dev)
+            if self.overlapping:
+                carry_before = self._carry   # the emit runs before the advance
+                sieve_t = ac.sieve(dev)[0]
+                scratch = torch.empty(3, dtype=torch.int64, device=dev)
+                for b, o, w in ((data, offsets, chunk_bits), (self._seam, self._seam_offsets, seam_bits)):
+                    rc = L.acb_match_mask_overlapping_filtered(ac._h, sieve_t.data_ptr(), b.data_ptr(), o.data_ptr(), n, b.numel(),
+                                                               w.data_ptr(), 0, scratch.data_ptr(), flt, stream)
+                    if rc != _capi.ACB_OK:
+                        raise RuntimeError(_capi.last_error())
+                stats = {}
+            else:
+                # the overlapping lists, in bytes, of the chunks as they are and of the seams (as StreamBatch.feed_device)
+                m_c, mo_c, tot_c = ac.scan_device(data, offsets, 2, False, ws_slot=self._slots[0], flt=self._flt)
+                m_s, mo_s, tot_s = ac.scan_device(self._seam, self._seam_offsets, 2, False, ws_slot=self._slots[1], flt=self._flt)
+                if m_c.dtype != torch.int32 or m_s.dtype != torch.int32:
+                    raise RuntimeError("match-mask stream: a list came back in the windowed int64 form acb_stream_resolve cannot read")
+                cap = int(tot_c) + int(tot_s)
+
+                def ptr(t):   # an empty list is still a view of its workspace's buffer: pass that buffer's (non-null) address
+                    return t.data_ptr() if t.numel() else t.untyped_storage().data_ptr() + t.storage_offset() * t.element_size()
+
+                carry_before = self._carry.clone()   # the resolve moves the carry (and zeroes it on `last`)
+                scratch = torch.empty(2 + 6 * n + 4 * cap, dtype=torch.int64, device=dev)
+                rows = torch.empty((max(cap, 1), 4), dtype=torch.int64, device=dev)
+                row_offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
+                rc = L.acb_stream_resolve(ac._h, None, data.data_ptr(), offsets.data_ptr(), n, data.numel(), last_p, 0, 0,
+                                          self._carry.data_ptr(), self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(),
+                                          ptr(m_s), mo_s.data_ptr(), ptr(m_c), mo_c.data_ptr(), scratch.data_ptr(), rows.data_ptr(),
+                                          row_offsets.data_ptr(), stream)
+                if rc != _capi.ACB_OK:
+                    raise RuntimeError(_capi.last_error())
+                rc = L.acb_stream_mask_rows(offsets.data_ptr(), n, carry_before.data_ptr(), self._seam_offsets.data_ptr(), rows.data_ptr(),
+                                            row_offsets.data_ptr(), chunk_bits.data_ptr(), seam_bits.data_ptr(), stream)
+                if rc != _capi.ACB_OK:
+                    raise RuntimeError(_capi.last_error())
+                stats = {"records": scratch[0]}
+            flags = torch.empty(max(data.numel() + n * self._halo, 1), dtype=torch.bool, device=dev)
+            flag_offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
+            flag_starts = torch.empty(n, dtype=torch.int64, device=dev)
+            held_in, held_out = self._held
+            rc = L.acb_stream_mask_emit(ac._h, offsets.data_ptr(), n, last_p, int(self.overlapping), self._stride, carry_before.data_ptr(),
+                                        self._seam_offsets.data_ptr(), chunk_bits.data_ptr(), seam_bits.data_ptr(), held_in.data_ptr(),
+                                        held_out.data_ptr(), flags.data_ptr(), flag_offsets.data_ptr(), flag_starts.data_ptr(), stream)
+            if rc != _capi.ACB_OK:
+                raise (ValueError if rc == _capi.ACB_EUNSUPPORTED else RuntimeError)(_capi.last_error())
+            self._held = (held_out, held_in)
+            if self.overlapping:
+                rc = L.acb_stream_advance(ac._h, data.data_ptr(), offsets.data_ptr(), n, data.numel(), last_p, 0, self._carry.data_ptr(),
+                                          self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(), None, stream)
+                if rc != _capi.ACB_OK:
+                    raise RuntimeError(_capi.last_error())
+            counts = torch.stack([flag_offsets[n], self._seam_offsets[n], self._carry[:, 2].sum(), *stats.values()]).tolist()
+            k, seam_bytes, held = counts[:3]
+            task_bytes = int(ac._plan(data, max(n, 1)).task_bytes)
+            self.last_stats = {"engine": "sieve", "mode": self.MODE, **ac.sieve_geometry(dev, task_bytes), "seam_bytes": seam_bytes,
+                               "released": k, "held": held, **dict(zip(stats, counts[3:])), **ac._set_stats(self._flt)}
+        ac.last_stats = dict(self.last_stats)
+        return flags[:k], flag_offsets, flag_starts
+
+
 class QueryStream:
     """One query stream fed from the host (a query batch of one, with its own pinned staging buffer): feed(chunk) and
     finish() return the answer after the feed (see the batch classes); finish() ends the stream."""
@@ -2217,6 +2317,76 @@ class QueryStream:
         if last:
             self._done = True
         return ans
+
+
+class MaskStream(QueryStream):
+    """One match-mask stream fed from the host (a MaskStreamBatch of one): feed(chunk) returns the runs [(start, end),
+    ...] of covered positions inside the range this feed released, clipped to it, in the class's unit (code points,
+    bytes or tokens); finish() returns the rest and ends the stream.  Merging every feed's runs that touch at a feed
+    boundary gives match_spans(concatenation, overlapping, patterns).  For str chunks a code point is released with its
+    lead byte: the stream keeps the bytes fed but not released, to tell lead bytes from continuation bytes."""
+
+    def __init__(self, batch: MaskStreamBatch, codepoints: bool):
+        super().__init__(batch, None)
+        self._codepoints = codepoints
+        self._pending = np.zeros(0, dtype=np.uint8)   # str: the bytes [R, F), fed but not released
+        self._released = 0
+
+    @property
+    def released(self) -> int:
+        """The positions released so far (code points, bytes or tokens)."""
+        return self._released
+
+    def _feed(self, chunk, last: bool):
+        if self._done:
+            raise RuntimeError("the stream is finished: feed after finish()")
+        n = len(chunk)
+        ac = self._batch._ac
+        if n > ac.WINDOW_BYTES:
+            raise ValueError(f"one feed addresses at most {ac.WINDOW_BYTES} bytes (WINDOW_BYTES): feed larger data in more chunks")
+        torch = _require_cuda()
+        dev = self._batch.device or torch.device("cuda", torch.cuda.current_device())
+        if self._offs is None:
+            self._offs = torch.zeros(2, dtype=torch.int64, device=dev)
+        with self._lock:   # the staging buffer is reused once the flags are on the host
+            if self._pinned is None or self._pinned.numel() < n:
+                self._pinned = torch.empty(max(n, 1 << 16), dtype=torch.uint8, pin_memory=True)
+            host = self._pinned
+            if n:
+                host.numpy()[:n] = np.frombuffer(chunk, dtype=np.uint8)
+            d = host[:n].to(dev, non_blocking=True)
+            self._offs[1] = n
+            flags, _, _ = self._batch.feed_device(d, self._offs, torch.ones(1, dtype=torch.bool, device=dev) if last else None)
+            flags = flags.cpu().numpy()
+            if self._codepoints:   # a flag per byte: keep those of lead bytes, one per code point
+                text = np.concatenate([self._pending, host.numpy()[:n]])
+                self._pending = text[flags.size:]
+                flags = flags[(text[:flags.size] & 0xC0) != 0x80]
+        start = self._released   # each feed's positions follow the last feed's
+        self._released += flags.size
+        if last:
+            self._done = True
+        prev = np.concatenate([[False], flags])
+        nxt = np.concatenate([flags, [False]])
+        return list(zip((np.flatnonzero(nxt & ~prev) + start).tolist(), (np.flatnonzero(prev & ~nxt) + start).tolist()))
+
+
+def _mask_stream_batch(ac, n_streams: int, overlapping: bool, pattern_sets=None, set_index=None, stride: int = 1) -> MaskStreamBatch:
+    """A match-mask batch; pattern_sets= / set_index= fix each stream's pattern set for the batch's life."""
+    batch = MaskStreamBatch(ac, n_streams, overlapping, stride)
+    if pattern_sets is not None or set_index is not None:
+        dev = pattern_sets.device if isinstance(pattern_sets, PatternSets) else None
+        batch._flt = _filter_args(ac, pattern_sets, set_index, n_streams, dev)
+    return batch
+
+
+def _mask_stream(ac, overlapping: bool, codepoints: bool, patterns=None, stride: int = 1) -> MaskStream:
+    """A host-fed match-mask stream; `patterns`: the stream's pattern ids, or None."""
+    if patterns is None:
+        return MaskStream(_mask_stream_batch(ac, 1, overlapping, stride=stride), codepoints)
+    torch = _require_cuda()
+    ps = PatternSets(ac, [patterns])
+    return MaskStream(_mask_stream_batch(ac, 1, overlapping, ps, torch.zeros(1, dtype=torch.int32, device=ps.device), stride), codepoints)
 
 
 def _first_answer(row):
@@ -2586,6 +2756,17 @@ class AhoCorasick(_PatternSetMethods):
         self._ac.check_overlapping(overlapping)
         return _query_stream(self._ac, "count", overlapping, codepoints=True)
 
+    def match_mask_stream_batch(self, n_streams: int, overlapping: bool = False, pattern_sets=None, set_index=None) -> MaskStreamBatch:
+        """``n_streams`` match-mask streams fed from the device: ``feed_device(data, offsets, last=None)`` -> (flags,
+        flag_offsets, flag_starts), a flag per byte for each stream's bytes that no later data can change (see
+        MaskStreamBatch).  pattern_sets= / set_index= (n_streams,): stream i searches only for set set_index[i]."""
+        return _mask_stream_batch(self._ac, n_streams, overlapping, pattern_sets, set_index)
+
+    def match_spans_stream(self, overlapping: bool = False, patterns=None) -> MaskStream:
+        """One match-mask stream fed ``str`` chunks: ``feed(chunk)`` -> the runs (start, end) of covered code points
+        this feed released, ``finish()`` -> the rest (see MaskStream).  `patterns`: search only for these ids."""
+        return _mask_stream(self._ac, overlapping, True, patterns)
+
     def scan_host(self, data, offsets, overlapping: bool = False, **kw):
         """Host-resident UTF-8 batch (uint8 array + int64 offsets) -> host arrays (matches (k, 4), match_offsets (n + 1));
         code point indexes.  Copies and scans are pipelined (see _Automaton.scan_host)."""
@@ -2785,6 +2966,17 @@ class BytesAhoCorasick(_PatternSetMethods):
         self._ac.check_overlapping(overlapping)
         return _query_stream(self._ac, "count", overlapping, codepoints=False)
 
+    def match_mask_stream_batch(self, n_streams: int, overlapping: bool = False, pattern_sets=None, set_index=None) -> MaskStreamBatch:
+        """``n_streams`` match-mask streams fed from the device: ``feed_device(data, offsets, last=None)`` -> (flags,
+        flag_offsets, flag_starts), a flag per byte for each stream's bytes that no later data can change (see
+        MaskStreamBatch).  pattern_sets= / set_index= (n_streams,): stream i searches only for set set_index[i]."""
+        return _mask_stream_batch(self._ac, n_streams, overlapping, pattern_sets, set_index)
+
+    def match_spans_stream(self, overlapping: bool = False, patterns=None) -> MaskStream:
+        """One match-mask stream fed bytes-like chunks: ``feed(chunk)`` -> the runs (start, end) of covered bytes this
+        feed released, ``finish()`` -> the rest (see MaskStream).  `patterns`: search only for these ids."""
+        return _mask_stream(self._ac, overlapping, False, patterns)
+
     def scan_host(self, data, offsets, overlapping: bool = False, **kw):
         """Host-resident batch (uint8 array + int64 offsets) -> host arrays (matches (k, 4), match_offsets (n + 1));
         byte offsets.  Copies and scans are pipelined (see _Automaton.scan_host)."""
@@ -2979,6 +3171,12 @@ class TokenStream:
 
     def finish(self):
         return self._convert(self._stream._feed(b"", True))
+
+
+class TokenMaskStream(TokenStream):
+    """A MaskStream fed host chunks of token ids; `released` counts tokens."""
+
+    released = property(lambda self: self._stream.released)
 
 
 def _same(x):
@@ -3234,6 +3432,19 @@ class TokenAhoCorasick(_PatternSetMethods):
     def count_matches_stream(self, overlapping: bool = False) -> TokenStream:
         self._ac.check_overlapping(overlapping)
         return self._query_stream("count", overlapping)
+
+    def match_mask_stream_batch(self, n_streams: int, overlapping: bool = False, pattern_sets=None, set_index=None) -> TokenStreamBatch:
+        """``feed_device(tokens, offsets, last=None)`` -> (flags, flag_offsets, flag_starts), a flag per token for each
+        stream's tokens that no later ids can change: all but the last k - 1 fed, k the longest pattern in tokens (see
+        MaskStreamBatch).  Masking banned sequences as a model emits them.  pattern_sets= / set_index= (n_streams,)."""
+        _token_stream_limits(self._ac, n_streams)
+        return TokenStreamBatch(_mask_stream_batch(self._ac, n_streams, overlapping, pattern_sets, set_index, _capi.ACB_TOKEN_BYTES), _same)
+
+    def match_spans_stream(self, overlapping: bool = False, patterns=None) -> "TokenMaskStream":
+        """One match-mask stream fed host chunks of ids: ``feed(chunk)`` -> the runs (start, end) of covered tokens this
+        feed released, ``finish()`` -> the rest (see MaskStream)."""
+        _token_stream_limits(self._ac, 1)
+        return TokenMaskStream(_mask_stream(self._ac, overlapping, False, patterns, _capi.ACB_TOKEN_BYTES), _same)
 
 
 def _token_tuples_of_rows(rows):

@@ -650,6 +650,52 @@ int acb_mask_rows(const void *dev_rows, int row_bytes, uint64_t n_rows, const in
                   uint64_t bit_base, void *stream);
 int acb_mask_unpack(const uint32_t *dev_mask, uint64_t bit_base, uint64_t stride, uint64_t n, uint8_t *dev_out, void *stream);
 
+/*
+ * Match-mask streams: the match mask of each stream's concatenation, flag by flag, released once no later data can
+ * change it.  Let halo = acb_max_pattern_len - 1 and F the bytes a stream has been fed.  After a feed the stream has
+ * released the positions [0, R), R = F - T = max(0, F - halo) (T = dev_carry[2]); a feed with dev_last[i] != 0 sets
+ * R = F, releases everything still held and starts the slot again at position 0.  A released flag is final: it equals
+ * the mask of the whole concatenation (acb_match_mask_*, overlapping or not, with a filter the stream's set).  A match
+ * covering p < R starts at most p, so start + max_pattern_len <= F and end <= F: the stream search has released it.
+ *
+ * State: the stream search's dev_carry, dev_tail and seams (above), and the HELD flags, uint8[n_streams][halo] twice:
+ * byte k of stream i's row in the read buffer is the flag of position R + k, k < T.  Each feed reads one buffer and
+ * writes the other (a chunk shorter than the tail shifts it); the caller swaps them.  Both zero-filled at first (may
+ * be null when halo == 0).  A feed, on one CUDA stream, with dev_chunk_mask = u32[ceil(total_bytes / 32)] and
+ * dev_seam_mask = u32[ceil(seam buffer bytes / 32)] zero-filled for it (bit q: byte q of that buffer):
+ *   1. acb_stream_seams.
+ *   2. overlapping = 1 (Standard): acb_match_mask_overlapping(_filtered) on the chunks into dev_chunk_mask and on the
+ *      seams into dev_seam_mask, bit_base 0.  Every match that ends past the old F lies wholly in one of them; matches
+ *      that end before were OR-ed by earlier feeds, and their bits past the old R are in the held flags.
+ *      overlapping = 0 (every kind): the stream search's two list scans and acb_stream_resolve with codepoints = 0,
+ *      after copying dev_carry (int64[n_streams][4]) to dev_carry_before; then acb_stream_mask_rows ORs each released
+ *      row into the bit spaces: the part in the old tail into dev_seam_mask, the rest into dev_chunk_mask.  A row this
+ *      feed releases starts at or after the old R, so it lies in old tail || chunk.  One launch, grid-stride over the
+ *      rows (their count is read on the device).
+ *   3. acb_stream_mask_emit writes the flags of the positions in [R_old, R_new) that are multiples of stride (1: a flag
+ *      per byte; ACB_TOKEN_BYTES: a flag per token id, read at its first byte), packed by stream into dev_flags (room
+ *      for total_bytes + n_streams * halo flags), dev_flag_offsets = int64[n_streams + 1] bracketing each stream's and
+ *      dev_flag_starts = int64[n_streams] = the index of each stream's first one (ceil(R_old / stride)).  The flag of
+ *      byte p is, in the old tail, its held flag OR its seam bit; in the chunk, its chunk bit OR (overlapping = 1) the
+ *      seam bit of the head byte it is.  It writes the held flags of [R_new, F_new) to dev_held_out.  It reads F and T
+ *      from dev_carry_before, the carry as it was before this feed: dev_carry itself on the overlapping path, where it
+ *      runs before step 4; the copy on the other, whose resolve has already moved the carry (and zeroed it on
+ *      dev_last).  Three launches (count, prefix, the flags and held flags on the whole grid), no synchronisation.
+ *   4. overlapping = 1: acb_stream_advance (codepoints = 0).  overlapping = 0: nothing, the resolve advanced the carry.
+ *
+ * ACB_EINVAL, before any CUDA call: a null pointer (dev_last may be null: no stream ends; the held buffers when halo
+ * == 0), the same buffer for dev_held_in and dev_held_out, overlapping other than 0 / 1, stride outside [1, 2^32 - 1],
+ * n_streams outside [0, 2^32 - 2].  acb_stream_mask_emit returns ACB_EUNSUPPORTED for overlapping = 1 on a leftmost
+ * automaton.  n_streams == 0 launches nothing (the emit zeroes dev_flag_offsets[0]).
+ */
+int acb_stream_mask_rows(const int64_t *dev_offsets, int64_t n_streams, const int64_t *dev_carry_before, const int64_t *dev_seam_offsets,
+                         const int64_t *dev_rows, const int64_t *dev_row_offsets, uint32_t *dev_chunk_mask, uint32_t *dev_seam_mask,
+                         void *stream);
+int acb_stream_mask_emit(const acb_automaton *a, const int64_t *dev_offsets, int64_t n_streams, const uint8_t *dev_last, int overlapping,
+                         uint64_t stride, const int64_t *dev_carry_before, const int64_t *dev_seam_offsets, const uint32_t *dev_chunk_mask,
+                         const uint32_t *dev_seam_mask, const uint8_t *dev_held_in, uint8_t *dev_held_out, uint8_t *dev_flags,
+                         int64_t *dev_flag_offsets, int64_t *dev_flag_starts, void *stream);
+
 #define ACB_TOKEN_ID_LIMIT (1u << 21)
 #define ACB_TOKEN_BYTES 3
 int acb_tokens_encode(const void *dev_tokens, int token_bytes, uint64_t n_tokens, uint8_t *dev_out, uint64_t *dev_bad, void *stream);
