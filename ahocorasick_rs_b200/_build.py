@@ -13,8 +13,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libacb200.so")
 STAMP = LIB + ".cmd"
-SOURCES = ["capi.cu", "automaton.cpp", "sieve.cpp"]
-HEADERS = ["automaton.h", "scan_core.cuh", "scan_staged.cuh", "scan_global.cuh", "scan_sieve.cuh", "sieve.h", "repair.cuh", "tokens.cuh", os.path.join("..", "..", "include", "acb200.h")]
+SOURCES = ["capi.cu", "automaton.cpp", "sieve.cpp", "completions.cpp"]
+HEADERS = ["automaton.h", "scan_core.cuh", "scan_staged.cuh", "scan_global.cuh", "scan_sieve.cuh", "sieve.h", "repair.cuh", "tokens.cuh", "completions.h", "completions.cuh", os.path.join("..", "..", "include", "acb200.h")]
 FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-diag-suppress", "186",
          "-shared", "-Xcompiler", "-fPIC,-pthread"]
 

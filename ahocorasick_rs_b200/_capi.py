@@ -14,6 +14,7 @@ ACB_OK = 0
 ACB_EINVAL, ACB_EBUILD, ACB_EUNSUPPORTED, ACB_ECUDA, ACB_ECAPACITY = -1, -2, -3, -4, -5
 ACB_TOKEN_ID_LIMIT = 1 << 21   # include/acb200.h: token ids lie in [0, ACB_TOKEN_ID_LIMIT)
 ACB_TOKEN_BYTES = 3            # ... and each becomes this many bytes (csrc/tokens.cuh)
+ACB_LOGITS_F32, ACB_LOGITS_F16, ACB_LOGITS_BF16 = 0, 1, 2   # include/acb200.h: acb_completions_mask's logits dtypes
 ACB_LONG_STRETCH = 4096   # include/acb200.h: longer per-haystack overlapping lists are counted by the whole grid
 
 
@@ -41,6 +42,10 @@ class Tuning(C.Structure):
 class SieveDesc(C.Structure):
     _fields_ = [("window", C.c_uint32), ("last_level", C.c_uint32), ("probes", C.c_uint32), ("bloom_bytes", C.c_uint32),
                 ("nodes", C.c_uint32), ("keys", C.c_uint32), ("filter_entries", C.c_uint32), ("table_slots", C.c_uint32)]
+
+
+class CompletionsDesc(C.Structure):
+    _fields_ = [("nodes", C.c_uint32), ("entries", C.c_uint32), ("depth", C.c_uint32), ("max_last", C.c_uint32)]
 
 
 class HotDesc(C.Structure):
@@ -148,6 +153,13 @@ def lib():
         L.acb_mask_unpack.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]
         L.acb_stream_mask_rows.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 7
         L.acb_stream_mask_emit.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_uint64] + [C.c_void_p] * 10
+        L.acb_completions_build.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+        L.acb_completions_write.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
+        L.acb_completions_describe.argtypes = [C.c_void_p, C.POINTER(CompletionsDesc)]
+        compl = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_uint64, C.c_void_p, C.c_int64]
+        L.acb_completions_count.argtypes = compl + [C.c_void_p, F, C.c_void_p]
+        L.acb_completions_emit.argtypes = compl + [C.c_void_p, C.c_void_p, F, C.c_void_p]
+        L.acb_completions_mask.argtypes = compl + [C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_float, F, C.c_void_p]
         _lib = L
     return _lib
 
@@ -188,4 +200,6 @@ EXPORTS = [
     "acb_count_overlapping_filtered", "acb_count_non_overlapping_filtered", "acb_stream_first_resolve_filtered",
     "acb_match_mask_overlapping", "acb_match_mask_overlapping_filtered", "acb_match_mask_non_overlapping",
     "acb_match_mask_non_overlapping_filtered", "acb_mask_rows", "acb_mask_unpack", "acb_stream_mask_rows", "acb_stream_mask_emit",
+    "acb_completions_build", "acb_completions_write", "acb_completions_describe", "acb_completions_count", "acb_completions_emit",
+    "acb_completions_mask",
 ]

@@ -83,6 +83,7 @@ struct Automaton {
     std::mutex sieve_mutex;
     std::vector<uint8_t> sieve;       // built by acb_sieve_build
     uint32_t sieve_bloom_max = 0, sieve_w_max = 0;
+    std::vector<uint8_t> completions; // built by acb_completions_build (token-format patterns only), under sieve_mutex
 };
 
 // Builds the automaton; throws std::runtime_error with a message on failure.

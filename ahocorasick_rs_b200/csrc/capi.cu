@@ -15,6 +15,7 @@
 #include "scan_global.cuh"
 #include "scan_sieve.cuh"
 #include "tokens.cuh"
+#include "completions.cuh"
 
 namespace acb {
 
@@ -3875,6 +3876,190 @@ int acb_stream_mask_emit(const acb_automaton *a, const int64_t *dev_offsets, int
     // the flag count is on the device only: a grid of 8 blocks per SM, grid-stride over the flags and the held bytes
     stream_mask_emit_kernel<<<(unsigned)(8 * d.sms), 256, 0, st>>>(A);
     g_launches += 3;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+}  // extern "C"
+
+// ===========================================================================
+// Completing tokens (completions.h, completions.cuh)
+// ===========================================================================
+template <typename T, typename L, int MODE, bool FILT>
+static void completions_launch(const ComplView &V, const void *tokens, uint64_t n_tokens, const int64_t *offsets, int64_t n_rows,
+                               const SieveFilter &F, void *logits, int64_t row_stride, int64_t vocab, float value, int64_t *out,
+                               const int64_t *out_offsets, int sms, cudaStream_t st) {
+    constexpr int64_t kWarps = kComplThreads / 32;
+    int64_t blocks = (n_rows + kWarps - 1) / kWarps;
+    if (blocks > 32ll * sms) blocks = 32ll * sms;   // grid-stride beyond that
+    completions_kernel<T, L, MODE, FILT><<<(unsigned)blocks, kComplThreads, 0, st>>>(
+        V, static_cast<const T *>(tokens), n_tokens, offsets, n_rows, F, static_cast<L *>(logits), row_stride, vocab, value, out, out_offsets);
+}
+
+template <typename L, int MODE>
+static void completions_dispatch(int token_bytes, bool filt, const ComplView &V, const void *tokens, uint64_t n_tokens,
+                                 const int64_t *offsets, int64_t n_rows, const SieveFilter &F, void *logits, int64_t row_stride,
+                                 int64_t vocab, float value, int64_t *out, const int64_t *out_offsets, int sms, cudaStream_t st) {
+#define ACB_COMPL_LAUNCH(T, FL) \
+    completions_launch<T, L, MODE, FL>(V, tokens, n_tokens, offsets, n_rows, F, logits, row_stride, vocab, value, out, out_offsets, sms, st)
+    if (token_bytes == 2) {
+        if (filt) ACB_COMPL_LAUNCH(uint16_t, true); else ACB_COMPL_LAUNCH(uint16_t, false);
+    } else if (token_bytes == 4) {
+        if (filt) ACB_COMPL_LAUNCH(int32_t, true); else ACB_COMPL_LAUNCH(int32_t, false);
+    } else {
+        if (filt) ACB_COMPL_LAUNCH(int64_t, true); else ACB_COMPL_LAUNCH(int64_t, false);
+    }
+#undef ACB_COMPL_LAUNCH
+}
+
+extern "C" {
+
+int acb_completions_build(acb_automaton *a, uint64_t *image_bytes) {
+    if (!a || !image_bytes) return fail(ACB_EINVAL, "null argument");
+    Automaton &A = *a->impl;
+    std::lock_guard<std::mutex> lock(A.sieve_mutex);
+    if (A.completions.empty()) {
+        // the patterns must be in the token format: whole 3-byte groups, each some id's token_code
+        const uint64_t n = A.hdr.n_patterns;
+        std::vector<uint32_t> ids;
+        std::vector<uint64_t> offs(n + 1, 0);
+        ids.reserve(A.pat_blob.size() / ACB_TOKEN_BYTES);
+        for (uint64_t i = 0; i < n; i++) {
+            const uint64_t s = A.pat_offs[i], e = A.pat_offs[i + 1];
+            if ((e - s) % ACB_TOKEN_BYTES) return fail(ACB_EINVAL, "pattern " + std::to_string(i) + " is not in the token format (length not a multiple of 3)");
+            for (uint64_t k = s; k < e; k += ACB_TOKEN_BYTES) {
+                uint32_t t;
+                if (!token_decode(A.pat_blob[k], A.pat_blob[k + 1], A.pat_blob[k + 2], t))
+                    return fail(ACB_EINVAL, "pattern " + std::to_string(i) + " is not in the token format (byte " + std::to_string(k - s) + ")");
+                ids.push_back(t);
+            }
+            offs[i + 1] = ids.size();
+        }
+        try {
+            completions_image_build(ids.data(), offs.data(), n, A.completions);
+        } catch (const std::exception &e) {
+            A.completions.clear();
+            return fail(ACB_EBUILD, e.what());
+        }
+    }
+    *image_bytes = A.completions.size();
+    return ACB_OK;
+}
+
+int acb_completions_write(acb_automaton *a, void *host_dst, uint64_t dst_bytes) {
+    if (!a || !host_dst) return fail(ACB_EINVAL, "null argument");
+    Automaton &A = *a->impl;
+    std::lock_guard<std::mutex> lock(A.sieve_mutex);
+    if (A.completions.empty()) return fail(ACB_EINVAL, "acb_completions_build has not been called");
+    if (dst_bytes < A.completions.size()) return fail(ACB_ECAPACITY, "completions image buffer too small");
+    std::memcpy(host_dst, A.completions.data(), A.completions.size());
+    return ACB_OK;
+}
+
+int acb_completions_describe(const void *host_image, acb_completions_desc *d) {
+    const ComplHeader *h = static_cast<const ComplHeader *>(host_image);
+    if (!h || !d || h->magic != kComplMagic) return fail(ACB_EINVAL, "not a completions image");
+    d->nodes = h->n_nodes;
+    d->entries = h->n_entries;
+    d->depth = h->depth;
+    d->max_last = h->max_last;
+    return ACB_OK;
+}
+
+}  // extern "C"
+
+// the checks every completions entry point makes, before any CUDA call; the host header and the filter view
+static int completions_check(const acb_automaton *a, const void *dev_image, const void *dev_tokens, int token_bytes, uint64_t n_tokens,
+                             const int64_t *dev_offsets, int64_t n_rows, const acb_pattern_filter *filter, ComplHeader &h,
+                             SieveFilter &F, bool &filt) {
+    if (!a || !dev_image || (n_tokens && !dev_tokens) || (n_rows && !dev_offsets)) return fail(ACB_EINVAL, "null argument");
+    if (token_bytes != 2 && token_bytes != 4 && token_bytes != 8) return fail(ACB_EINVAL, "token_bytes must be 2, 4 or 8");
+    if (n_tokens >= (1ull << 60)) return fail(ACB_EINVAL, "n_tokens must be below 2^60");
+    if (n_rows < 0 || n_rows > 0xfffffffell) return fail(ACB_EINVAL, "n_rows out of range (0 .. 2^32 - 2)");
+    {
+        std::lock_guard<std::mutex> lock(a->impl->sieve_mutex);
+        if (a->impl->completions.size() < sizeof(ComplHeader)) return fail(ACB_EINVAL, "acb_completions_build has not been called");
+        std::memcpy(&h, a->impl->completions.data(), sizeof(h));
+    }
+    return filter_view(a, filter, n_rows, F, filt);
+}
+
+static ComplView completions_view(const ComplHeader &h, const void *dev_image) {
+    const uint8_t *b = static_cast<const uint8_t *>(dev_image);
+    ComplView V;
+    V.nodes = reinterpret_cast<const ComplNode *>(b + h.off_nodes);
+    V.kid_tok = reinterpret_cast<const uint32_t *>(b + h.off_kid_tok);
+    V.entries = reinterpret_cast<const ComplEntry *>(b + h.off_entries);
+    V.depth = h.depth;
+    return V;
+}
+
+extern "C" {
+
+int acb_completions_count(const acb_automaton *a, const void *dev_image, const void *dev_tokens, int token_bytes, uint64_t n_tokens,
+                          const int64_t *dev_offsets, int64_t n_rows, int64_t *dev_counts, const acb_pattern_filter *filter, void *stream) {
+    ComplHeader h;
+    SieveFilter F{};
+    bool filt = false;
+    if (int rc = completions_check(a, dev_image, dev_tokens, token_bytes, n_tokens, dev_offsets, n_rows, filter, h, F, filt)) return rc;
+    if (n_rows && !dev_counts) return fail(ACB_EINVAL, "null argument");
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    if (n_rows == 0) return ACB_OK;
+    completions_dispatch<float, kComplCount>(token_bytes, filt, completions_view(h, dev_image), dev_tokens, n_tokens, dev_offsets, n_rows, F,
+                                             nullptr, 0, 0, 0.f, dev_counts, nullptr, d.sms, static_cast<cudaStream_t>(stream));
+    g_launches++;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+int acb_completions_emit(const acb_automaton *a, const void *dev_image, const void *dev_tokens, int token_bytes, uint64_t n_tokens,
+                         const int64_t *dev_offsets, int64_t n_rows, const int64_t *dev_row_offsets, int64_t *dev_ids,
+                         const acb_pattern_filter *filter, void *stream) {
+    ComplHeader h;
+    SieveFilter F{};
+    bool filt = false;
+    if (int rc = completions_check(a, dev_image, dev_tokens, token_bytes, n_tokens, dev_offsets, n_rows, filter, h, F, filt)) return rc;
+    if (n_rows && (!dev_row_offsets || !dev_ids)) return fail(ACB_EINVAL, "null argument");
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    if (n_rows == 0) return ACB_OK;
+    completions_dispatch<float, kComplEmit>(token_bytes, filt, completions_view(h, dev_image), dev_tokens, n_tokens, dev_offsets, n_rows, F,
+                                            nullptr, 0, 0, 0.f, dev_ids, dev_row_offsets, d.sms, static_cast<cudaStream_t>(stream));
+    g_launches++;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+int acb_completions_mask(const acb_automaton *a, const void *dev_image, const void *dev_tokens, int token_bytes, uint64_t n_tokens,
+                         const int64_t *dev_offsets, int64_t n_rows, void *dev_logits, int logits_dtype, int64_t row_stride, int64_t vocab,
+                         float value, const acb_pattern_filter *filter, void *stream) {
+    ComplHeader h;
+    SieveFilter F{};
+    bool filt = false;
+    if (int rc = completions_check(a, dev_image, dev_tokens, token_bytes, n_tokens, dev_offsets, n_rows, filter, h, F, filt)) return rc;
+    if (n_rows && !dev_logits) return fail(ACB_EINVAL, "null argument");
+    if (logits_dtype != ACB_LOGITS_F32 && logits_dtype != ACB_LOGITS_F16 && logits_dtype != ACB_LOGITS_BF16)
+        return fail(ACB_EINVAL, "logits_dtype must be ACB_LOGITS_F32, ACB_LOGITS_F16 or ACB_LOGITS_BF16");
+    if (vocab < 1 || vocab >= (1ll << 62)) return fail(ACB_EINVAL, "vocab out of range (1 .. 2^62 - 1)");
+    if (row_stride < 0 || row_stride >= (1ll << 62)) return fail(ACB_EINVAL, "row_stride out of range (0 .. 2^62 - 1)");
+    if (h.n_entries && (int64_t)h.max_last >= vocab)
+        return fail(ACB_EINVAL, "vocab " + std::to_string(vocab) + " does not hold the largest completing id " + std::to_string(h.max_last));
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    if (n_rows == 0) return ACB_OK;
+    const ComplView V = completions_view(h, dev_image);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (logits_dtype == ACB_LOGITS_F32)
+        completions_dispatch<float, kComplMask>(token_bytes, filt, V, dev_tokens, n_tokens, dev_offsets, n_rows, F, dev_logits, row_stride,
+                                                vocab, value, nullptr, nullptr, d.sms, st);
+    else if (logits_dtype == ACB_LOGITS_F16)
+        completions_dispatch<__half, kComplMask>(token_bytes, filt, V, dev_tokens, n_tokens, dev_offsets, n_rows, F, dev_logits, row_stride,
+                                                 vocab, value, nullptr, nullptr, d.sms, st);
+    else
+        completions_dispatch<__nv_bfloat16, kComplMask>(token_bytes, filt, V, dev_tokens, n_tokens, dev_offsets, n_rows, F, dev_logits,
+                                                        row_stride, vocab, value, nullptr, nullptr, d.sms, st);
+    g_launches++;
     CUDA_OK(cudaGetLastError());
     return ACB_OK;
 }

@@ -22,6 +22,14 @@ __host__ __device__ __forceinline__ uint32_t token_code(uint32_t t) {
     return (0x80u | (t >> 14)) | (((t >> 7) & 0x7fu) << 8) | ((t & 0x7fu) << 16);
 }
 
+// the inverse of token_code: the id whose three bytes are b0 b1 b2, or false when they are not a token's encoding
+// (b0 without its high bit, or b1 / b2 with theirs)
+__host__ __device__ __forceinline__ bool token_decode(uint32_t b0, uint32_t b1, uint32_t b2, uint32_t &t) {
+    if (b0 < 0x80u || b0 > 0xffu || b1 > 0x7fu || b2 > 0x7fu) return false;
+    t = ((b0 & 0x7fu) << 14) | (b1 << 7) | b2;
+    return true;
+}
+
 // the id of element i as a signed 64-bit value (uint16 ids are non-negative, int32 / int64 ids keep their sign)
 template <typename T>
 __host__ __device__ __forceinline__ long long token_value(T v) {

@@ -18,7 +18,9 @@ are already device resident; ``is_match`` / ``is_match_batch`` /
 ``count_matches_by_pattern_device``, how many matches each pattern has over a batch.
 
 ``TokenAhoCorasick`` is the same API over token-id sequences (uint16 / int32 / int64): the ids are encoded into a
-self-synchronising 3-byte format (include/acb200.h) and searched as bytes, positions divided by 3.
+self-synchronising 3-byte format (include/acb200.h) and searched as bytes, positions divided by 3.  Its
+``completing_tokens`` / ``completing_tokens_batch`` / ``completing_tokens_device`` and ``mask_completing_tokens_`` give
+the next ids that would complete a pattern (a bad-words logits processor) from a token-level kernel of their own.
 """
 from __future__ import annotations
 
@@ -179,6 +181,18 @@ class PatternSets:
 def _filter_args(ac: "_Automaton", pattern_sets, set_index, n: int, dev):
     """Checks a device call's (pattern_sets, set_index) -> the filter the internal paths carry: None, or
     (PatternSets, contiguous int32 / int64 index tensor (n,))."""
+    flt = _filter_shape_args(ac, pattern_sets, set_index, n, dev)
+    if flt is not None and n:
+        lo, hi = (int(v) for v in _torch().stack(_torch().aminmax(set_index)).tolist())
+        if lo < 0 or hi >= pattern_sets.n_sets:
+            raise ValueError(f"set_index values must lie in [0, {pattern_sets.n_sets}); found [{lo}, {hi}]")
+    return flt
+
+
+def _filter_shape_args(ac: "_Automaton", pattern_sets, set_index, n: int, dev):
+    """_filter_args without reading set_index back: everything it checks but the index values, so the call neither
+    synchronises nor allocates (for a contiguous index).  The kernels give an index outside [0, n_sets) its defined
+    meaning: the row admits no pattern."""
     torch = _torch()
     if pattern_sets is None and set_index is None:
         return None
@@ -191,10 +205,6 @@ def _filter_args(ac: "_Automaton", pattern_sets, set_index, n: int, dev):
     if (not torch.is_tensor(set_index) or set_index.dtype not in (torch.int32, torch.int64) or set_index.dim() != 1 or
             set_index.shape[0] != n or set_index.device != dev):
         raise ValueError(f"set_index must be an int32 or int64 tensor of shape ({n},) on {dev}")
-    if n:
-        lo, hi = (int(v) for v in torch.stack(torch.aminmax(set_index)).tolist())
-        if lo < 0 or hi >= pattern_sets.n_sets:
-            raise ValueError(f"set_index values must lie in [0, {pattern_sets.n_sets}); found [{lo}, {hi}]")
     return pattern_sets, set_index.contiguous()
 
 
@@ -251,6 +261,7 @@ class _Automaton:
         self.max_pattern_len = int(L.acb_max_pattern_len(h))
         self._images = {}      # device index -> uint8 tensor
         self._sieves = {}      # device index -> (uint8 tensor, SieveDesc)
+        self._completions = {}   # device index -> (uint8 tensor, CompletionsDesc): token-format patterns only
         self._hot = {}         # device index -> dict(tensor, rows, reprofile, calls, backoff)
         self._ws = {}          # (device index, slot) -> dict of tensors
         self._small = {}       # device index -> the small-call context
@@ -310,6 +321,28 @@ class _Automaton:
                 raise RuntimeError(_capi.last_error())
             ent = (host.to(torch.device("cuda", idx)), desc)
             self._sieves[idx] = ent
+        return ent
+
+    def completions(self, device):
+        """(device tensor, CompletionsDesc) of the completions image on `device` (csrc/completions.h: the reverse trie
+        over every pattern's p[:-1] in token ids), built on the first call and uploaded once per device.  ValueError
+        when the patterns are not in the token format."""
+        torch = _require_cuda()
+        idx = device.index if device.index is not None else torch.cuda.current_device()
+        with self._lock:
+            ent = self._completions.get(idx)
+            if ent is None:
+                nbytes = C.c_uint64(0)
+                if self._L.acb_completions_build(self._h, C.byref(nbytes)) != _capi.ACB_OK:
+                    raise ValueError(_capi.last_error())
+                host = torch.empty(nbytes.value, dtype=torch.uint8)
+                if self._L.acb_completions_write(self._h, host.data_ptr(), nbytes.value) != _capi.ACB_OK:
+                    raise RuntimeError(_capi.last_error())
+                desc = _capi.CompletionsDesc()
+                if self._L.acb_completions_describe(host.data_ptr(), C.byref(desc)) != _capi.ACB_OK:
+                    raise RuntimeError(_capi.last_error())
+                ent = (host.to(torch.device("cuda", idx)), desc)
+                self._completions[idx] = ent
         return ent
 
     def sieve_geometry(self, device, task_bytes):
@@ -2999,6 +3032,33 @@ def _encode_host_tokens(seq, what: str) -> np.ndarray:
     """One 1-D integer sequence (list, tuple, numpy array or memmap, CPU tensor) -> its encoded bytes, a uint8 numpy
     array of 3 bytes per id (acb_tokens_encode_host).  TypeError for anything but integers, ValueError naming `what`,
     the index and the value of the first id outside [0, 2^21)."""
+    a, ids = _host_token_ids(seq, what)
+    if ids.size == 0:
+        return np.zeros(0, dtype=np.uint8)
+    out = np.empty(_capi.ACB_TOKEN_BYTES * ids.size, dtype=np.uint8)
+    bad = np.full(1, np.iinfo(np.uint64).max, dtype=np.uint64)
+    if _capi.lib().acb_tokens_encode_host(ids.ctypes.data, ids.itemsize, ids.size, out.ctypes.data, bad.ctypes.data) != _capi.ACB_OK:
+        raise RuntimeError(_capi.last_error())
+    if bad[0] != np.iinfo(np.uint64).max:
+        j = int(bad[0])
+        raise _token_range_error(what, j, int(a[j]))
+    return out
+
+
+def _checked_host_ids(seq, what: str) -> np.ndarray:
+    """One 1-D integer sequence -> its ids as a contiguous uint16 / int32 / int64 numpy array, with the errors of
+    _encode_host_tokens (the range checked here, without encoding)."""
+    a, ids = _host_token_ids(seq, what)
+    bad = np.flatnonzero((ids < 0) | (ids >= _capi.ACB_TOKEN_ID_LIMIT))
+    if bad.size:
+        j = int(bad[0])
+        raise _token_range_error(what, j, int(a[j]))
+    return ids
+
+
+def _host_token_ids(seq, what: str):
+    """The type checks of _encode_host_tokens -> (the sequence as a numpy array, its ids as a contiguous uint16 /
+    int32 / int64 array; empty for an empty sequence).  Ids of object arrays are range-checked here, the rest not."""
     torch = __import__("sys").modules.get("torch")
     if torch is not None and torch.is_tensor(seq):
         if seq.device.type != "cpu":
@@ -3011,7 +3071,7 @@ def _encode_host_tokens(seq, what: str) -> np.ndarray:
     if a.ndim != 1:
         raise TypeError(f"{what} must be a one-dimensional sequence of token ids")
     if a.size == 0:
-        return np.zeros(0, dtype=np.uint8)
+        return a, np.zeros(0, dtype=np.int64)
     if a.dtype == object:   # Python ints beyond int64, or mixed objects
         for j, v in enumerate(a.tolist()):
             if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
@@ -3025,14 +3085,7 @@ def _encode_host_tokens(seq, what: str) -> np.ndarray:
         ids = np.ascontiguousarray(a)
     else:   # narrower ints widen to int32, uint32 / uint64 to int64 (an id past 2^63 wraps negative: still out of range)
         ids = np.ascontiguousarray(a, dtype=np.int32 if a.itemsize < 4 else np.int64)
-    out = np.empty(_capi.ACB_TOKEN_BYTES * ids.size, dtype=np.uint8)
-    bad = np.full(1, np.iinfo(np.uint64).max, dtype=np.uint64)
-    if _capi.lib().acb_tokens_encode_host(ids.ctypes.data, ids.itemsize, ids.size, out.ctypes.data, bad.ctypes.data) != _capi.ACB_OK:
-        raise RuntimeError(_capi.last_error())
-    if bad[0] != np.iinfo(np.uint64).max:
-        j = int(bad[0])
-        raise _token_range_error(what, j, int(a[j]))
-    return out
+    return a, ids
 
 
 def _token_offsets(offsets, tokens):
@@ -3375,6 +3428,135 @@ class TokenAhoCorasick(_PatternSetMethods):
         """Device-resident batch of ids -> (row_offsets, patterns, counts) (see _Automaton.hits_device)."""
         self._ac.check_overlapping(overlapping)
         return self._on_device(lambda d, o: self._ac.hits_device(d, o, overlapping), tokens, offsets)
+
+    # ---- completing tokens: the next ids that would complete a pattern -----------------------------------------------
+    # Id t completes a pattern for a row with history C when some admitted pattern p is a suffix of C || [t]: p[:-1] is
+    # a suffix of C and p[-1] == t (a match of a Standard search would end right after C).  It does not depend on the
+    # match kind, and only the last K - 1 ids of C matter (K = the longest pattern in tokens).  One warp per row walks
+    # the completions image (csrc/completions.h) backwards over those ids (include/acb200.h, acb_completions_*).
+    def _completions_args(self, tokens, offsets, pattern_sets, set_index):
+        """The device forms' checks, none of which reads the device: -> (tokens, offsets, n, filter)."""
+        torch = _torch()
+        if (not torch.is_tensor(tokens) or tokens.dim() != 1 or tokens.device.type != "cuda" or
+                tokens.dtype not in (torch.uint16, torch.int32, torch.int64)):
+            raise TypeError("tokens must be a 1-D CUDA tensor of uint16, int32 or int64 token ids")
+        if not torch.is_tensor(offsets) or offsets.dtype != torch.int64 or offsets.dim() != 1 or offsets.numel() < 1:
+            raise TypeError("offsets must be a 1-D int64 tensor of n + 1 token offsets")
+        if offsets.device != tokens.device:
+            raise ValueError(f"offsets live on {offsets.device}, the tokens on {tokens.device}")
+        n = offsets.numel() - 1
+        flt = _filter_shape_args(self._ac, pattern_sets, set_index, n, tokens.device)
+        _require_cuda()
+        return tokens.contiguous(), offsets.contiguous(), n, flt
+
+    def _completions_stats(self, desc):
+        self._ac.last_stats = {"mode": "completions", "nodes": int(desc.nodes), "entries": int(desc.entries)}
+
+    def completing_tokens(self, history, patterns=None) -> list:
+        """-> the sorted distinct ids t for which some pattern (of `patterns`, when given) is a suffix of
+        ``history + [t]``: the next tokens that would complete a pattern.  Ids outside [0, 2^21) raise ValueError."""
+        return self.completing_tokens_batch([history], _one_set(patterns))[0]
+
+    def completing_tokens_batch(self, histories: Sequence, patterns=None) -> list:
+        """One sorted list of completing ids per history (``completing_tokens`` of each); `patterns`: one iterable of
+        pattern ids per history.  The last K - 1 ids of every history go to the device in one batch."""
+        hists = [_checked_host_ids(h, f"history {i}") for i, h in enumerate(histories)]
+        n = len(hists)
+        sets = _batch_sets(patterns, n)
+        if n == 0:
+            return []
+        torch = _require_cuda()
+        dev = torch.device("cuda", torch.cuda.current_device())
+        depth = int(self._ac.completions(dev)[1].depth)
+        tails = [ids[max(ids.size - depth, 0):].astype(np.int64) for ids in hists]
+        flt = None if sets is None else _host_sets(self._ac, sets, n, dev)
+        offs = np.zeros(n + 1, dtype=np.int64)
+        np.cumsum([t.size for t in tails], out=offs[1:])
+        tokens = torch.from_numpy(np.concatenate(tails)).to(dev)
+        with torch.cuda.device(dev):
+            ids, row_offsets = self._completions_csr(tokens, torch.from_numpy(offs).to(dev), n, flt)
+        ids, row_offsets = ids.cpu().numpy(), row_offsets.cpu().numpy()
+        return [ids[row_offsets[i]:row_offsets[i + 1]].tolist() for i in range(n)]
+
+    def completing_tokens_device(self, tokens, offsets, pattern_sets=None, set_index=None):
+        """Device-resident histories -> (ids int64 (k,), row_offsets int64 (n + 1,)): row i's completing ids are
+        ids[row_offsets[i]:row_offsets[i + 1]], ascending and distinct.  One synchronisation (k).
+
+        ``tokens``: a 1-D uint16 / int32 / int64 CUDA tensor; ``offsets``: int64 (n + 1,) in tokens.  An (n, L)
+        ``input_ids`` tensor is passed as ``ids.reshape(-1)`` with ``offsets = arange(n + 1) * L``.  Offsets are not
+        validated: row i's history is tokens[a:b], a and b being offsets[i] and offsets[i + 1] clamped to
+        [0, len(tokens)], and b < a is an empty history.  Ids outside [0, 2^21) (a negative pad id) equal no pattern
+        token.  ``pattern_sets`` / ``set_index`` (n,): each row's own set; an index outside [0, n_sets) admits nothing."""
+        tokens, offsets, n, flt = self._completions_args(tokens, offsets, pattern_sets, set_index)
+        torch = _torch()
+        with torch.cuda.device(tokens.device):
+            return self._completions_csr(tokens, offsets, n, flt)
+
+    def _completions_csr(self, tokens, offsets, n: int, flt):
+        torch = _torch()
+        dev = tokens.device
+        img, desc = self._ac.completions(dev)
+        L = self._ac._L
+        st = torch.cuda.current_stream(dev).cuda_stream
+        counts = torch.empty(n, dtype=torch.int64, device=dev)
+        rc = L.acb_completions_count(self._ac._h, img.data_ptr(), tokens.data_ptr(), tokens.element_size(), tokens.numel(),
+                                     offsets.data_ptr(), n, counts.data_ptr(), _filter_struct(flt), st)
+        if rc != _capi.ACB_OK:
+            raise RuntimeError(_capi.last_error())
+        row_offsets = torch.zeros(n + 1, dtype=torch.int64, device=dev)
+        torch.cumsum(counts, 0, out=row_offsets[1:])
+        k = int(row_offsets[-1].item())
+        ids = torch.empty(k, dtype=torch.int64, device=dev)
+        if k:
+            rc = L.acb_completions_emit(self._ac._h, img.data_ptr(), tokens.data_ptr(), tokens.element_size(), tokens.numel(),
+                                        offsets.data_ptr(), n, row_offsets.data_ptr(), ids.data_ptr(), _filter_struct(flt), st)
+            if rc != _capi.ACB_OK:
+                raise RuntimeError(_capi.last_error())
+            # each row's ids come out distinct and ascending per trie node: one sort of (row, id) keys orders them
+            rows = torch.repeat_interleave(torch.arange(n, device=dev), counts, output_size=k)
+            ids = torch.bitwise_and(torch.sort(rows * _capi.ACB_TOKEN_ID_LIMIT + ids).values, _capi.ACB_TOKEN_ID_LIMIT - 1)
+        self._completions_stats(desc)
+        return ids, row_offsets
+
+    _LOGITS_DTYPES = {"float32": _capi.ACB_LOGITS_F32, "float16": _capi.ACB_LOGITS_F16, "bfloat16": _capi.ACB_LOGITS_BF16}
+
+    def mask_completing_tokens_(self, logits, tokens, offsets, pattern_sets=None, set_index=None, value: float = float("-inf")):
+        """In place: logits[i, t] = value for every id t that completes a pattern for row i (the bad-words logits
+        processor: ban every next token that would finish a banned sequence); every other element is untouched.
+        Returns `logits`.
+
+        ``logits``: float32 / float16 / bfloat16 CUDA tensor (n, V) with stride(1) == 1 and any row stride (so
+        ``scores[:, -1, :]`` works).  ``tokens``, ``offsets``, ``pattern_sets``, ``set_index``: as for
+        ``completing_tokens_device`` -- an (n, L) ``input_ids`` tensor is ``ids.reshape(-1)`` with
+        ``offsets = arange(n + 1) * L``; offsets are clamped to [0, len(tokens)], not validated; a set index outside
+        [0, n_sets) bans nothing.  Nothing is read back and, for contiguous tokens, offsets and set_index, nothing is
+        allocated: after the first call (which builds and uploads the image) the call can be captured in a CUDA graph.
+        ValueError when the largest id that ends a pattern is >= V (checked on the host)."""
+        tokens, offsets, n, flt = self._completions_args(tokens, offsets, pattern_sets, set_index)
+        torch = _torch()
+        code = self._LOGITS_DTYPES.get(str(logits.dtype).replace("torch.", "")) if torch.is_tensor(logits) else None
+        if code is None or logits.dim() != 2:
+            raise TypeError("logits must be a 2-D float32, float16 or bfloat16 tensor (n, V)")
+        if logits.device != tokens.device:
+            raise ValueError(f"logits live on {logits.device}, the tokens on {tokens.device}")
+        V = int(logits.shape[1])
+        if logits.shape[0] != n:
+            raise ValueError(f"logits have {logits.shape[0]} rows, offsets describe {n} histories")
+        if V < 1:
+            raise ValueError("logits need at least one column")
+        if logits.stride(1) != 1 and V > 1:
+            raise ValueError("logits rows must be contiguous (stride(1) == 1); any row stride is fine")
+        img, desc = self._ac.completions(tokens.device)
+        if desc.entries and desc.max_last >= V:
+            raise ValueError(f"logits have {V} columns, but id {desc.max_last} ends a pattern: V must exceed every pattern's last id")
+        with torch.cuda.device(tokens.device):
+            rc = self._ac._L.acb_completions_mask(self._ac._h, img.data_ptr(), tokens.data_ptr(), tokens.element_size(), tokens.numel(),
+                                                  offsets.data_ptr(), n, logits.data_ptr(), code, logits.stride(0) if n > 1 else V, V,
+                                                  float(value), _filter_struct(flt), torch.cuda.current_stream(tokens.device).cuda_stream)
+        if rc != _capi.ACB_OK:
+            raise RuntimeError(_capi.last_error())
+        self._completions_stats(desc)
+        return logits
 
     # ---- streams: ids fed in chunks ----------------------------------------------------------------------------------
     def stream(self, overlapping: bool = False) -> TokenStream:

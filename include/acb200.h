@@ -702,6 +702,57 @@ int acb_tokens_encode(const void *dev_tokens, int token_bytes, uint64_t n_tokens
 int acb_tokens_encode_host(const void *host_tokens, int token_bytes, uint64_t n_tokens, uint8_t *host_out, uint64_t *host_bad);
 
 /*
+ * Completing tokens: for each row of token-id histories, the next ids that would complete a pattern.  With C a row's
+ * history and S its admitted patterns (all, or with a filter the row's set), id t COMPLETES a pattern when some p in S
+ * is a suffix of C || [t]: p[:-1] is a suffix of C and p[-1] == t.  That is a new match ending right after C, for any
+ * match kind -- it does not depend on the automaton's.  Only the last K - 1 ids of C matter (K = the longest pattern
+ * in tokens); an id outside [0, ACB_TOKEN_ID_LIMIT) equals no pattern token.  The automaton's patterns must be in the
+ * token format (acb_tokens_encode_host of each pattern).
+ *
+ * The completions image (csrc/completions.h) is a reverse trie over every pattern's p[:-1] at token granularity.
+ * acb_completions_build builds it once on the host and writes its size to *image_bytes (ACB_EINVAL when a pattern is
+ * not in the token format); the caller uploads acb_completions_write()'s copy and passes the device pointer as
+ * dev_image.  acb_completions_describe reads a host copy's node and entry counts, depth = K - 1 and max_last = the
+ * largest id that ends a pattern (0 without patterns).
+ *
+ * The three calls walk the image for every row, one warp per row: row i is dev_tokens[a, b) with a, b =
+ * dev_offsets[i], dev_offsets[i + 1] clamped to [0, n_tokens] (b < a: an empty history), token_bytes 2 (uint16), 4
+ * (int32) or 8 (int64).  Offsets are never checked on the device and nothing outside the ids is read.  Filter: as
+ * acb_pattern_filter, one set per row (an index outside [0, n_sets) admits nothing).  One launch each, nothing
+ * synchronises, nothing is allocated.
+ *   acb_completions_count   dev_counts[i] = the number of distinct completing ids of row i (int64[n_rows])
+ *   acb_completions_emit    those ids, written to dev_ids from dev_row_offsets[i] (int64[n_rows]: the exclusive prefix
+ *                           sum of the counts), each once, ascending within a trie node (not overall)
+ *   acb_completions_mask    logits[i * row_stride + t] = value for every completing id t of row i; every other element
+ *                           untouched.  dev_logits: logits_dtype ACB_LOGITS_F32 / _F16 / _BF16, rows of `vocab`
+ *                           elements row_stride elements apart.
+ * ACB_EINVAL, before any CUDA call: a null pointer (dev_tokens may be null when n_tokens == 0, the per-row pointers
+ * when n_rows == 0), acb_completions_build not called, token_bytes not 2, 4 or 8, n_tokens >= 2^60, n_rows outside
+ * [0, 2^32 - 2], a malformed filter, and for the mask a logits_dtype not listed, vocab outside [1, 2^62), row_stride
+ * outside [0, 2^62) or vocab <= max_last (the image has an id the rows cannot hold).  n_rows == 0 launches nothing.
+ */
+#define ACB_LOGITS_F32 0
+#define ACB_LOGITS_F16 1
+#define ACB_LOGITS_BF16 2
+typedef struct acb_completions_desc {
+    uint32_t nodes;      /* reverse-trie nodes, the root included */
+    uint32_t entries;    /* (last token, pattern) entries: the number of patterns */
+    uint32_t depth;      /* K - 1: the history ids a walk may read */
+    uint32_t max_last;   /* the largest id that ends a pattern */
+} acb_completions_desc;
+int acb_completions_build(acb_automaton *a, uint64_t *image_bytes);
+int acb_completions_write(acb_automaton *a, void *host_dst, uint64_t dst_bytes);
+int acb_completions_describe(const void *host_image, acb_completions_desc *desc);
+int acb_completions_count(const acb_automaton *a, const void *dev_image, const void *dev_tokens, int token_bytes, uint64_t n_tokens,
+                          const int64_t *dev_offsets, int64_t n_rows, int64_t *dev_counts, const acb_pattern_filter *filter, void *stream);
+int acb_completions_emit(const acb_automaton *a, const void *dev_image, const void *dev_tokens, int token_bytes, uint64_t n_tokens,
+                         const int64_t *dev_offsets, int64_t n_rows, const int64_t *dev_row_offsets, int64_t *dev_ids,
+                         const acb_pattern_filter *filter, void *stream);
+int acb_completions_mask(const acb_automaton *a, const void *dev_image, const void *dev_tokens, int token_bytes, uint64_t n_tokens,
+                         const int64_t *dev_offsets, int64_t n_rows, void *dev_logits, int logits_dtype, int64_t row_stride, int64_t vocab,
+                         float value, const acb_pattern_filter *filter, void *stream);
+
+/*
  * Multi-GPU: the fixed-size block a rank contributes to the gather of the per-shard match lists (the only exchange
  * of the sharded path; NCCL all-gather over NVLink).  dev_block holds (cap + 1) records of 16 bytes: record 0 =
  * (match count, hay_base, complete flag, 0), then the first `cap` matches of a finished scan (dev_total / dev_out of
