@@ -14,7 +14,7 @@ ACB_OK = 0
 ACB_EINVAL, ACB_EBUILD, ACB_EUNSUPPORTED, ACB_ECUDA, ACB_ECAPACITY = -1, -2, -3, -4, -5
 ACB_TOKEN_ID_LIMIT = 1 << 21   # include/acb200.h: token ids lie in [0, ACB_TOKEN_ID_LIMIT)
 ACB_TOKEN_BYTES = 3            # ... and each becomes this many bytes (csrc/tokens.cuh)
-ACB_LOGITS_F32, ACB_LOGITS_F16, ACB_LOGITS_BF16 = 0, 1, 2   # include/acb200.h: acb_completions_mask's logits dtypes
+ACB_LOGITS_F32, ACB_LOGITS_F16, ACB_LOGITS_BF16 = 0, 1, 2   # include/acb200.h: acb_completions_mask's / _bias's logits dtypes
 ACB_LONG_STRETCH = 4096   # include/acb200.h: longer per-haystack overlapping lists are counted by the whole grid
 
 
@@ -160,6 +160,7 @@ def lib():
         L.acb_completions_count.argtypes = compl + [C.c_void_p, F, C.c_void_p]
         L.acb_completions_emit.argtypes = compl + [C.c_void_p, C.c_void_p, F, C.c_void_p]
         L.acb_completions_mask.argtypes = compl + [C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_float, F, C.c_void_p]
+        L.acb_completions_bias.argtypes = compl + [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64, F, C.c_void_p]
         _lib = L
     return _lib
 
@@ -201,5 +202,5 @@ EXPORTS = [
     "acb_match_mask_overlapping", "acb_match_mask_overlapping_filtered", "acb_match_mask_non_overlapping",
     "acb_match_mask_non_overlapping_filtered", "acb_mask_rows", "acb_mask_unpack", "acb_stream_mask_rows", "acb_stream_mask_emit",
     "acb_completions_build", "acb_completions_write", "acb_completions_describe", "acb_completions_count", "acb_completions_emit",
-    "acb_completions_mask",
+    "acb_completions_mask", "acb_completions_bias",
 ]

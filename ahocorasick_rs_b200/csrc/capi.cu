@@ -3984,6 +3984,19 @@ static int completions_check(const acb_automaton *a, const void *dev_image, cons
     return filter_view(a, filter, n_rows, F, filt);
 }
 
+// the logits checks of the mask and bias modes: the pointer, the dtype code, V, the row stride, and V > max_last
+static int completions_logits_check(const ComplHeader &h, int64_t n_rows, const void *dev_logits, int logits_dtype, int64_t row_stride,
+                                    int64_t vocab) {
+    if (n_rows && !dev_logits) return fail(ACB_EINVAL, "null argument");
+    if (logits_dtype != ACB_LOGITS_F32 && logits_dtype != ACB_LOGITS_F16 && logits_dtype != ACB_LOGITS_BF16)
+        return fail(ACB_EINVAL, "logits_dtype must be ACB_LOGITS_F32, ACB_LOGITS_F16 or ACB_LOGITS_BF16");
+    if (vocab < 1 || vocab >= (1ll << 62)) return fail(ACB_EINVAL, "vocab out of range (1 .. 2^62 - 1)");
+    if (row_stride < 0 || row_stride >= (1ll << 62)) return fail(ACB_EINVAL, "row_stride out of range (0 .. 2^62 - 1)");
+    if (h.n_entries && (int64_t)h.max_last >= vocab)
+        return fail(ACB_EINVAL, "vocab " + std::to_string(vocab) + " does not hold the largest completing id " + std::to_string(h.max_last));
+    return ACB_OK;
+}
+
 static ComplView completions_view(const ComplHeader &h, const void *dev_image) {
     const uint8_t *b = static_cast<const uint8_t *>(dev_image);
     ComplView V;
@@ -4038,13 +4051,7 @@ int acb_completions_mask(const acb_automaton *a, const void *dev_image, const vo
     SieveFilter F{};
     bool filt = false;
     if (int rc = completions_check(a, dev_image, dev_tokens, token_bytes, n_tokens, dev_offsets, n_rows, filter, h, F, filt)) return rc;
-    if (n_rows && !dev_logits) return fail(ACB_EINVAL, "null argument");
-    if (logits_dtype != ACB_LOGITS_F32 && logits_dtype != ACB_LOGITS_F16 && logits_dtype != ACB_LOGITS_BF16)
-        return fail(ACB_EINVAL, "logits_dtype must be ACB_LOGITS_F32, ACB_LOGITS_F16 or ACB_LOGITS_BF16");
-    if (vocab < 1 || vocab >= (1ll << 62)) return fail(ACB_EINVAL, "vocab out of range (1 .. 2^62 - 1)");
-    if (row_stride < 0 || row_stride >= (1ll << 62)) return fail(ACB_EINVAL, "row_stride out of range (0 .. 2^62 - 1)");
-    if (h.n_entries && (int64_t)h.max_last >= vocab)
-        return fail(ACB_EINVAL, "vocab " + std::to_string(vocab) + " does not hold the largest completing id " + std::to_string(h.max_last));
+    if (int rc = completions_logits_check(h, n_rows, dev_logits, logits_dtype, row_stride, vocab)) return rc;
     DeviceInfo d;
     if (int rc = device_info(d)) return rc;
     if (n_rows == 0) return ACB_OK;
@@ -4059,6 +4066,65 @@ int acb_completions_mask(const acb_automaton *a, const void *dev_image, const vo
     else
         completions_dispatch<__nv_bfloat16, kComplMask>(token_bytes, filt, V, dev_tokens, n_tokens, dev_offsets, n_rows, F, dev_logits,
                                                         row_stride, vocab, value, nullptr, nullptr, d.sms, st);
+    g_launches++;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+}  // extern "C"
+
+template <typename T, typename L, bool FILT>
+static void completions_bias_launch(const ComplView &V, const void *tokens, uint64_t n_tokens, const int64_t *offsets, int64_t n_rows,
+                                    const SieveFilter &F, const float *bias, void *logits, int64_t row_stride, int64_t vocab, int sms,
+                                    cudaStream_t st) {
+    constexpr int64_t kWarps = kComplThreads / 32;
+    int64_t blocks = (n_rows + kWarps - 1) / kWarps;
+    if (blocks > 32ll * sms) blocks = 32ll * sms;   // grid-stride beyond that
+    completions_bias_kernel<T, L, FILT><<<(unsigned)blocks, kComplThreads, 0, st>>>(
+        V, static_cast<const T *>(tokens), n_tokens, offsets, n_rows, F, bias, static_cast<L *>(logits), row_stride, vocab);
+}
+
+template <typename L>
+static void completions_bias_dispatch(int token_bytes, bool filt, const ComplView &V, const void *tokens, uint64_t n_tokens,
+                                      const int64_t *offsets, int64_t n_rows, const SieveFilter &F, const float *bias, void *logits,
+                                      int64_t row_stride, int64_t vocab, int sms, cudaStream_t st) {
+#define ACB_COMPL_BIAS_LAUNCH(T, FL) \
+    completions_bias_launch<T, L, FL>(V, tokens, n_tokens, offsets, n_rows, F, bias, logits, row_stride, vocab, sms, st)
+    if (token_bytes == 2) {
+        if (filt) ACB_COMPL_BIAS_LAUNCH(uint16_t, true); else ACB_COMPL_BIAS_LAUNCH(uint16_t, false);
+    } else if (token_bytes == 4) {
+        if (filt) ACB_COMPL_BIAS_LAUNCH(int32_t, true); else ACB_COMPL_BIAS_LAUNCH(int32_t, false);
+    } else {
+        if (filt) ACB_COMPL_BIAS_LAUNCH(int64_t, true); else ACB_COMPL_BIAS_LAUNCH(int64_t, false);
+    }
+#undef ACB_COMPL_BIAS_LAUNCH
+}
+
+extern "C" {
+
+int acb_completions_bias(const acb_automaton *a, const void *dev_image, const void *dev_tokens, int token_bytes, uint64_t n_tokens,
+                         const int64_t *dev_offsets, int64_t n_rows, const float *dev_bias, void *dev_logits, int logits_dtype,
+                         int64_t row_stride, int64_t vocab, const acb_pattern_filter *filter, void *stream) {
+    ComplHeader h;
+    SieveFilter F{};
+    bool filt = false;
+    if (int rc = completions_check(a, dev_image, dev_tokens, token_bytes, n_tokens, dev_offsets, n_rows, filter, h, F, filt)) return rc;
+    if (int rc = completions_logits_check(h, n_rows, dev_logits, logits_dtype, row_stride, vocab)) return rc;
+    if (n_rows && !dev_bias) return fail(ACB_EINVAL, "null argument");
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    if (n_rows == 0) return ACB_OK;
+    const ComplView V = completions_view(h, dev_image);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (logits_dtype == ACB_LOGITS_F32)
+        completions_bias_dispatch<float>(token_bytes, filt, V, dev_tokens, n_tokens, dev_offsets, n_rows, F, dev_bias, dev_logits, row_stride,
+                                         vocab, d.sms, st);
+    else if (logits_dtype == ACB_LOGITS_F16)
+        completions_bias_dispatch<__half>(token_bytes, filt, V, dev_tokens, n_tokens, dev_offsets, n_rows, F, dev_bias, dev_logits, row_stride,
+                                          vocab, d.sms, st);
+    else
+        completions_bias_dispatch<__nv_bfloat16>(token_bytes, filt, V, dev_tokens, n_tokens, dev_offsets, n_rows, F, dev_bias, dev_logits,
+                                                 row_stride, vocab, d.sms, st);
     g_launches++;
     CUDA_OK(cudaGetLastError());
     return ACB_OK;

@@ -20,7 +20,8 @@ are already device resident; ``is_match`` / ``is_match_batch`` /
 ``TokenAhoCorasick`` is the same API over token-id sequences (uint16 / int32 / int64): the ids are encoded into a
 self-synchronising 3-byte format (include/acb200.h) and searched as bytes, positions divided by 3.  Its
 ``completing_tokens`` / ``completing_tokens_batch`` / ``completing_tokens_device`` and ``mask_completing_tokens_`` give
-the next ids that would complete a pattern (a bad-words logits processor) from a token-level kernel of their own.
+the next ids that would complete a pattern (a bad-words logits processor) from a token-level kernel of their own, and
+``bias_completing_tokens_`` adds a bias per pattern to them (a sequence-bias logits processor).
 """
 from __future__ import annotations
 
@@ -3534,6 +3535,20 @@ class TokenAhoCorasick(_PatternSetMethods):
         ValueError when the largest id that ends a pattern is >= V (checked on the host)."""
         tokens, offsets, n, flt = self._completions_args(tokens, offsets, pattern_sets, set_index)
         torch = _torch()
+        code, V, img, desc = self._logits_args(logits, tokens, n)
+        with torch.cuda.device(tokens.device):
+            rc = self._ac._L.acb_completions_mask(self._ac._h, img.data_ptr(), tokens.data_ptr(), tokens.element_size(), tokens.numel(),
+                                                  offsets.data_ptr(), n, logits.data_ptr(), code, logits.stride(0) if n > 1 else V, V,
+                                                  float(value), _filter_struct(flt), torch.cuda.current_stream(tokens.device).cuda_stream)
+        if rc != _capi.ACB_OK:
+            raise RuntimeError(_capi.last_error())
+        self._completions_stats(desc)
+        return logits
+
+    def _logits_args(self, logits, tokens, n: int):
+        """The logits checks of the mask and the bias, none of which reads the device, and the vocabulary check against
+        the image's largest last id (on the host): -> (dtype code, V, image, desc)."""
+        torch = _torch()
         code = self._LOGITS_DTYPES.get(str(logits.dtype).replace("torch.", "")) if torch.is_tensor(logits) else None
         if code is None or logits.dim() != 2:
             raise TypeError("logits must be a 2-D float32, float16 or bfloat16 tensor (n, V)")
@@ -3549,12 +3564,47 @@ class TokenAhoCorasick(_PatternSetMethods):
         img, desc = self._ac.completions(tokens.device)
         if desc.entries and desc.max_last >= V:
             raise ValueError(f"logits have {V} columns, but id {desc.max_last} ends a pattern: V must exceed every pattern's last id")
-        with torch.cuda.device(tokens.device):
-            rc = self._ac._L.acb_completions_mask(self._ac._h, img.data_ptr(), tokens.data_ptr(), tokens.element_size(), tokens.numel(),
-                                                  offsets.data_ptr(), n, logits.data_ptr(), code, logits.stride(0) if n > 1 else V, V,
-                                                  float(value), _filter_struct(flt), torch.cuda.current_stream(tokens.device).cuda_stream)
-        if rc != _capi.ACB_OK:
-            raise RuntimeError(_capi.last_error())
+        return code, V, img, desc
+
+    def bias_completing_tokens_(self, logits, tokens, offsets, bias, pattern_sets=None, set_index=None):
+        """In place: adds a signed bias per pattern to the ids that would complete it (the sequence-bias logits
+        processor: a positive bias encourages a sequence, a negative one discourages it, -inf bans it).  Returns
+        `logits`.
+
+        ``bias``: float32 CUDA tensor (len(patterns),) on the tokens' device.  For row i and id t, let P_t be the
+        admitted pids p that t completes (p[:-1] is a suffix of the row's history and p[-1] == t), ordered longest
+        pattern first, ties by ascending pid: s = bias[p1] + bias[p2] + ... summed in float32 from the first term, then
+        logits[i, t] = logits[i, t] + s computed in float32 and rounded once (nearest-even) to the logits dtype.
+        Every other element is untouched, and the result is the same bit for bit on every run.  With every bias -inf
+        this equals ``mask_completing_tokens_``.  Per-request values: give the same sequence twice, as two patterns
+        with their own biases, each in its request's pattern set; duplicates that are both admitted both count.
+
+        Differences from Hugging Face's ``SequenceBiasLogitsProcessor``: it accumulates in the logits dtype, in dict
+        order, where this sums in float32 and rounds once; and it skips every sequence longer than the padded batch
+        width and compares pad ids, where this applies every pattern whose p[:-1] is a suffix of the row's own history.
+
+        ``logits``, ``tokens``, ``offsets``, ``pattern_sets``, ``set_index``: as for ``mask_completing_tokens_``.
+        Nothing is read back and, for contiguous inputs, nothing is allocated: after the first call the call can be
+        captured in a CUDA graph (rewrite the histories, set indices and biases in place between replays)."""
+        tokens, offsets, n, flt = self._completions_args(tokens, offsets, pattern_sets, set_index)
+        torch = _torch()
+        P = self._ac.n_patterns
+        if not torch.is_tensor(bias) or bias.dtype != torch.float32:
+            raise TypeError("bias must be a float32 tensor with one value per pattern")
+        if bias.dim() != 1 or bias.numel() != P:
+            raise ValueError(f"bias has shape {tuple(bias.shape)}, expected ({P},): one value per pattern")
+        if bias.device != tokens.device:
+            raise ValueError(f"bias lives on {bias.device}, the tokens on {tokens.device}")
+        code, V, img, desc = self._logits_args(logits, tokens, n)
+        if P:   # without patterns there is nothing to add (and an empty bias has no storage to pass)
+            bias = bias.contiguous()
+            with torch.cuda.device(tokens.device):
+                rc = self._ac._L.acb_completions_bias(self._ac._h, img.data_ptr(), tokens.data_ptr(), tokens.element_size(),
+                                                      tokens.numel(), offsets.data_ptr(), n, bias.data_ptr(), logits.data_ptr(), code,
+                                                      logits.stride(0) if n > 1 else V, V, _filter_struct(flt),
+                                                      torch.cuda.current_stream(tokens.device).cuda_stream)
+            if rc != _capi.ACB_OK:
+                raise RuntimeError(_capi.last_error())
         self._completions_stats(desc)
         return logits
 

@@ -726,10 +726,18 @@ int acb_tokens_encode_host(const void *host_tokens, int token_bytes, uint64_t n_
  *   acb_completions_mask    logits[i * row_stride + t] = value for every completing id t of row i; every other element
  *                           untouched.  dev_logits: logits_dtype ACB_LOGITS_F32 / _F16 / _BF16, rows of `vocab`
  *                           elements row_stride elements apart.
+ *   acb_completions_bias    a signed bias per pattern (a sequence-bias logits processor): with P_t the admitted pids
+ *                           that t completes, ordered longest pattern first, ties by ascending pid (p1 .. pk),
+ *                           s = dev_bias[p1], then s = fl32(s + dev_bias[pj]) for j = 2 .. k (the sum starts from its
+ *                           first term, not from 0), and logits[i * row_stride + t] = round(fl32(logits[..] + s)) to
+ *                           the logits dtype, nearest-even, once; every other element untouched.  dev_bias:
+ *                           float32[n_patterns].  Each element is written by one thread: no atomics, the result is
+ *                           the same bit for bit on every run.  All -inf biases give the mask's -inf.
  * ACB_EINVAL, before any CUDA call: a null pointer (dev_tokens may be null when n_tokens == 0, the per-row pointers
  * when n_rows == 0), acb_completions_build not called, token_bytes not 2, 4 or 8, n_tokens >= 2^60, n_rows outside
- * [0, 2^32 - 2], a malformed filter, and for the mask a logits_dtype not listed, vocab outside [1, 2^62), row_stride
- * outside [0, 2^62) or vocab <= max_last (the image has an id the rows cannot hold).  n_rows == 0 launches nothing.
+ * [0, 2^32 - 2], a malformed filter, and for the mask and the bias a logits_dtype not listed, vocab outside [1, 2^62),
+ * row_stride outside [0, 2^62) or vocab <= max_last (the image has an id the rows cannot hold).  n_rows == 0 launches
+ * nothing.
  */
 #define ACB_LOGITS_F32 0
 #define ACB_LOGITS_F16 1
@@ -751,6 +759,9 @@ int acb_completions_emit(const acb_automaton *a, const void *dev_image, const vo
 int acb_completions_mask(const acb_automaton *a, const void *dev_image, const void *dev_tokens, int token_bytes, uint64_t n_tokens,
                          const int64_t *dev_offsets, int64_t n_rows, void *dev_logits, int logits_dtype, int64_t row_stride, int64_t vocab,
                          float value, const acb_pattern_filter *filter, void *stream);
+int acb_completions_bias(const acb_automaton *a, const void *dev_image, const void *dev_tokens, int token_bytes, uint64_t n_tokens,
+                         const int64_t *dev_offsets, int64_t n_rows, const float *dev_bias, void *dev_logits, int logits_dtype,
+                         int64_t row_stride, int64_t vocab, const acb_pattern_filter *filter, void *stream);
 
 /*
  * Multi-GPU: the fixed-size block a rank contributes to the gather of the per-shard match lists (the only exchange
