@@ -25,6 +25,7 @@ the next ids that would complete a pattern (a bad-words logits processor) from a
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import enum
 import threading
@@ -80,15 +81,14 @@ def scan_in_windows(scan_window, hay, window_bytes: int, halo: int, codepoints: 
     reported, whole, by the predecessor) -- a suffix of its sorted rows --, rebased to the haystack.  `hay` is a uint8
     numpy array or torch tensor; returns the list of per-window row blocks, in order (concatenated they are in the
     reference's order)."""
-    total_len = len(hay)
-    step = window_bytes - halo
-    if step <= 0:
-        raise ValueError("window smaller than the longest pattern")
     parts = []
     cont_before = 0  # continuation bytes before the window start (code point indexes)
-    w0 = 0
-    while w0 < total_len:
-        w1 = min(w0 + window_bytes, total_len)
+    counted = 0      # ... counted up to here
+    for w0, w1 in _windows(len(hay), window_bytes, halo):
+        if codepoints:
+            for a in range(counted, w0, 1 << 28):  # count in slices: the mask is a temporary of the slice's size
+                cont_before += _count_cont(hay[a:min(a + (1 << 28), w0)])
+            counted = w0
         window = hay[w0:w1]
         part = scan_window(window)
         if w0 > 0 and part.shape[0]:
@@ -112,14 +112,77 @@ def scan_in_windows(scan_window, hay, window_bytes: int, halo: int, codepoints: 
             part[:, 2] += base
             part[:, 3] += base
         parts.append(part)
-        if w1 == total_len:
-            break
-        if codepoints:
-            nxt = w0 + step
-            for a in range(w0, nxt, 1 << 28):  # count in slices: the mask is a temporary of the slice's size
-                cont_before += _count_cont(hay[a:min(a + (1 << 28), nxt)])
-        w0 += step
     return parts
+
+
+def _windows(total_len: int, limit: int, halo: int):
+    """The windows [w0, w1) of `limit` bytes at most that cover a haystack of total_len bytes, in order, each sharing
+    `halo` bytes (max_pattern_len - 1) with its predecessor: every match lies inside one of them whole.  None for an
+    empty haystack.  ValueError when limit <= halo (the windows would not advance)."""
+    step = limit - halo
+    if step <= 0:
+        raise ValueError("window smaller than the longest pattern")
+    w0 = 0
+    while w0 < total_len:
+        w1 = min(w0 + limit, total_len)
+        yield w0, w1
+        if w1 == total_len:
+            return
+        w0 += step
+
+
+def _haystack_runs(offsets, limit: int):
+    """Cuts a batch (offsets: int64 tensor (n + 1,)) that one call cannot take into calls, in haystack order: yields
+    (h, h1, start, end, large), haystacks [h, h1) at bytes [start, end).  large = False: the longest run of whole
+    haystacks from h that fits `limit` bytes and stops before an oversized one (at least one haystack; zero-byte runs
+    too).  large = True: the single haystack h (h1 = h + 1) of more than `limit` bytes.  The host reads a few scalars
+    of `offsets` per item and nothing else."""
+    torch = _torch()
+    n = offsets.numel() - 1
+    if n <= 0:
+        return
+    lens = offsets[1:] - offsets[:-1]
+    oversized = bool((lens > limit).any().item())
+    h = 0
+    while h < n:
+        start = int(offsets[h].item())
+        if oversized:
+            size = int(lens[h].item())
+            if size > limit:
+                yield h, h + 1, start, start + size, True
+                h += 1
+                continue
+        h1 = int(torch.searchsorted(offsets, torch.tensor([start + limit], dtype=torch.int64, device=offsets.device), right=True).item()) - 1
+        h1 = max(h + 1, min(h1, n))
+        if oversized:
+            big = torch.nonzero(lens[h:h1] > limit)
+            if big.numel():
+                h1 = h + int(big[0].item())
+        yield h, h1, start, int(offsets[h1].item()), False
+        h = h1
+
+
+def _pack_host(buf, chunks):
+    """Lays bytes-like chunks (one per haystack) out for one host->device copy: the n + 1 int64 offsets, then the bytes
+    from the first 512-byte boundary after them.  buf(nbytes) returns the uint8 numpy buffer to write, of at least
+    nbytes.  -> (offsets, a numpy array of its own; head; total_bytes): the bytes are at buf[head:head + total_bytes]."""
+    n = len(chunks)
+    offs = np.zeros(n + 1, dtype=np.int64)
+    np.cumsum(np.fromiter((len(c) for c in chunks), dtype=np.int64, count=n), out=offs[1:])
+    total_bytes = int(offs[-1])
+    head = (8 * (n + 1) + 511) & ~511   # the offsets, then the bytes at a 512-byte boundary of the buffer
+    hv = buf(head + total_bytes)
+    hv[:8 * (n + 1)].view(np.int64)[:] = offs
+    if n == 1:
+        hv[head:head + total_bytes] = np.frombuffer(chunks[0], dtype=np.uint8)
+    elif total_bytes:
+        hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
+    return offs, head, total_bytes
+
+
+def _check(rc):
+    if rc != _capi.ACB_OK:
+        raise RuntimeError(_capi.last_error())
 
 
 # last_stats["paths"] of a table-walker scan: the branches its epilogue took (kPath* in csrc/capi.cu).  They never
@@ -286,9 +349,7 @@ class _Automaton:
         if img is None:
             nbytes = int(self._L.acb_image_bytes(self._h))
             host = torch.empty(nbytes, dtype=torch.uint8, pin_memory=True)
-            rc = self._L.acb_image_write(self._h, host.data_ptr(), nbytes)
-            if rc != _capi.ACB_OK:
-                raise RuntimeError(_capi.last_error())
+            _check(self._L.acb_image_write(self._h, host.data_ptr(), nbytes))
             img = host.to(torch.device("cuda", idx), non_blocking=False)
             self._images[idx] = img
         return img
@@ -315,11 +376,9 @@ class _Automaton:
             if nbytes == 0:
                 raise RuntimeError(_capi.last_error())
             host = torch.empty(nbytes, dtype=torch.uint8, pin_memory=True)
-            if self._L.acb_sieve_write(self._h, host.data_ptr(), nbytes) != _capi.ACB_OK:
-                raise RuntimeError(_capi.last_error())
+            _check(self._L.acb_sieve_write(self._h, host.data_ptr(), nbytes))
             desc = _capi.SieveDesc()
-            if self._L.acb_sieve_describe(host.data_ptr(), C.byref(desc)) != _capi.ACB_OK:
-                raise RuntimeError(_capi.last_error())
+            _check(self._L.acb_sieve_describe(host.data_ptr(), C.byref(desc)))
             ent = (host.to(torch.device("cuda", idx)), desc)
             self._sieves[idx] = ent
         return ent
@@ -337,11 +396,9 @@ class _Automaton:
                 if self._L.acb_completions_build(self._h, C.byref(nbytes)) != _capi.ACB_OK:
                     raise ValueError(_capi.last_error())
                 host = torch.empty(nbytes.value, dtype=torch.uint8)
-                if self._L.acb_completions_write(self._h, host.data_ptr(), nbytes.value) != _capi.ACB_OK:
-                    raise RuntimeError(_capi.last_error())
+                _check(self._L.acb_completions_write(self._h, host.data_ptr(), nbytes.value))
                 desc = _capi.CompletionsDesc()
-                if self._L.acb_completions_describe(host.data_ptr(), C.byref(desc)) != _capi.ACB_OK:
-                    raise RuntimeError(_capi.last_error())
+                _check(self._L.acb_completions_describe(host.data_ptr(), C.byref(desc)))
                 ent = (host.to(torch.device("cuda", idx)), desc)
                 self._completions[idx] = ent
         return ent
@@ -370,12 +427,9 @@ class _Automaton:
         nbytes = int(self._L.acb_hot_bytes(self._h, rows))
         host = torch.empty(nbytes, dtype=torch.uint8, pin_memory=True)
         vp = visits_host.ctypes.data if visits_host is not None else None
-        rc = self._L.acb_hot_build(self._h, vp, rows, host.data_ptr(), nbytes)
-        if rc != _capi.ACB_OK:
-            raise RuntimeError(_capi.last_error())
+        _check(self._L.acb_hot_build(self._h, vp, rows, host.data_ptr(), nbytes))
         desc = _capi.HotDesc()
-        if self._L.acb_hot_describe(host.data_ptr(), C.byref(desc)) != _capi.ACB_OK:
-            raise RuntimeError(_capi.last_error())
+        _check(self._L.acb_hot_describe(host.data_ptr(), C.byref(desc)))
         return host.to(torch.device("cuda", idx)), desc
 
     def hot(self, device, data=None, offsets=None, overlapping=False):
@@ -392,10 +446,8 @@ class _Automaton:
             visits = torch.empty(self.num_states, dtype=torch.int32, device=device)
             stream = torch.cuda.current_stream(device).cuda_stream
             n = offsets.numel() - 1
-            rc = self._L.acb_profile(self._h, img.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
-                                     int(bool(overlapping)), visits.data_ptr(), stream)
-            if rc != _capi.ACB_OK:
-                raise RuntimeError(_capi.last_error())
+            _check(self._L.acb_profile(self._h, img.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
+                                       int(bool(overlapping)), visits.data_ptr(), stream))
             vh = visits.cpu().numpy().view(np.uint32)
             t, rows = self._upload_hot(idx, vh)
             # How much of the sampled scan the hot rows cover.  Every byte outside them costs the staged kernel a
@@ -427,15 +479,18 @@ class _Automaton:
 
     def _plan(self, data, n_haystacks: int):
         plan = _capi.Plan()
-        rc = self._L.acb_plan_scan(self._h, data.data_ptr(), data.numel(), n_haystacks, C.byref(plan))
-        if rc != _capi.ACB_OK:
-            raise RuntimeError(_capi.last_error())
+        _check(self._L.acb_plan_scan(self._h, data.data_ptr(), data.numel(), n_haystacks, C.byref(plan)))
         return plan
 
+    @staticmethod
+    def _ws_key(device, slot):
+        return (device.index if device.index is not None else _torch().cuda.current_device(), slot)
+
     def _workspace(self, device, plan, n_haystacks: int, capacity: int, slot: int = 0):
+        """Workspace `slot` on `device` (the host pipeline alternates between two), grown to fit, after making the
+        current stream wait for the last reader of the views it handed out (_mark_read)."""
         torch = _torch()
-        idx = device.index if device.index is not None else torch.cuda.current_device()
-        key = (idx, slot)   # (the host pipeline alternates between two workspaces)
+        key = self._ws_key(device, slot)
         ws = self._ws.get(key)
         need = (ws is None or ws["n_units"] < plan.n_units or ws["n_segments"] < plan.n_segments or
                 ws["scratch"].numel() < plan.scratch_words or ws["n_haystacks"] < n_haystacks or ws["capacity"] < capacity)
@@ -447,7 +502,7 @@ class _Automaton:
             n_hay = max(n_haystacks, ws["n_haystacks"] if ws else 0, 1)
             n_scr = max(plan.scratch_words, ws["scratch"].numel() if ws else 0, 16)
             cap = max(capacity, ws["capacity"] if ws else 0, 1024)
-            dev = torch.device("cuda", idx)
+            dev = torch.device("cuda", key[0])
             ws = {
                 "n_units": n_units, "n_segments": n_seg, "n_haystacks": n_hay, "capacity": cap,
                 "raw": torch.empty((cap, 4), dtype=torch.int32, device=dev),
@@ -463,7 +518,43 @@ class _Automaton:
                 "match_offsets": torch.empty(n_hay + 1, dtype=torch.int64, device=dev),
             }
             self._ws[key] = ws
+        reader = ws.pop("reader", None)
+        if reader is not None:   # a comparison of an earlier call (maybe on another stream) reads this workspace first
+            torch.cuda.current_stream(device).wait_event(reader)
         return ws
+
+    def _mark_read(self, device, slot=0):
+        """Records, on the current stream, that the views of workspace `slot` a scan handed out are read up to here:
+        the next scan that uses the slot waits for this point (_workspace), on whatever stream or thread it runs."""
+        torch = _torch()
+        ws = self._ws.get(self._ws_key(device, slot))
+        if ws is not None:
+            reader = torch.cuda.Event()
+            reader.record(torch.cuda.current_stream(device))
+            ws["reader"] = reader
+
+    def _list_attempt(self, device, plan, n_haystacks: int, capacity: Optional[int], launch, slot=0):
+        """One list scan into workspace `slot`, with room for `capacity` records (None: max(1024, 2n)):
+        launch(plan_ref, ws_struct_ref) -> rc calls the library.  A failure raises (ValueError for an unsupported
+        request) with the workspace's counters zeroed.  -> the workspace; its "total" words say whether the list fit."""
+        ws = self._workspace(device, plan, n_haystacks, capacity or max(1024, n_haystacks * 2), slot)
+        rc = launch(C.byref(plan), C.byref(self._ws_struct(ws)))
+        if rc != _capi.ACB_OK:
+            err = _capi.last_error()
+            ws["scratch"][:8].zero_()   # a scan that failed half way may have left its counters dirty
+            raise (ValueError if rc == _capi.ACB_EUNSUPPORTED else RuntimeError)(err)
+        return ws
+
+    def _list_scan(self, device, plan, n_haystacks: int, capacity: Optional[int], launch):
+        """_list_attempt on workspace slot 0 until the list fit (or was empty), each retry with room for all of it (a
+        call whose list did not fit added nothing to its outputs) -> (workspace, its "total" words as a list)."""
+        while True:
+            ws = self._list_attempt(device, plan, n_haystacks, capacity, launch)
+            tot = ws["total"].tolist()
+            total, complete, raw_total = tot[0], tot[1], tot[4]
+            if complete or (total == 0 and raw_total == 0):
+                return ws, tot
+            capacity = max(total, raw_total) + max(total, raw_total) // 8 + 16
 
     def _ws_struct(self, ws):
         s = _capi.Workspace()
@@ -543,11 +634,9 @@ class _Automaton:
                 sieve_t, _ = self.sieve(dev)
                 plan = self._plan(data, n)
                 scratch = torch.empty(3, dtype=torch.int64, device=dev)
-                rc = self._L.acb_any_match_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
-                                                    out.data_ptr(), scratch.data_ptr(), _filter_struct(flt),
-                                                    torch.cuda.current_stream(dev).cuda_stream)
-                if rc != _capi.ACB_OK:
-                    raise RuntimeError(_capi.last_error())
+                _check(self._L.acb_any_match_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
+                                                      out.data_ptr(), scratch.data_ptr(), _filter_struct(flt),
+                                                      torch.cuda.current_stream(dev).cuda_stream))
             else:
                 # scan_device (it takes the lock again and makes the same choice) with sync=True: it retries until the
                 # list is complete.  Its match_offsets are a view of workspace slot 0, which every scan of this
@@ -559,9 +648,7 @@ class _Automaton:
                     out = hit
                 else:
                     out |= hit
-                reader = torch.cuda.Event()
-                reader.record(torch.cuda.current_stream(dev))
-                self._ws[(dev.index if dev.index is not None else torch.cuda.current_device(), 0)]["reader"] = reader
+                self._mark_read(dev)
                 self.last_stats = {"engine": self.last_stats.get("engine", "table"), "mode": "any"}
                 return out
         if sync:
@@ -581,36 +668,17 @@ class _Automaton:
         of `out`; one haystack above the limit is scanned in windows that share max_pattern_len - 1 bytes (an
         occurrence lies inside one of them whole) and share its flag, stopping at the first window that sets it."""
         torch = _require_cuda()
-        dev = data.device
-        n = offsets.numel() - 1
-        limit = self.WINDOW_BYTES
-        lens = offsets[1:] - offsets[:-1]
-        oversized = bool((lens > limit).any().item())
-        h = 0
-        while h < n:
-            start = int(offsets[h].item())
-            if oversized and int(lens[h].item()) > limit:
-                hay, flag = data[start:start + int(lens[h].item())], out[h:h + 1]
-                step = limit - max(self.max_pattern_len - 1, 0)
-                w0 = 0
-                while not bool(flag.item()):
-                    w1 = min(w0 + limit, hay.numel())
-                    self.any_device(hay[w0:w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=dev), flag, flt=_filter_slice(flt, h, h + 1))
-                    if w1 == hay.numel():
-                        break
-                    w0 += step
-                h += 1
+        halo = max(self.max_pattern_len - 1, 0)
+        for h, h1, start, end, large in _haystack_runs(offsets, self.WINDOW_BYTES):
+            if not large:
+                self.any_device(data[start:end], offsets[h:h1 + 1] - start, out[h:h1], flt=_filter_slice(flt, h, h1))
                 continue
-            # the longest run of whole haystacks that fits one call (and stops before an oversized one)
-            h1 = int(torch.searchsorted(offsets, torch.tensor([start + limit], dtype=torch.int64, device=dev), right=True).item()) - 1
-            h1 = max(h + 1, min(h1, n))
-            if oversized:
-                big = torch.nonzero(lens[h:h1] > limit)
-                if big.numel():
-                    h1 = h + int(big[0].item())
-            end = int(offsets[h1].item())
-            self.any_device(data[start:end], offsets[h:h1 + 1] - start, out[h:h1], flt=_filter_slice(flt, h, h1))
-            h = h1
+            flag = out[h:h1]
+            for w0, w1 in _windows(end - start, self.WINDOW_BYTES, halo):
+                if bool(flag.item()):
+                    break
+                self.any_device(data[start + w0:start + w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=data.device), flag,
+                                flt=_filter_slice(flt, h, h1))
         return out
 
     # ---- the first match per haystack (the crate's AhoCorasick::find) ---------------------------------------------
@@ -632,10 +700,8 @@ class _Automaton:
         n = offsets.numel() - 1
         sieve_t, _ = self.sieve(dev)
         scratch = torch.empty(3, dtype=torch.int64, device=dev)
-        rc = self._L.acb_find_first_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
-                                             keys.data_ptr(), scratch.data_ptr(), _filter_struct(flt), torch.cuda.current_stream(dev).cuda_stream)
-        if rc != _capi.ACB_OK:
-            raise RuntimeError(_capi.last_error())
+        _check(self._L.acb_find_first_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
+                                               keys.data_ptr(), scratch.data_ptr(), _filter_struct(flt), torch.cuda.current_stream(dev).cuda_stream))
         return scratch
 
     def first_rows(self, data, offsets, keys, flt=None):
@@ -645,19 +711,15 @@ class _Automaton:
         n = offsets.numel() - 1
         sieve_t, _ = self.sieve(dev)
         rows = torch.empty((n, 3), dtype=torch.int64, device=dev)
-        rc = self._L.acb_first_rows_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, keys.data_ptr(),
-                                             rows.data_ptr(), _filter_struct(flt), torch.cuda.current_stream(dev).cuda_stream)
-        if rc != _capi.ACB_OK:
-            raise RuntimeError(_capi.last_error())
+        _check(self._L.acb_first_rows_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, keys.data_ptr(),
+                                               rows.data_ptr(), _filter_struct(flt), torch.cuda.current_stream(dev).cuda_stream))
         return rows
 
     def _rows_to_codepoints(self, data, offsets, rows):
         torch = _torch()
         out = torch.empty_like(rows)
-        rc = self._L.acb_rows_to_codepoints(data.data_ptr(), offsets.data_ptr(), offsets.numel() - 1, data.numel(), rows.data_ptr(),
-                                            out.data_ptr(), torch.cuda.current_stream(data.device).cuda_stream)
-        if rc != _capi.ACB_OK:
-            raise RuntimeError(_capi.last_error())
+        _check(self._L.acb_rows_to_codepoints(data.data_ptr(), offsets.data_ptr(), offsets.numel() - 1, data.numel(), rows.data_ptr(),
+                                              out.data_ptr(), torch.cuda.current_stream(data.device).cuda_stream))
         return out
 
     def first_device(self, data, offsets, codepoints: bool = False, flt=None):
@@ -688,9 +750,7 @@ class _Automaton:
                     has = mo[1:] > mo[:-1]
                     first = m[mo[:-1].clamp(max=total - 1), 1:4].to(torch.int64)
                     rows = torch.where(has[:, None], first, rows)
-                reader = torch.cuda.Event()
-                reader.record(torch.cuda.current_stream(dev))
-                self._ws[(dev.index if dev.index is not None else torch.cuda.current_device(), 0)]["reader"] = reader
+                self._mark_read(dev)
                 self.last_stats = {"engine": self.last_stats.get("engine", "table"), "mode": "first"}
                 return rows
             keys = torch.full((n,), -1, dtype=torch.int64, device=dev)   # all ones: no match yet
@@ -708,30 +768,14 @@ class _Automaton:
         _first_one_large."""
         torch = _require_cuda()
         dev = data.device
-        n = offsets.numel() - 1
-        limit = self.WINDOW_BYTES
-        rows = torch.full((n, 3), -1, dtype=torch.int64, device=dev)
-        lens = offsets[1:] - offsets[:-1]
-        oversized = bool((lens > limit).any().item())
-        h = 0
-        while h < n:
-            start = int(offsets[h].item())
-            if oversized and int(lens[h].item()) > limit:
-                best = self._first_one_large(data[start:start + int(lens[h].item())], _filter_slice(flt, h, h + 1))
+        rows = torch.full((offsets.numel() - 1, 3), -1, dtype=torch.int64, device=dev)
+        for h, h1, start, end, large in _haystack_runs(offsets, self.WINDOW_BYTES):
+            if large:
+                best = self._first_one_large(data[start:end], _filter_slice(flt, h, h1))
                 if best is not None:
                     rows[h] = torch.tensor(best, dtype=torch.int64, device=dev)
-                h += 1
-                continue
-            # the longest run of whole haystacks that fits one call (and stops before an oversized one)
-            h1 = int(torch.searchsorted(offsets, torch.tensor([start + limit], dtype=torch.int64, device=dev), right=True).item()) - 1
-            h1 = max(h + 1, min(h1, n))
-            if oversized:
-                big = torch.nonzero(lens[h:h1] > limit)
-                if big.numel():
-                    h1 = h + int(big[0].item())
-            end = int(offsets[h1].item())
-            rows[h:h1] = self.first_device(data[start:end], offsets[h:h1 + 1] - start, flt=_filter_slice(flt, h, h1))
-            h = h1
+            else:
+                rows[h:h1] = self.first_device(data[start:end], offsets[h:h1 + 1] - start, flt=_filter_slice(flt, h, h1))
         return rows
 
     def _first_one_large(self, hay, flt=None):
@@ -741,72 +785,50 @@ class _Automaton:
         earliest end.  The leftmost kinds: every match not seen yet ends past the current window, so it starts at or
         after the next window's start; the search stops once the best start lies strictly before that."""
         torch = _require_cuda()
-        dev = hay.device
-        limit = self.WINDOW_BYTES
-        step = limit - max(self.max_pattern_len - 1, 0)
+        halo = max(self.max_pattern_len - 1, 0)
         best = None
-        w0 = 0
-        while True:
-            w1 = min(w0 + limit, hay.numel())
-            p, s, e = self.first_device(hay[w0:w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=dev), flt=flt)[0].tolist()
+        for w0, w1 in _windows(hay.numel(), self.WINDOW_BYTES, halo):
+            p, s, e = self.first_device(hay[w0:w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=hay.device), flt=flt)[0].tolist()
             if p >= 0 and (best is None or self.first_order((p, s + w0, e + w0)) < self.first_order(best)):
                 best = (p, s + w0, e + w0)
-            if w1 == hay.numel():
-                return best
-            if best is not None and (self.matchkind == MatchKind.Standard or best[1] < w0 + step):
-                return best
-            w0 += step
+            if best is not None and (self.matchkind == MatchKind.Standard or best[1] < w1 - halo):
+                break
+        return best
+
+    @contextlib.contextmanager
+    def _host_staged(self, chunks):
+        """Host buffers (bytes-like objects, one per haystack) -> (data, offsets) on the current device: gathered into
+        the pinned staging buffer (_pack_host) and sent in one copy.  Also yields the host offsets and the host view of
+        the bytes (valid inside the block).  Holds _host_lock: the staging buffer, and the workspaces until the results
+        are on the host."""
+        torch = _torch()
+        dev = torch.device("cuda", torch.cuda.current_device())
+        with self._host_lock:
+            offs, head, total_bytes = _pack_host(lambda nbytes: self._pinned(nbytes).numpy(), chunks)
+            host = self._pinned(head + total_bytes)
+            d = host[:head + total_bytes].to(dev, non_blocking=True)
+            yield d[head:], d[:8 * len(offs)].view(torch.int64), offs, host.numpy()[head:head + total_bytes]
 
     def first_host_batch(self, chunks: Sequence[bytes], codepoints: bool, patterns=None):
         """Host buffers (bytes-like objects, one per haystack) -> list of (pattern, start, end) or None: each one's first
-        match.  The offsets and the haystacks are gathered into the pinned staging buffer and go to the device in one
-        copy; the rows come back in one."""
-        torch = _require_cuda()
-        n = len(chunks)
-        if n == 0:
+        match.  The offsets and the haystacks go to the device in one copy (_host_staged); the rows come back in one."""
+        _require_cuda()
+        if len(chunks) == 0:
             return []
-        offs = np.zeros(n + 1, dtype=np.int64)
-        np.cumsum(np.fromiter((len(c) for c in chunks), dtype=np.int64, count=n), out=offs[1:])
-        total_bytes = int(offs[-1])
-        head = (8 * (n + 1) + 511) & ~511   # the offsets, then the bytes at a 512-byte boundary of the buffer
-        dev = torch.device("cuda", torch.cuda.current_device())
-        with self._host_lock:
-            host = self._pinned(head + total_bytes)
-            hv = host.numpy()
-            hv[:8 * (n + 1)].view(np.int64)[:] = offs
-            if n == 1:
-                hv[head:head + total_bytes] = np.frombuffer(chunks[0], dtype=np.uint8)
-            elif total_bytes:
-                hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
-            d = host[:head + total_bytes].to(dev, non_blocking=True)
-            flt = _host_sets(self, patterns, n, dev) if patterns is not None else None
-            rows = self.first_device(d[head:], d[:8 * (n + 1)].view(torch.int64), codepoints, flt).cpu().tolist()
+        with self._host_staged(chunks) as (data, offsets, _, _):
+            flt = _host_sets(self, patterns, len(chunks), data.device) if patterns is not None else None
+            rows = self.first_device(data, offsets, codepoints, flt).cpu().tolist()
         return [tuple(r) if r[0] >= 0 else None for r in rows]
 
     def any_host_batch(self, chunks: Sequence[bytes], patterns=None):
         """Host buffers (bytes-like objects, one per haystack) -> list of bool: does each contain any pattern.  The
-        offsets and the haystacks are gathered into the pinned staging buffer and go to the device in one copy."""
-        torch = _require_cuda()
-        n = len(chunks)
-        if n == 0:
+        offsets and the haystacks go to the device in one copy (_host_staged)."""
+        _require_cuda()
+        if len(chunks) == 0:
             return []
-        offs = np.zeros(n + 1, dtype=np.int64)
-        np.cumsum(np.fromiter((len(c) for c in chunks), dtype=np.int64, count=n), out=offs[1:])
-        total_bytes = int(offs[-1])
-        head = (8 * (n + 1) + 511) & ~511   # the offsets, then the bytes at a 512-byte boundary of the buffer
-        dev = torch.device("cuda", torch.cuda.current_device())
-        with self._host_lock:
-            host = self._pinned(head + total_bytes)
-            hv = host.numpy()
-            hv[:8 * (n + 1)].view(np.int64)[:] = offs
-            if n == 1:
-                hv[head:head + total_bytes] = np.frombuffer(chunks[0], dtype=np.uint8)
-            elif total_bytes:
-                hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
-            d = host[:head + total_bytes].to(dev, non_blocking=True)
-            flt = _host_sets(self, patterns, n, dev) if patterns is not None else None
-            mask = self.any_device(d[head:], d[:8 * (n + 1)].view(torch.int64), flt=flt)
-            return mask.cpu().tolist()
+        with self._host_staged(chunks) as (data, offsets, _, _):
+            flt = _host_sets(self, patterns, len(chunks), data.device) if patterns is not None else None
+            return self.any_device(data, offsets, flt=flt).cpu().tolist()
 
     # ---- match counts per haystack: len(find_matches_as_indexes(h, overlapping)) without the list ----------------
     def count_device(self, data, offsets, overlapping=False, capacity: Optional[int] = None, flt=None):
@@ -834,43 +856,24 @@ class _Automaton:
             if flt is None and self._pick_engine(dev, data, offsets, overlapping) is not None:
                 _, mo, _ = self.scan_device(data, offsets, overlapping, False)
                 counts = mo[1:] - mo[:-1]
-                reader = torch.cuda.Event()
-                reader.record(stream)
-                self._ws[(dev.index if dev.index is not None else torch.cuda.current_device(), 0)]["reader"] = reader
+                self._mark_read(dev)
                 self.last_stats = {"engine": self.last_stats.get("engine", "table"), "mode": "count", "long_stretches": 0}
                 return counts
             sieve_t, _ = self.sieve(dev)
             counts = torch.zeros(n, dtype=torch.int64, device=dev)
             if overlapping:
                 scratch = torch.empty(3, dtype=torch.int64, device=dev)
-                rc = self._L.acb_count_overlapping_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n,
-                                                            data.numel(), counts.data_ptr(), scratch.data_ptr(), _filter_struct(flt),
-                                                            stream.cuda_stream)
-                if rc != _capi.ACB_OK:
-                    raise RuntimeError(_capi.last_error())
+                _check(self._L.acb_count_overlapping_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n,
+                                                              data.numel(), counts.data_ptr(), scratch.data_ptr(), _filter_struct(flt),
+                                                              stream.cuda_stream))
                 self.last_stats = {"engine": "sieve", "mode": "count", **self.sieve_geometry(dev, self._plan(data, n).task_bytes),
                                    "long_stretches": 0, **self._set_stats(flt)}
                 return counts
             plan = self._plan(data, n)
-            cap = capacity or max(1024, n * 2)
-            while True:
-                ws = self._workspace(dev, plan, n, cap, 0)
-                reader = ws.pop("reader", None)
-                if reader is not None:   # a comparison of an earlier call (maybe on another stream) reads this workspace first
-                    stream.wait_event(reader)
-                st = self._ws_struct(ws)
-                rc = self._L.acb_count_non_overlapping_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n,
-                                                                data.numel(), C.byref(plan), C.byref(st), counts.data_ptr(),
-                                                                _filter_struct(flt), stream.cuda_stream)
-                if rc != _capi.ACB_OK:
-                    err = _capi.last_error()
-                    ws["scratch"][:8].zero_()   # a scan that failed half way may have left its counters dirty
-                    raise RuntimeError(err)
-                tot = ws["total"].tolist()
-                total, complete, long_stretches, raw_total = tot[0], tot[1], tot[2], tot[4]
-                if complete or (total == 0 and raw_total == 0):
-                    break
-                cap = max(total, raw_total) + max(total, raw_total) // 8 + 16
+            _, tot = self._list_scan(dev, plan, n, capacity, lambda plan_ref, ws_ref: self._L.acb_count_non_overlapping_filtered(
+                self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(), plan_ref, ws_ref, counts.data_ptr(),
+                _filter_struct(flt), stream.cuda_stream))
+            long_stretches, raw_total = tot[2], tot[4]
             self.last_stats = {"engine": "sieve", "mode": "count", **self.sieve_geometry(dev, plan.task_bytes), "list_records": raw_total,
                                "long_stretches": long_stretches, **self._set_stats(flt)}
             return counts
@@ -881,33 +884,17 @@ class _Automaton:
         runs'."""
         torch = _require_cuda()
         dev = data.device
-        n = offsets.numel() - 1
-        limit = self.WINDOW_BYTES
-        counts = torch.zeros(n, dtype=torch.int64, device=dev)
-        lens = offsets[1:] - offsets[:-1]
-        oversized = bool((lens > limit).any().item())
-        long_stretches = 0
-        h = 0
-        while h < n:
-            start = int(offsets[h].item())
-            if oversized and int(lens[h].item()) > limit:
-                counts[h:h + 1] = self._count_one_large(data[start:start + int(lens[h].item())], overlapping, _filter_slice(flt, h, h + 1))
-                h += 1
-                continue
-            # the longest run of whole haystacks that fits one call (and stops before an oversized one)
-            h1 = int(torch.searchsorted(offsets, torch.tensor([start + limit], dtype=torch.int64, device=dev), right=True).item()) - 1
-            h1 = max(h + 1, min(h1, n))
-            if oversized:
-                big = torch.nonzero(lens[h:h1] > limit)
-                if big.numel():
-                    h1 = h + int(big[0].item())
-            end = int(offsets[h1].item())
-            counts[h:h1] = self.count_device(data[start:end], offsets[h:h1 + 1] - start, overlapping, flt=_filter_slice(flt, h, h1))
-            long_stretches += self.last_stats.get("long_stretches", 0)
-            h = h1
+        counts = torch.zeros(offsets.numel() - 1, dtype=torch.int64, device=dev)
+        long_stretches, engine = 0, None
+        for h, h1, start, end, large in _haystack_runs(offsets, self.WINDOW_BYTES):
+            if large:
+                counts[h:h1] = self._count_one_large(data[start:end], overlapping, _filter_slice(flt, h, h1))
+            else:
+                counts[h:h1] = self.count_device(data[start:end], offsets[h:h1 + 1] - start, overlapping, flt=_filter_slice(flt, h, h1))
+                long_stretches += self.last_stats.get("long_stretches", 0)
+            engine = self.last_stats.get("engine") or engine
         torch.cuda.current_stream(dev).synchronize()
-        self.last_stats = {"engine": self.last_stats.get("engine"), "mode": "count", "long_stretches": long_stretches, "windows": True,
-                           **self._set_stats(flt)}
+        self.last_stats = {"engine": engine, "mode": "count", "long_stretches": long_stretches, "windows": True, **self._set_stats(flt)}
         return counts
 
     def _count_one_large(self, hay, overlapping, flt=None):
@@ -919,51 +906,31 @@ class _Automaton:
         torch = _require_cuda()
         dev = hay.device
         if overlapping:
-            limit, halo = self.WINDOW_BYTES, max(self.max_pattern_len - 1, 0)
+            halo = max(self.max_pattern_len - 1, 0)
             total = torch.zeros(1, dtype=torch.int64, device=dev)
-            w0 = 0
-            while True:
-                w1 = min(w0 + limit, hay.numel())
+            for w0, w1 in _windows(hay.numel(), self.WINDOW_BYTES, halo):
                 total += self.count_device(hay[w0:w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=dev), True, flt=flt)
                 if w0 and halo:
                     total -= self.count_device(hay[w0:w0 + halo], torch.tensor([0, halo], dtype=torch.int64, device=dev), True, flt=flt)
-                if w1 == hay.numel():
-                    return total
-                w0 += limit - halo
+            return total
         rows = self._overlapping_rows_large(hay, False, flt).contiguous()
         count = torch.zeros(1, dtype=torch.int64, device=dev)
         if rows.shape[0]:
             scratch = torch.empty((rows.shape[0], 2), dtype=torch.int64, device=dev)   # 16 bytes per row
-            rc = self._L.acb_count_rows(self._h, rows.data_ptr(), rows.shape[0], scratch.data_ptr(), count.data_ptr(),
-                                        torch.cuda.current_stream(dev).cuda_stream)
-            if rc != _capi.ACB_OK:
-                raise RuntimeError(_capi.last_error())
+            _check(self._L.acb_count_rows(self._h, rows.data_ptr(), rows.shape[0], scratch.data_ptr(), count.data_ptr(),
+                                          torch.cuda.current_stream(dev).cuda_stream))
         return count
 
     def count_host_batch(self, chunks: Sequence[bytes], overlapping, patterns=None):
         """Host buffers (bytes-like objects, one per haystack) -> list of int: each one's match count.  The offsets and
-        the haystacks are gathered into the pinned staging buffer and go to the device in one copy."""
-        torch = _require_cuda()
+        the haystacks go to the device in one copy (_host_staged)."""
+        _require_cuda()
         self.check_overlapping(overlapping)
-        n = len(chunks)
-        if n == 0:
+        if len(chunks) == 0:
             return []
-        offs = np.zeros(n + 1, dtype=np.int64)
-        np.cumsum(np.fromiter((len(c) for c in chunks), dtype=np.int64, count=n), out=offs[1:])
-        total_bytes = int(offs[-1])
-        head = (8 * (n + 1) + 511) & ~511   # the offsets, then the bytes at a 512-byte boundary of the buffer
-        dev = torch.device("cuda", torch.cuda.current_device())
-        with self._host_lock:
-            host = self._pinned(head + total_bytes)
-            hv = host.numpy()
-            hv[:8 * (n + 1)].view(np.int64)[:] = offs
-            if n == 1:
-                hv[head:head + total_bytes] = np.frombuffer(chunks[0], dtype=np.uint8)
-            elif total_bytes:
-                hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
-            d = host[:head + total_bytes].to(dev, non_blocking=True)
-            flt = _host_sets(self, patterns, n, dev) if patterns is not None else None
-            return self.count_device(d[head:], d[:8 * (n + 1)].view(torch.int64), overlapping, flt=flt).cpu().tolist()
+        with self._host_staged(chunks) as (data, offsets, _, _):
+            flt = _host_sets(self, patterns, len(chunks), data.device) if patterns is not None else None
+            return self.count_device(data, offsets, overlapping, flt=flt).cpu().tolist()
 
     # ---- match counts per pattern: bincount of find_matches_as_indexes' patterns, summed over a batch, without the list
     def pattern_counts_device(self, data, offsets, overlapping=False, capacity: Optional[int] = None):
@@ -1002,41 +969,22 @@ class _Automaton:
             if self._pick_engine(dev, data, offsets, overlapping) is not None:
                 m, _, _ = self.scan_device(data, offsets, overlapping, False)
                 counts += torch.bincount(m[:, 1].long(), minlength=self.n_patterns)
-                reader = torch.cuda.Event()
-                reader.record(stream)
-                self._ws[(dev.index if dev.index is not None else torch.cuda.current_device(), 0)]["reader"] = reader
+                self._mark_read(dev)
                 self.last_stats = {"engine": self.last_stats.get("engine", "table"), "mode": "pattern_counts", "long_stretches": 0}
                 return
             sieve_t, _ = self.sieve(dev)
             if overlapping:
                 scratch = torch.empty(3, dtype=torch.int64, device=dev)
-                rc = self._L.acb_pattern_counts_overlapping(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n,
-                                                            data.numel(), counts.data_ptr(), scratch.data_ptr(), stream.cuda_stream)
-                if rc != _capi.ACB_OK:
-                    raise RuntimeError(_capi.last_error())
+                _check(self._L.acb_pattern_counts_overlapping(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n,
+                                                              data.numel(), counts.data_ptr(), scratch.data_ptr(), stream.cuda_stream))
                 self.last_stats = {"engine": "sieve", "mode": "pattern_counts", **self.sieve_geometry(dev, self._plan(data, n).task_bytes),
                                    "long_stretches": 0}
                 return
             plan = self._plan(data, n)
-            cap = capacity or max(1024, n * 2)
-            while True:
-                ws = self._workspace(dev, plan, n, cap, 0)
-                reader = ws.pop("reader", None)
-                if reader is not None:   # a comparison of an earlier call (maybe on another stream) reads this workspace first
-                    stream.wait_event(reader)
-                st = self._ws_struct(ws)
-                rc = self._L.acb_pattern_counts_non_overlapping(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n,
-                                                                data.numel(), C.byref(plan), C.byref(st), counts.data_ptr(),
-                                                                stream.cuda_stream)
-                if rc != _capi.ACB_OK:
-                    err = _capi.last_error()
-                    ws["scratch"][:8].zero_()   # a scan that failed half way may have left its counters dirty
-                    raise RuntimeError(err)
-                tot = ws["total"].tolist()
-                total, complete, long_stretches, raw_total = tot[0], tot[1], tot[2], tot[4]
-                if complete or (total == 0 and raw_total == 0):
-                    break
-                cap = max(total, raw_total) + max(total, raw_total) // 8 + 16   # (nothing was added: the counts stay as they were)
+            _, tot = self._list_scan(dev, plan, n, capacity, lambda plan_ref, ws_ref: self._L.acb_pattern_counts_non_overlapping(
+                self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(), plan_ref, ws_ref, counts.data_ptr(),
+                stream.cuda_stream))
+            long_stretches, raw_total = tot[2], tot[4]
             self.last_stats = {"engine": "sieve", "mode": "pattern_counts", **self.sieve_geometry(dev, plan.task_bytes),
                                "list_records": raw_total, "long_stretches": long_stretches}
 
@@ -1044,34 +992,15 @@ class _Automaton:
         """pattern_counts_device above WINDOW_BYTES: runs of whole haystacks that fit one call each add their counts;
         one haystack above the limit goes to _pattern_counts_one_large.  last_stats["long_stretches"] sums the runs'."""
         torch = _require_cuda()
-        dev = data.device
-        n = offsets.numel() - 1
-        limit = self.WINDOW_BYTES
-        lens = offsets[1:] - offsets[:-1]
-        oversized = bool((lens > limit).any().item())
-        long_stretches = 0
-        engine = None
-        h = 0
-        while h < n:
-            start = int(offsets[h].item())
-            if oversized and int(lens[h].item()) > limit:
-                self._pattern_counts_one_large(counts, data[start:start + int(lens[h].item())], overlapping)
-                h += 1
-                continue
-            # the longest run of whole haystacks that fits one call (and stops before an oversized one)
-            h1 = int(torch.searchsorted(offsets, torch.tensor([start + limit], dtype=torch.int64, device=dev), right=True).item()) - 1
-            h1 = max(h + 1, min(h1, n))
-            if oversized:
-                big = torch.nonzero(lens[h:h1] > limit)
-                if big.numel():
-                    h1 = h + int(big[0].item())
-            end = int(offsets[h1].item())
-            if end > start:
+        long_stretches, engine = 0, None
+        for h, h1, start, end, large in _haystack_runs(offsets, self.WINDOW_BYTES):
+            if large:
+                self._pattern_counts_one_large(counts, data[start:end], overlapping)
+            elif end > start:
                 self._pattern_counts_into(counts, data[start:end], offsets[h:h1 + 1] - start, overlapping)
                 long_stretches += self.last_stats.get("long_stretches", 0)
-                engine = self.last_stats.get("engine")
-            h = h1
-        torch.cuda.current_stream(dev).synchronize()
+            engine = self.last_stats.get("engine") or engine
+        torch.cuda.current_stream(data.device).synchronize()
         self.last_stats = {"engine": engine, "mode": "pattern_counts", "long_stretches": long_stretches, "windows": True}
 
     def _pattern_counts_one_large(self, counts, hay, overlapping):
@@ -1083,44 +1012,26 @@ class _Automaton:
         torch = _require_cuda()
         dev = hay.device
         if overlapping:
-            limit, halo = self.WINDOW_BYTES, max(self.max_pattern_len - 1, 0)
+            halo = max(self.max_pattern_len - 1, 0)
             head = torch.zeros_like(counts)
-            w0 = 0
-            while True:
-                w1 = min(w0 + limit, hay.numel())
+            for w0, w1 in _windows(hay.numel(), self.WINDOW_BYTES, halo):
                 self._pattern_counts_into(counts, hay[w0:w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=dev), True)
                 if w0 and halo:
                     self._pattern_counts_into(head, hay[w0:w0 + halo], torch.tensor([0, halo], dtype=torch.int64, device=dev), True)
-                if w1 == hay.numel():
-                    counts -= head
-                    return
-                w0 += limit - halo
+            counts -= head
+            return
         rows = self._scan_one_large(hay, False, False)
         counts += torch.bincount(rows[:, 1], minlength=self.n_patterns)
 
     def pattern_counts_host_batch(self, chunks: Sequence[bytes], overlapping):
         """Host buffers (bytes-like objects, one per haystack) -> list of int: each pattern's match count over all of
-        them.  The offsets and the haystacks are gathered into the pinned staging buffer and go to the device in one copy."""
-        torch = _require_cuda()
+        them.  The offsets and the haystacks go to the device in one copy (_host_staged)."""
+        _require_cuda()
         self.check_overlapping(overlapping)
-        n = len(chunks)
-        if n == 0:
+        if len(chunks) == 0:
             return [0] * self.n_patterns
-        offs = np.zeros(n + 1, dtype=np.int64)
-        np.cumsum(np.fromiter((len(c) for c in chunks), dtype=np.int64, count=n), out=offs[1:])
-        total_bytes = int(offs[-1])
-        head = (8 * (n + 1) + 511) & ~511   # the offsets, then the bytes at a 512-byte boundary of the buffer
-        dev = torch.device("cuda", torch.cuda.current_device())
-        with self._host_lock:
-            host = self._pinned(head + total_bytes)
-            hv = host.numpy()
-            hv[:8 * (n + 1)].view(np.int64)[:] = offs
-            if n == 1:
-                hv[head:head + total_bytes] = np.frombuffer(chunks[0], dtype=np.uint8)
-            elif total_bytes:
-                hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
-            d = host[:head + total_bytes].to(dev, non_blocking=True)
-            return self.pattern_counts_device(d[head:], d[:8 * (n + 1)].view(torch.int64), overlapping).cpu().tolist()
+        with self._host_staged(chunks) as (data, offsets, _, _):
+            return self.pattern_counts_device(data, offsets, overlapping).cpu().tolist()
 
     # ---- hits per haystack: the distinct patterns of find_matches_as_indexes with their counts, without the list ----
     def hits_device(self, data, offsets, overlapping=False, capacity: Optional[int] = None):
@@ -1154,32 +1065,21 @@ class _Automaton:
                 m, _, _ = self.scan_device(data, offsets, overlapping, False)
                 keys, counts = torch.unique(m[:, 0].long() * P + m[:, 1].long(), return_counts=True)
                 row_offsets = torch.searchsorted(keys, torch.arange(n + 1, dtype=torch.int64, device=dev) * P)
-                reader = torch.cuda.Event()
-                reader.record(stream)
-                self._ws[(dev.index if dev.index is not None else torch.cuda.current_device(), 0)]["reader"] = reader
+                self._mark_read(dev)
                 self.last_stats = {"engine": self.last_stats.get("engine", "table"), "mode": "matching_patterns", "long_stretches": 0,
                                    "rows": 0, "list_records": int(m.shape[0]), "hits": int(keys.numel())}
                 return row_offsets, keys % P, counts
             sieve_t, _ = self.sieve(dev)
             plan = self._plan(data, n)
-            cap = capacity or max(1024, n * 2)
+            cap = capacity
             row_words = self._hit_row_words
             rows = None
             while True:
-                ws = self._workspace(dev, plan, n, cap, 0)
-                reader = ws.pop("reader", None)
-                if reader is not None:   # a comparison of an earlier call (maybe on another stream) reads this workspace first
-                    stream.wait_event(reader)
                 if row_words and (rows is None or rows.numel() < row_words):
                     rows = torch.empty(row_words, dtype=torch.int32, device=dev)
-                st = self._ws_struct(ws)
-                rc = self._L.acb_pattern_hits(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
-                                              int(bool(overlapping)), C.byref(plan), C.byref(st),
-                                              rows.data_ptr() if rows is not None else None, row_words, stream.cuda_stream)
-                if rc != _capi.ACB_OK:
-                    err = _capi.last_error()
-                    ws["scratch"][:8].zero_()   # a scan that failed half way may have left its counters dirty
-                    raise (ValueError if rc == _capi.ACB_EUNSUPPORTED else RuntimeError)(err)
+                ws = self._list_attempt(dev, plan, n, cap, lambda plan_ref, ws_ref: self._L.acb_pattern_hits(
+                    self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(), int(bool(overlapping)), plan_ref,
+                    ws_ref, rows.data_ptr() if rows is not None else None, row_words, stream.cuda_stream))
                 hits, complete, long_stretches, n_rows, raw_total, need_words = ws["total"].tolist()[:6]
                 if complete:
                     break
@@ -1192,9 +1092,7 @@ class _Automaton:
             row_offsets = ws["match_offsets"][: n + 1].clone()
             out = ws["out"][:hits]
             patterns, counts = out[:, 1].long(), out[:, 2].long()
-            reader = torch.cuda.Event()
-            reader.record(stream)
-            ws["reader"] = reader
+            self._mark_read(dev)
             self.last_stats = {"engine": "sieve", "mode": "matching_patterns", **self.sieve_geometry(dev, plan.task_bytes),
                                "list_records": raw_total, "long_stretches": long_stretches, "rows": n_rows, "hits": hits}
             return row_offsets, patterns, counts
@@ -1206,40 +1104,24 @@ class _Automaton:
         torch = _require_cuda()
         dev = data.device
         n = offsets.numel() - 1
-        limit = self.WINDOW_BYTES
-        lens = offsets[1:] - offsets[:-1]
-        oversized = bool((lens > limit).any().item())
         sizes, patterns, counts = [], [], []
         stats = {"long_stretches": 0, "rows": 0, "list_records": 0}
         engine = None
-        h = 0
-        while h < n:
-            start = int(offsets[h].item())
-            if oversized and int(lens[h].item()) > limit:
-                size = int(lens[h].item())
-                pc = self.pattern_counts_device(data[start:start + size], torch.tensor([0, size], dtype=torch.int64, device=dev), overlapping)
+        for h, h1, start, end, large in _haystack_runs(offsets, self.WINDOW_BYTES):
+            if large:
+                pc = self.pattern_counts_device(data[start:end], torch.tensor([0, end - start], dtype=torch.int64, device=dev), overlapping)
                 pids = torch.nonzero(pc).flatten()
                 sizes.append(torch.tensor([pids.numel()], dtype=torch.int64, device=dev))
                 patterns.append(pids)
                 counts.append(pc[pids])
-                h += 1
-                continue
-            # the longest run of whole haystacks that fits one call (and stops before an oversized one)
-            h1 = int(torch.searchsorted(offsets, torch.tensor([start + limit], dtype=torch.int64, device=dev), right=True).item()) - 1
-            h1 = max(h + 1, min(h1, n))
-            if oversized:
-                big = torch.nonzero(lens[h:h1] > limit)
-                if big.numel():
-                    h1 = h + int(big[0].item())
-            end = int(offsets[h1].item())
-            ro, p, c = self.hits_device(data[start:end], offsets[h:h1 + 1] - start, overlapping)
-            sizes.append(ro[1:] - ro[:-1])
-            patterns.append(p)
-            counts.append(c)
-            for k in stats:
-                stats[k] += self.last_stats.get(k, 0)
+            else:
+                ro, p, c = self.hits_device(data[start:end], offsets[h:h1 + 1] - start, overlapping)
+                sizes.append(ro[1:] - ro[:-1])
+                patterns.append(p)
+                counts.append(c)
+                for k in stats:
+                    stats[k] += self.last_stats.get(k, 0)
             engine = self.last_stats.get("engine") or engine
-            h = h1
         row_offsets = torch.zeros(n + 1, dtype=torch.int64, device=dev)
         torch.cumsum(torch.cat(sizes), 0, out=row_offsets[1:])
         patterns, counts = torch.cat(patterns), torch.cat(counts)
@@ -1248,28 +1130,14 @@ class _Automaton:
 
     def hits_host_batch(self, chunks: Sequence[bytes], overlapping):
         """Host buffers (bytes-like objects, one per haystack) -> one list per haystack: the distinct pattern ids of its
-        matches, ascending.  The offsets and the haystacks are gathered into the pinned staging buffer and go to the
-        device in one copy."""
-        torch = _require_cuda()
+        matches, ascending.  The offsets and the haystacks go to the device in one copy (_host_staged)."""
+        _require_cuda()
         self.check_overlapping(overlapping)
         n = len(chunks)
         if n == 0:
             return []
-        offs = np.zeros(n + 1, dtype=np.int64)
-        np.cumsum(np.fromiter((len(c) for c in chunks), dtype=np.int64, count=n), out=offs[1:])
-        total_bytes = int(offs[-1])
-        head = (8 * (n + 1) + 511) & ~511   # the offsets, then the bytes at a 512-byte boundary of the buffer
-        dev = torch.device("cuda", torch.cuda.current_device())
-        with self._host_lock:
-            host = self._pinned(head + total_bytes)
-            hv = host.numpy()
-            hv[:8 * (n + 1)].view(np.int64)[:] = offs
-            if n == 1:
-                hv[head:head + total_bytes] = np.frombuffer(chunks[0], dtype=np.uint8)
-            elif total_bytes:
-                hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
-            d = host[:head + total_bytes].to(dev, non_blocking=True)
-            ro, p, _ = self.hits_device(d[head:], d[:8 * (n + 1)].view(torch.int64), overlapping)
+        with self._host_staged(chunks) as (data, offsets, _, _):
+            ro, p, _ = self.hits_device(data, offsets, overlapping)
             ro, p = ro.cpu().tolist(), p.cpu().tolist()
         return [p[ro[i]:ro[i + 1]] for i in range(n)]
 
@@ -1305,42 +1173,23 @@ class _Automaton:
             if flt is None and self._pick_engine(dev, data, offsets, overlapping) is not None:
                 m, _, _ = self.scan_device(data, offsets, overlapping, False)
                 self._mask_rows(words, bit_base, m, offsets)
-                reader = torch.cuda.Event()
-                reader.record(stream)
-                self._ws[(dev.index if dev.index is not None else torch.cuda.current_device(), 0)]["reader"] = reader
+                self._mark_read(dev)
                 self.last_stats = {"engine": self.last_stats.get("engine", "table"), "mode": "match_mask", "long_stretches": 0}
                 return words
             sieve_t, _ = self.sieve(dev)
             if overlapping:
                 scratch = torch.empty(3, dtype=torch.int64, device=dev)
-                rc = self._L.acb_match_mask_overlapping_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n,
-                                                                 data.numel(), words.data_ptr(), bit_base, scratch.data_ptr(),
-                                                                 _filter_struct(flt), stream.cuda_stream)
-                if rc != _capi.ACB_OK:
-                    raise RuntimeError(_capi.last_error())
+                _check(self._L.acb_match_mask_overlapping_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n,
+                                                                   data.numel(), words.data_ptr(), bit_base, scratch.data_ptr(),
+                                                                   _filter_struct(flt), stream.cuda_stream))
                 self.last_stats = {"engine": "sieve", "mode": "match_mask", **self.sieve_geometry(dev, self._plan(data, n).task_bytes),
                                    **self._set_stats(flt)}
                 return words
             plan = self._plan(data, n)
-            cap = capacity or max(1024, n * 2)
-            while True:
-                ws = self._workspace(dev, plan, n, cap, 0)
-                reader = ws.pop("reader", None)
-                if reader is not None:   # a comparison of an earlier call (maybe on another stream) reads this workspace first
-                    stream.wait_event(reader)
-                st = self._ws_struct(ws)
-                rc = self._L.acb_match_mask_non_overlapping_filtered(self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n,
-                                                                     data.numel(), C.byref(plan), C.byref(st), words.data_ptr(), bit_base,
-                                                                     _filter_struct(flt), stream.cuda_stream)
-                if rc != _capi.ACB_OK:
-                    err = _capi.last_error()
-                    ws["scratch"][:8].zero_()   # a scan that failed half way may have left its counters dirty
-                    raise RuntimeError(err)
-                tot = ws["total"].tolist()
-                total, complete, long_stretches, raw_total = tot[0], tot[1], tot[2], tot[4]
-                if complete or (total == 0 and raw_total == 0):
-                    break
-                cap = max(total, raw_total) + max(total, raw_total) // 8 + 16   # (nothing was OR-ed: the mask stays as it was)
+            _, tot = self._list_scan(dev, plan, n, capacity, lambda plan_ref, ws_ref: self._L.acb_match_mask_non_overlapping_filtered(
+                self._h, sieve_t.data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(), plan_ref, ws_ref, words.data_ptr(),
+                bit_base, _filter_struct(flt), stream.cuda_stream))
+            long_stretches, raw_total = tot[2], tot[4]
             self.last_stats = {"engine": "sieve", "mode": "match_mask", **self.sieve_geometry(dev, plan.task_bytes),
                                "list_records": raw_total, "long_stretches": long_stretches, **self._set_stats(flt)}
             return words
@@ -1352,45 +1201,24 @@ class _Automaton:
         if rows.shape[0] == 0:
             return
         rows = rows.contiguous()
-        rc = self._L.acb_mask_rows(rows.data_ptr(), rows.element_size(), rows.shape[0], offsets.data_ptr(), offsets.numel() - 1,
-                                   words.data_ptr(), bit_base, torch.cuda.current_stream(rows.device).cuda_stream)
-        if rc != _capi.ACB_OK:
-            raise RuntimeError(_capi.last_error())
+        _check(self._L.acb_mask_rows(rows.data_ptr(), rows.element_size(), rows.shape[0], offsets.data_ptr(), offsets.numel() - 1,
+                                     words.data_ptr(), bit_base, torch.cuda.current_stream(rows.device).cuda_stream))
 
     def _mask_windows(self, words, bit_base: int, data, offsets, overlapping, flt=None):
         """mask_device above WINDOW_BYTES: runs of whole haystacks that fit one call each OR their bits, from the run's
         first byte on; one haystack above the limit goes to _mask_one_large.  last_stats["long_stretches"] sums the
         runs'."""
         torch = _require_cuda()
-        dev = data.device
-        n = offsets.numel() - 1
-        limit = self.WINDOW_BYTES
-        lens = offsets[1:] - offsets[:-1]
-        oversized = bool((lens > limit).any().item())
-        long_stretches = 0
-        engine = None
-        h = 0
-        while h < n:
-            start = int(offsets[h].item())
-            if oversized and int(lens[h].item()) > limit:
-                self._mask_one_large(words, bit_base + start, data[start:start + int(lens[h].item())], overlapping, _filter_slice(flt, h, h + 1))
-                h += 1
-                continue
-            # the longest run of whole haystacks that fits one call (and stops before an oversized one)
-            h1 = int(torch.searchsorted(offsets, torch.tensor([start + limit], dtype=torch.int64, device=dev), right=True).item()) - 1
-            h1 = max(h + 1, min(h1, n))
-            if oversized:
-                big = torch.nonzero(lens[h:h1] > limit)
-                if big.numel():
-                    h1 = h + int(big[0].item())
-            end = int(offsets[h1].item())
-            if end > start:
+        long_stretches, engine = 0, None
+        for h, h1, start, end, large in _haystack_runs(offsets, self.WINDOW_BYTES):
+            if large:
+                self._mask_one_large(words, bit_base + start, data[start:end], overlapping, _filter_slice(flt, h, h1))
+            elif end > start:
                 self.mask_device(data[start:end], offsets[h:h1 + 1] - start, overlapping, flt=_filter_slice(flt, h, h1), words=words,
                                  bit_base=bit_base + start)
                 long_stretches += self.last_stats.get("long_stretches", 0)
-                engine = self.last_stats.get("engine") or engine
-            h = h1
-        torch.cuda.current_stream(dev).synchronize()
+            engine = self.last_stats.get("engine") or engine
+        torch.cuda.current_stream(data.device).synchronize()
         self.last_stats = {"engine": engine, "mode": "match_mask", "long_stretches": long_stretches, "windows": True,
                            **self._set_stats(flt)}
 
@@ -1402,15 +1230,10 @@ class _Automaton:
         torch = _require_cuda()
         dev = hay.device
         if overlapping:
-            limit, halo = self.WINDOW_BYTES, max(self.max_pattern_len - 1, 0)
-            w0 = 0
-            while True:
-                w1 = min(w0 + limit, hay.numel())
+            for w0, w1 in _windows(hay.numel(), self.WINDOW_BYTES, max(self.max_pattern_len - 1, 0)):
                 self.mask_device(hay[w0:w1], torch.tensor([0, w1 - w0], dtype=torch.int64, device=dev), True, flt=flt, words=words,
                                  bit_base=bit_base + w0)
-                if w1 == hay.numel():
-                    return
-                w0 += limit - halo
+            return
         rows = self._scan_one_large(hay, False, False, flt)
         self._mask_rows(words, bit_base, rows, torch.tensor([0, hay.numel()], dtype=torch.int64, device=dev))
 
@@ -1418,38 +1241,22 @@ class _Automaton:
         """acb_mask_unpack: bool CUDA tensor (n,), entry i = bit stride * i of the packed mask."""
         torch = _require_cuda()
         out = torch.empty(n, dtype=torch.bool, device=words.device)
-        rc = self._L.acb_mask_unpack(words.data_ptr(), 0, stride, n, out.data_ptr(), torch.cuda.current_stream(words.device).cuda_stream)
-        if rc != _capi.ACB_OK:
-            raise RuntimeError(_capi.last_error())
+        _check(self._L.acb_mask_unpack(words.data_ptr(), 0, stride, n, out.data_ptr(), torch.cuda.current_stream(words.device).cuda_stream))
         return out
 
     def spans_host_batch(self, chunks: Sequence[bytes], overlapping, codepoints: bool, patterns=None, unit: int = 1):
         """Host buffers (bytes-like objects, one per haystack) -> one list of (start, end) per haystack: the maximal
         runs of covered positions, haystack-relative, in code points with `codepoints`, else in bytes divided by `unit`.
-        The offsets and the haystacks are gathered into the pinned staging buffer and go to the device in one copy; the
-        packed mask (one bit per byte) comes back."""
-        torch = _require_cuda()
+        The offsets and the haystacks go to the device in one copy (_host_staged); the packed mask (one bit per byte)
+        comes back."""
+        _require_cuda()
         self.check_overlapping(overlapping)
-        n = len(chunks)
-        if n == 0:
+        if len(chunks) == 0:
             return []
-        offs = np.zeros(n + 1, dtype=np.int64)
-        np.cumsum(np.fromiter((len(c) for c in chunks), dtype=np.int64, count=n), out=offs[1:])
-        total_bytes = int(offs[-1])
-        head = (8 * (n + 1) + 511) & ~511   # the offsets, then the bytes at a 512-byte boundary of the buffer
-        dev = torch.device("cuda", torch.cuda.current_device())
-        with self._host_lock:
-            host = self._pinned(head + total_bytes)
-            hv = host.numpy()
-            hv[:8 * (n + 1)].view(np.int64)[:] = offs
-            if n == 1:
-                hv[head:head + total_bytes] = np.frombuffer(chunks[0], dtype=np.uint8)
-            elif total_bytes:
-                hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
-            d = host[:head + total_bytes].to(dev, non_blocking=True)
-            flt = _host_sets(self, patterns, n, dev) if patterns is not None else None
-            words = self.mask_device(d[head:], d[:8 * (n + 1)].view(torch.int64), overlapping, flt=flt).cpu().numpy()
-            text = hv[head:head + total_bytes].copy() if codepoints else None
+        with self._host_staged(chunks) as (data, offsets, offs, text):
+            flt = _host_sets(self, patterns, len(chunks), data.device) if patterns is not None else None
+            words = self.mask_device(data, offsets, overlapping, flt=flt).cpu().numpy()
+            text = text.copy() if codepoints else None
         return spans_from_words(words, offs, text, unit)
 
     def scan_device(self, data, offsets, overlapping=False, codepoints=False, capacity: Optional[int] = None,
@@ -1474,7 +1281,7 @@ class _Automaton:
                 raise ValueError(f"buffers above {self.WINDOW_BYTES} bytes are scanned in windows: sync=False is not available")
             return self._scan_device_windows(data, offsets, overlapping, codepoints, flt)
         img = self.image(dev)
-        cap = capacity or max(1024, n * 2)
+        cap = capacity
         stream = torch.cuda.current_stream(dev).cuda_stream
         with self._lock, torch.cuda.device(dev):
             hot = self._pick_engine(dev, data, offsets, overlapping) if flt is None else None   # (pattern sets: the sieve)
@@ -1483,21 +1290,11 @@ class _Automaton:
                 sieve_t, sieve_d = self.sieve(dev)
             plan = self._plan(data, n)
             while True:
-                ws = self._workspace(dev, plan, n, cap, ws_slot)
-                reader = ws.pop("reader", None)
-                if reader is not None:   # any_device's comparison (maybe on another stream) reads this workspace first
-                    torch.cuda.current_stream(dev).wait_event(reader)
-                st = self._ws_struct(ws)
-                rc = self._L.acb_scan_batch_filtered(self._h, img.data_ptr(),
-                                                     hot["tensor"].data_ptr() if hot else None, C.byref(hot["rows"]) if hot else None,
-                                                     sieve_t.data_ptr() if use_sieve else None,
-                                                     data.data_ptr(), offsets.data_ptr(), n, data.numel(),
-                                                     2 if overlapping == 2 else int(bool(overlapping)), int(bool(codepoints)), C.byref(plan),
-                                                     C.byref(st), _filter_struct(flt), stream)
-                if rc != _capi.ACB_OK:
-                    err = _capi.last_error()
-                    ws["scratch"][:8].zero_()   # a scan that failed half way may have left its counters dirty
-                    raise (ValueError if rc == _capi.ACB_EUNSUPPORTED else RuntimeError)(err)
+                ws = self._list_attempt(dev, plan, n, cap, lambda plan_ref, ws_ref: self._L.acb_scan_batch_filtered(
+                    self._h, img.data_ptr(), hot["tensor"].data_ptr() if hot else None, C.byref(hot["rows"]) if hot else None,
+                    sieve_t.data_ptr() if use_sieve else None, data.data_ptr(), offsets.data_ptr(), n, data.numel(),
+                    2 if overlapping == 2 else int(bool(overlapping)), int(bool(codepoints)), plan_ref, ws_ref, _filter_struct(flt),
+                    stream), ws_slot)
                 if not sync:
                     return ws["out"], ws["match_offsets"][: n + 1], ws["total"]
                 tot = ws["total"].tolist()
@@ -1529,31 +1326,17 @@ class _Automaton:
         torch = _require_cuda()
         dev = data.device
         n = offsets.numel() - 1
-        limit = self.WINDOW_BYTES
         parts = []          # (k, 4) int64 tensors in haystack order
         mo = torch.zeros(n + 1, dtype=torch.int64, device=dev)
-        lens = offsets[1:] - offsets[:-1]
-        oversized = bool((lens > limit).any().item()) if n else False
         base_count = 0
-        h = 0
-        while h < n:
-            start = int(offsets[h].item())
-            if oversized and int(lens[h].item()) > limit:
-                part = self._scan_one_large(data[start:start + int(lens[h].item())], overlapping, codepoints, _filter_slice(flt, h, h + 1))
+        for h, h1, start, end, large in _haystack_runs(offsets, self.WINDOW_BYTES):
+            if large:
+                part = self._scan_one_large(data[start:end], overlapping, codepoints, _filter_slice(flt, h, h1))
                 part[:, 0] = h
                 parts.append(part)
                 base_count += int(part.shape[0])
                 mo[h + 1] = base_count
-                h += 1
                 continue
-            # the longest run of whole haystacks that fits one call (and stops before an oversized one)
-            h1 = int(torch.searchsorted(offsets, torch.tensor([start + limit], dtype=torch.int64, device=dev), right=True).item()) - 1
-            h1 = max(h + 1, min(h1, n))
-            if oversized:
-                big = torch.nonzero(lens[h:h1] > limit)
-                if big.numel():
-                    h1 = h + int(big[0].item())
-            end = int(offsets[h1].item())
             sub_offs = offsets[h:h1 + 1] - start
             _t0 = __import__("time").perf_counter() if _TRACE else 0
             m, mo_run, total = self.scan_device(data[start:end], sub_offs, overlapping, codepoints, flt=_filter_slice(flt, h, h1))
@@ -1567,7 +1350,6 @@ class _Automaton:
             if _TRACE:
                 torch.cuda.synchronize()
                 print(f"[trace] run haystacks {h}..{h1} ({end - start} B): scan_device {(_t1 - _t0) * 1e3:.2f} ms, post {(__import__('time').perf_counter() - _t1) * 1e3:.2f} ms, total {total}", flush=True)
-            h = h1
         out = torch.cat(parts, dim=0) if len(parts) != 1 else parts[0]
         if not parts:
             out = torch.zeros((0, 4), dtype=torch.int64, device=dev)
@@ -1587,10 +1369,8 @@ class _Automaton:
         rows = rows.contiguous()
         out = torch.empty_like(rows)
         count = torch.zeros(1, dtype=torch.int64, device=dev)
-        rc = self._L.acb_select_non_overlapping(self._h, rows.data_ptr(), rows.shape[0], out.data_ptr(), count.data_ptr(),
-                                                torch.cuda.current_stream(dev).cuda_stream)
-        if rc != _capi.ACB_OK:
-            raise RuntimeError(_capi.last_error())
+        _check(self._L.acb_select_non_overlapping(self._h, rows.data_ptr(), rows.shape[0], out.data_ptr(), count.data_ptr(),
+                                                  torch.cuda.current_stream(dev).cuda_stream))
         return out[: int(count.item())]
 
     def _overlapping_rows_large(self, hay, codepoints, flt=None):
@@ -1743,8 +1523,7 @@ class _Automaton:
             h_in = torch.zeros(16 + cap_b + 16, dtype=torch.uint8, pin_memory=True)
             d_in = torch.zeros(16 + cap_b + 16, dtype=torch.uint8, device=dev)
             plan = _capi.Plan()
-            if self._L.acb_plan_scan(self._h, d_in.data_ptr() + 16, cap_b, 1, C.byref(plan)) != _capi.ACB_OK:
-                raise RuntimeError(_capi.last_error())
+            _check(self._L.acb_plan_scan(self._h, d_in.data_ptr() + 16, cap_b, 1, C.byref(plan)))
             cap = 4096
             n_units = int(plan.n_units) + 8
             res = torch.zeros(8 + 2 * cap, dtype=torch.int64, device=dev)
@@ -1784,8 +1563,7 @@ class _Automaton:
             d_in[:16 + n].copy_(ctx["h_in"][:16 + n], non_blocking=True)
             plan = ctx["plan"]
             base = d_in.data_ptr()
-            if self._L.acb_plan_scan(self._h, base + 16, n, 1, C.byref(plan)) != _capi.ACB_OK:
-                raise RuntimeError(_capi.last_error())
+            _check(self._L.acb_plan_scan(self._h, base + 16, n, 1, C.byref(plan)))
             if plan.scratch_words > ctx["max_scratch"] or plan.n_units > ctx["max_units"]:
                 return None   # (a tuning knob changed the plan beyond what was allocated: let the general path do it)
             stream = torch.cuda.current_stream(dev)
@@ -1835,29 +1613,15 @@ class _Automaton:
     def _scan_host_batch_filtered(self, chunks: Sequence[bytes], overlapping: bool, codepoints: bool, patterns):
         """scan_host_batch with one pattern set per haystack: the haystacks are gathered into the pinned staging buffer
         with their offsets, go to the device in one copy and are scanned by scan_device with the sets (the sieve)."""
-        torch = _require_cuda()
+        _require_cuda()
         n = len(chunks)
-        dev = torch.device("cuda", torch.cuda.current_device())
-        offs = np.zeros(n + 1, dtype=np.int64)
-        if n:
-            np.cumsum(np.fromiter((len(c) for c in chunks), dtype=np.int64, count=n), out=offs[1:])
-        total_bytes = int(offs[-1])
         if n == 0:
             if len(list(patterns)) != 0:
                 raise ValueError("patterns= needs one set of pattern ids per haystack: 0 haystacks")
-            return np.zeros((0, 4), dtype=np.uint32), offs
-        head = (8 * (n + 1) + 511) & ~511   # the offsets, then the bytes at a 512-byte boundary of the buffer
-        with self._host_lock:
-            flt = _host_sets(self, patterns, n, dev)
-            host = self._pinned(head + total_bytes)
-            hv = host.numpy()
-            hv[:8 * (n + 1)].view(np.int64)[:] = offs
-            if n == 1:
-                hv[head:head + total_bytes] = np.frombuffer(chunks[0], dtype=np.uint8)
-            elif total_bytes:
-                hv[head:head + total_bytes] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
-            d = host[:head + total_bytes].to(dev, non_blocking=True)
-            m, mo, _ = self.scan_device(d[head:], d[:8 * (n + 1)].view(torch.int64), overlapping, codepoints, flt=flt)
+            return np.zeros((0, 4), dtype=np.uint32), np.zeros(1, dtype=np.int64)
+        with self._host_staged(chunks) as (data, offsets, _, _):
+            flt = _host_sets(self, patterns, n, data.device)
+            m, mo, _ = self.scan_device(data, offsets, overlapping, codepoints, flt=flt)
             m = m.cpu().numpy()
             return (m.view(np.uint32) if m.dtype == np.int32 else m), mo.cpu().numpy().astype(np.int64)
 
@@ -1937,10 +1701,8 @@ class StreamBatch:
             if self.device is None:
                 self._allocate(dev)
             stream = torch.cuda.current_stream(dev).cuda_stream
-            rc = L.acb_stream_seams(ac._h, data.data_ptr(), offsets.data_ptr(), n, data.numel(), self._carry.data_ptr(),
-                                    self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(), stream)
-            if rc != _capi.ACB_OK:
-                raise RuntimeError(_capi.last_error())
+            _check(L.acb_stream_seams(ac._h, data.data_ptr(), offsets.data_ptr(), n, data.numel(), self._carry.data_ptr(),
+                                      self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(), stream))
             # the overlapping lists, in bytes, of the chunks as they are and of the seams
             m_c, mo_c, tot_c = ac.scan_device(data, offsets, 2, False, ws_slot=self._slots[0])
             geometry = {k: ac.last_stats.get(k) for k in ("window", "last_level", "probes", "bloom_bytes", "ring", "task_bytes")}
@@ -2067,18 +1829,14 @@ class _QueryStreamBatch(StreamBatch):
                 self._allocate(dev)
                 self._allocate_query(dev)
             stream = torch.cuda.current_stream(dev).cuda_stream
-            rc = L.acb_stream_seams(ac._h, data.data_ptr(), offsets.data_ptr(), self.n_streams, data.numel(), self._carry.data_ptr(),
-                                    self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(), stream)
-            if rc != _capi.ACB_OK:
-                raise RuntimeError(_capi.last_error())
+            _check(L.acb_stream_seams(ac._h, data.data_ptr(), offsets.data_ptr(), self.n_streams, data.numel(), self._carry.data_ptr(),
+                                      self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(), stream))
             out, stats = self._query(dev, data, offsets, last_u8, stream)
             cp = self._codepoints and self.POSITIONS
             scratch = torch.empty(6 * self.n_streams if cp else 1, dtype=torch.int64, device=dev)
-            rc = L.acb_stream_advance(ac._h, data.data_ptr(), offsets.data_ptr(), self.n_streams, data.numel(),
-                                      last_u8.data_ptr() if last_u8 is not None else None, int(cp), self._carry.data_ptr(),
-                                      self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(), scratch.data_ptr(), stream)
-            if rc != _capi.ACB_OK:
-                raise RuntimeError(_capi.last_error())
+            _check(L.acb_stream_advance(ac._h, data.data_ptr(), offsets.data_ptr(), self.n_streams, data.numel(),
+                                        last_u8.data_ptr() if last_u8 is not None else None, int(cp), self._carry.data_ptr(),
+                                        self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(), scratch.data_ptr(), stream))
             task_bytes = int(ac._plan(data, max(self.n_streams, 1)).task_bytes)
             self.last_stats = {"engine": "sieve", "mode": self.MODE, **ac.sieve_geometry(dev, task_bytes),
                                "seam_bytes": int(self._seam_offsets[self.n_streams].item()), **stats, **ac._set_stats(self._flt)}
@@ -2108,10 +1866,8 @@ class IsMatchStreamBatch(_QueryStreamBatch):
         scratch = torch.empty((2, 3), dtype=torch.int64, device=dev)
         # the seams first: a stream whose match crosses the cut then has its chunk skipped
         for k, (b, o) in enumerate(((self._seam, self._seam_offsets), (data, offsets))):
-            rc = L.acb_any_match_filtered(ac._h, sieve_t.data_ptr(), b.data_ptr(), o.data_ptr(), n, b.numel(), self._flags.data_ptr(),
-                                          scratch[k].data_ptr(), _filter_struct(self._flt), stream)
-            if rc != _capi.ACB_OK:
-                raise RuntimeError(_capi.last_error())
+            _check(L.acb_any_match_filtered(ac._h, sieve_t.data_ptr(), b.data_ptr(), o.data_ptr(), n, b.numel(), self._flags.data_ptr(),
+                                            scratch[k].data_ptr(), _filter_struct(self._flt), stream))
         out = self._flags.clone()
         if last_u8 is not None:
             self._flags.masked_fill_(last_u8.view(torch.bool), False)
@@ -2140,13 +1896,11 @@ class FindFirstStreamBatch(_QueryStreamBatch):
         chunk_scratch = ac.first_keys(data, offsets, self._keys[1], self._flt)
         scratch = torch.empty(2 + 12 * n, dtype=torch.int64, device=dev)
         rows = torch.empty((n, 3), dtype=torch.int64, device=dev)
-        rc = L.acb_stream_first_resolve_filtered(ac._h, ac.sieve(dev)[0].data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
-                                                 last_u8.data_ptr() if last_u8 is not None else None, int(self._codepoints),
-                                                 self._carry.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(),
-                                                 self._seam.numel(), self._keys[0].data_ptr(), self._keys[1].data_ptr(), self._best.data_ptr(),
-                                                 scratch.data_ptr(), rows.data_ptr(), _filter_struct(self._flt), stream)
-        if rc != _capi.ACB_OK:
-            raise RuntimeError(_capi.last_error())
+        _check(L.acb_stream_first_resolve_filtered(ac._h, ac.sieve(dev)[0].data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
+                                                   last_u8.data_ptr() if last_u8 is not None else None, int(self._codepoints),
+                                                   self._carry.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(),
+                                                   self._seam.numel(), self._keys[0].data_ptr(), self._keys[1].data_ptr(), self._best.data_ptr(),
+                                                   scratch.data_ptr(), rows.data_ptr(), _filter_struct(self._flt), stream))
         return rows, {**self._skips(chunk_scratch), "pending": int(scratch[1].item())}
 
 
@@ -2169,10 +1923,8 @@ class CountStreamBatch(_QueryStreamBatch):
         if self.overlapping:
             chunk_counts = torch.zeros(n, dtype=torch.int64, device=dev)
             scratch = torch.empty(3, dtype=torch.int64, device=dev)
-            rc = L.acb_count_overlapping(ac._h, ac.sieve(dev)[0].data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
-                                         chunk_counts.data_ptr(), scratch.data_ptr(), stream)
-            if rc != _capi.ACB_OK:
-                raise RuntimeError(_capi.last_error())
+            _check(L.acb_count_overlapping(ac._h, ac.sieve(dev)[0].data_ptr(), data.data_ptr(), offsets.data_ptr(), n, data.numel(),
+                                           chunk_counts.data_ptr(), scratch.data_ptr(), stream))
             m_c = mo_c = None
             words = 4
         else:
@@ -2232,10 +1984,8 @@ class MaskStreamBatch(_QueryStreamBatch):
                 self._allocate_query(dev)
             stream = torch.cuda.current_stream(dev).cuda_stream
             last_p = last_u8.data_ptr() if last_u8 is not None else None
-            rc = L.acb_stream_seams(ac._h, data.data_ptr(), offsets.data_ptr(), n, data.numel(), self._carry.data_ptr(),
-                                    self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(), stream)
-            if rc != _capi.ACB_OK:
-                raise RuntimeError(_capi.last_error())
+            _check(L.acb_stream_seams(ac._h, data.data_ptr(), offsets.data_ptr(), n, data.numel(), self._carry.data_ptr(),
+                                      self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(), stream))
             chunk_bits = torch.zeros(max((data.numel() + 31) // 32, 1), dtype=torch.int32, device=dev)
             seam_bits = torch.zeros(max((self._seam.numel() + 31) // 32, 1), dtype=torch.int32, device=dev)
             if self.overlapping:
@@ -2243,10 +1993,8 @@ class MaskStreamBatch(_QueryStreamBatch):
                 sieve_t = ac.sieve(dev)[0]
                 scratch = torch.empty(3, dtype=torch.int64, device=dev)
                 for b, o, w in ((data, offsets, chunk_bits), (self._seam, self._seam_offsets, seam_bits)):
-                    rc = L.acb_match_mask_overlapping_filtered(ac._h, sieve_t.data_ptr(), b.data_ptr(), o.data_ptr(), n, b.numel(),
-                                                               w.data_ptr(), 0, scratch.data_ptr(), flt, stream)
-                    if rc != _capi.ACB_OK:
-                        raise RuntimeError(_capi.last_error())
+                    _check(L.acb_match_mask_overlapping_filtered(ac._h, sieve_t.data_ptr(), b.data_ptr(), o.data_ptr(), n, b.numel(),
+                                                                 w.data_ptr(), 0, scratch.data_ptr(), flt, stream))
                 stats = {}
             else:
                 # the overlapping lists, in bytes, of the chunks as they are and of the seams (as StreamBatch.feed_device)
@@ -2263,16 +2011,12 @@ class MaskStreamBatch(_QueryStreamBatch):
                 scratch = torch.empty(2 + 6 * n + 4 * cap, dtype=torch.int64, device=dev)
                 rows = torch.empty((max(cap, 1), 4), dtype=torch.int64, device=dev)
                 row_offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
-                rc = L.acb_stream_resolve(ac._h, None, data.data_ptr(), offsets.data_ptr(), n, data.numel(), last_p, 0, 0,
-                                          self._carry.data_ptr(), self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(),
-                                          ptr(m_s), mo_s.data_ptr(), ptr(m_c), mo_c.data_ptr(), scratch.data_ptr(), rows.data_ptr(),
-                                          row_offsets.data_ptr(), stream)
-                if rc != _capi.ACB_OK:
-                    raise RuntimeError(_capi.last_error())
-                rc = L.acb_stream_mask_rows(offsets.data_ptr(), n, carry_before.data_ptr(), self._seam_offsets.data_ptr(), rows.data_ptr(),
-                                            row_offsets.data_ptr(), chunk_bits.data_ptr(), seam_bits.data_ptr(), stream)
-                if rc != _capi.ACB_OK:
-                    raise RuntimeError(_capi.last_error())
+                _check(L.acb_stream_resolve(ac._h, None, data.data_ptr(), offsets.data_ptr(), n, data.numel(), last_p, 0, 0,
+                                            self._carry.data_ptr(), self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(),
+                                            ptr(m_s), mo_s.data_ptr(), ptr(m_c), mo_c.data_ptr(), scratch.data_ptr(), rows.data_ptr(),
+                                            row_offsets.data_ptr(), stream))
+                _check(L.acb_stream_mask_rows(offsets.data_ptr(), n, carry_before.data_ptr(), self._seam_offsets.data_ptr(), rows.data_ptr(),
+                                              row_offsets.data_ptr(), chunk_bits.data_ptr(), seam_bits.data_ptr(), stream))
                 stats = {"records": scratch[0]}
             flags = torch.empty(max(data.numel() + n * self._halo, 1), dtype=torch.bool, device=dev)
             flag_offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
@@ -2285,10 +2029,8 @@ class MaskStreamBatch(_QueryStreamBatch):
                 raise (ValueError if rc == _capi.ACB_EUNSUPPORTED else RuntimeError)(_capi.last_error())
             self._held = (held_out, held_in)
             if self.overlapping:
-                rc = L.acb_stream_advance(ac._h, data.data_ptr(), offsets.data_ptr(), n, data.numel(), last_p, 0, self._carry.data_ptr(),
-                                          self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(), None, stream)
-                if rc != _capi.ACB_OK:
-                    raise RuntimeError(_capi.last_error())
+                _check(L.acb_stream_advance(ac._h, data.data_ptr(), offsets.data_ptr(), n, data.numel(), last_p, 0, self._carry.data_ptr(),
+                                            self._tail.data_ptr(), self._seam.data_ptr(), self._seam_offsets.data_ptr(), None, stream))
             counts = torch.stack([flag_offsets[n], self._seam_offsets[n], self._carry[:, 2].sum(), *stats.values()]).tolist()
             k, seam_bytes, held = counts[:3]
             task_bytes = int(ac._plan(data, max(n, 1)).task_bytes)
@@ -3038,8 +2780,7 @@ def _encode_host_tokens(seq, what: str) -> np.ndarray:
         return np.zeros(0, dtype=np.uint8)
     out = np.empty(_capi.ACB_TOKEN_BYTES * ids.size, dtype=np.uint8)
     bad = np.full(1, np.iinfo(np.uint64).max, dtype=np.uint64)
-    if _capi.lib().acb_tokens_encode_host(ids.ctypes.data, ids.itemsize, ids.size, out.ctypes.data, bad.ctypes.data) != _capi.ACB_OK:
-        raise RuntimeError(_capi.last_error())
+    _check(_capi.lib().acb_tokens_encode_host(ids.ctypes.data, ids.itemsize, ids.size, out.ctypes.data, bad.ctypes.data))
     if bad[0] != np.iinfo(np.uint64).max:
         j = int(bad[0])
         raise _token_range_error(what, j, int(a[j]))
@@ -3146,8 +2887,7 @@ class _TokenEncoder:
         with torch.cuda.device(dev):
             rc = _capi.lib().acb_tokens_encode(tokens.data_ptr(), tokens.element_size(), n, buf.data_ptr(), bad.data_ptr(),
                                                stream.cuda_stream)
-        if rc != _capi.ACB_OK:
-            raise RuntimeError(_capi.last_error())
+        _check(rc)
         self._readers.pop(idx, None)
         j = int(bad.item())
         if j != -1:
@@ -3330,11 +3070,7 @@ class TokenAhoCorasick(_PatternSetMethods):
             with self._ac._lock:
                 m, mo, total = self._ac.scan_device(data, offs, overlapping, codepoints=False, capacity=capacity, flt=flt)
                 out = _token_rows(m, slice(2, 4)), mo.clone(), total
-                ws = self._ac._ws.get((data.device.index, 0))
-                if ws is not None:
-                    reader = torch.cuda.Event()
-                    reader.record(torch.cuda.current_stream(data.device))
-                    ws["reader"] = reader
+                self._ac._mark_read(data.device)
             return out
         return self._on_device(query, tokens, offsets)
 
@@ -3500,19 +3236,15 @@ class TokenAhoCorasick(_PatternSetMethods):
         L = self._ac._L
         st = torch.cuda.current_stream(dev).cuda_stream
         counts = torch.empty(n, dtype=torch.int64, device=dev)
-        rc = L.acb_completions_count(self._ac._h, img.data_ptr(), tokens.data_ptr(), tokens.element_size(), tokens.numel(),
-                                     offsets.data_ptr(), n, counts.data_ptr(), _filter_struct(flt), st)
-        if rc != _capi.ACB_OK:
-            raise RuntimeError(_capi.last_error())
+        _check(L.acb_completions_count(self._ac._h, img.data_ptr(), tokens.data_ptr(), tokens.element_size(), tokens.numel(),
+                                       offsets.data_ptr(), n, counts.data_ptr(), _filter_struct(flt), st))
         row_offsets = torch.zeros(n + 1, dtype=torch.int64, device=dev)
         torch.cumsum(counts, 0, out=row_offsets[1:])
         k = int(row_offsets[-1].item())
         ids = torch.empty(k, dtype=torch.int64, device=dev)
         if k:
-            rc = L.acb_completions_emit(self._ac._h, img.data_ptr(), tokens.data_ptr(), tokens.element_size(), tokens.numel(),
-                                        offsets.data_ptr(), n, row_offsets.data_ptr(), ids.data_ptr(), _filter_struct(flt), st)
-            if rc != _capi.ACB_OK:
-                raise RuntimeError(_capi.last_error())
+            _check(L.acb_completions_emit(self._ac._h, img.data_ptr(), tokens.data_ptr(), tokens.element_size(), tokens.numel(),
+                                          offsets.data_ptr(), n, row_offsets.data_ptr(), ids.data_ptr(), _filter_struct(flt), st))
             # each row's ids come out distinct and ascending per trie node: one sort of (row, id) keys orders them
             rows = torch.repeat_interleave(torch.arange(n, device=dev), counts, output_size=k)
             ids = torch.bitwise_and(torch.sort(rows * _capi.ACB_TOKEN_ID_LIMIT + ids).values, _capi.ACB_TOKEN_ID_LIMIT - 1)
@@ -3540,8 +3272,7 @@ class TokenAhoCorasick(_PatternSetMethods):
             rc = self._ac._L.acb_completions_mask(self._ac._h, img.data_ptr(), tokens.data_ptr(), tokens.element_size(), tokens.numel(),
                                                   offsets.data_ptr(), n, logits.data_ptr(), code, logits.stride(0) if n > 1 else V, V,
                                                   float(value), _filter_struct(flt), torch.cuda.current_stream(tokens.device).cuda_stream)
-        if rc != _capi.ACB_OK:
-            raise RuntimeError(_capi.last_error())
+        _check(rc)
         self._completions_stats(desc)
         return logits
 
@@ -3603,8 +3334,7 @@ class TokenAhoCorasick(_PatternSetMethods):
                                                       tokens.numel(), offsets.data_ptr(), n, bias.data_ptr(), logits.data_ptr(), code,
                                                       logits.stride(0) if n > 1 else V, V, _filter_struct(flt),
                                                       torch.cuda.current_stream(tokens.device).cuda_stream)
-            if rc != _capi.ACB_OK:
-                raise RuntimeError(_capi.last_error())
+            _check(rc)
         self._completions_stats(desc)
         return logits
 
