@@ -3,7 +3,7 @@
 Mirrors the reference's pysrc/ahocorasick_rs/__init__.py:1-23 (same exported
 names, including the deprecated MATCHKIND_* constants); the scan runs in
 hand-written sm_90a CUDA kernels behind the C ABI in include/acb200.h."""
-from .matcher import AhoCorasick, BytesAhoCorasick, TokenAhoCorasick, MatchKind, Implementation
+from .matcher import AhoCorasick, BytesAhoCorasick, TokenAhoCorasick, TokenVocabulary, MatchKind, Implementation
 
 # Backwards compatibility (reference: pysrc/ahocorasick_rs/__init__.py:10-12)
 MATCHKIND_STANDARD = MatchKind.Standard
@@ -14,6 +14,7 @@ __all__ = [
     "AhoCorasick",
     "BytesAhoCorasick",
     "TokenAhoCorasick",
+    "TokenVocabulary",
     "MatchKind",
     "Implementation",
     "MATCHKIND_STANDARD",

@@ -15,6 +15,7 @@ ACB_EINVAL, ACB_EBUILD, ACB_EUNSUPPORTED, ACB_ECUDA, ACB_ECAPACITY = -1, -2, -3,
 ACB_TOKEN_ID_LIMIT = 1 << 21   # include/acb200.h: token ids lie in [0, ACB_TOKEN_ID_LIMIT)
 ACB_TOKEN_BYTES = 3            # ... and each becomes this many bytes (csrc/tokens.cuh)
 ACB_LOGITS_F32, ACB_LOGITS_F16, ACB_LOGITS_BF16 = 0, 1, 2   # include/acb200.h: acb_completions_mask's / _bias's logits dtypes
+ACB_VOCAB_MAX_IDS = ACB_VOCAB_MAX_BYTES = (1 << 31) - 1   # include/acb200.h: the vocabulary image's index widths
 ACB_LONG_STRETCH = 4096   # include/acb200.h: longer per-haystack overlapping lists are counted by the whole grid
 
 
@@ -46,6 +47,11 @@ class SieveDesc(C.Structure):
 
 class CompletionsDesc(C.Structure):
     _fields_ = [("nodes", C.c_uint32), ("entries", C.c_uint32), ("depth", C.c_uint32), ("max_last", C.c_uint32)]
+
+
+class VocabDesc(C.Structure):
+    _fields_ = [("n_vocab", C.c_uint32), ("states", C.c_uint32), ("columns", C.c_uint32), ("max_pattern_len", C.c_uint32),
+                ("extra_dfa_bytes", C.c_uint64), ("tail_hit_ids", C.c_uint32), ("reserved", C.c_uint32)]
 
 
 class HotDesc(C.Structure):
@@ -161,6 +167,10 @@ def lib():
         L.acb_completions_emit.argtypes = compl + [C.c_void_p, C.c_void_p, F, C.c_void_p]
         L.acb_completions_mask.argtypes = compl + [C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_float, F, C.c_void_p]
         L.acb_completions_bias.argtypes = compl + [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64, F, C.c_void_p]
+        L.acb_vocab_build.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
+        L.acb_vocab_write.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]
+        L.acb_vocab_describe.argtypes = [C.c_void_p, C.POINTER(VocabDesc)]
+        L.acb_vocab_mask.argtypes = compl + [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_float, F, C.c_void_p]
         _lib = L
     return _lib
 
@@ -202,5 +212,5 @@ EXPORTS = [
     "acb_match_mask_overlapping", "acb_match_mask_overlapping_filtered", "acb_match_mask_non_overlapping",
     "acb_match_mask_non_overlapping_filtered", "acb_mask_rows", "acb_mask_unpack", "acb_stream_mask_rows", "acb_stream_mask_emit",
     "acb_completions_build", "acb_completions_write", "acb_completions_describe", "acb_completions_count", "acb_completions_emit",
-    "acb_completions_mask", "acb_completions_bias",
+    "acb_completions_mask", "acb_completions_bias", "acb_vocab_build", "acb_vocab_write", "acb_vocab_describe", "acb_vocab_mask",
 ]

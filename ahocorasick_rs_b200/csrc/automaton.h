@@ -5,6 +5,7 @@
 // out for HBM rather than for a CPU cache: see DESIGN.md "Data layout".
 #pragma once
 #include <cstdint>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -84,6 +85,7 @@ struct Automaton {
     std::vector<uint8_t> sieve;       // built by acb_sieve_build
     uint32_t sieve_bloom_max = 0, sieve_w_max = 0;
     std::vector<uint8_t> completions; // built by acb_completions_build (token-format patterns only), under sieve_mutex
+    std::unique_ptr<Automaton> vocab_dfa;  // a Standard build of the patterns for vocabularies of a leftmost automaton (vocab.h), under sieve_mutex
 };
 
 // Builds the automaton; throws std::runtime_error with a message on failure.

@@ -16,6 +16,7 @@
 #include "scan_sieve.cuh"
 #include "tokens.cuh"
 #include "completions.cuh"
+#include "vocab.cuh"
 
 namespace acb {
 
@@ -3984,14 +3985,20 @@ static int completions_check(const acb_automaton *a, const void *dev_image, cons
     return filter_view(a, filter, n_rows, F, filt);
 }
 
-// the logits checks of the mask and bias modes: the pointer, the dtype code, V, the row stride, and V > max_last
-static int completions_logits_check(const ComplHeader &h, int64_t n_rows, const void *dev_logits, int logits_dtype, int64_t row_stride,
-                                    int64_t vocab) {
+// the logits checks every logits writer makes: the pointer, the dtype code, V and the row stride
+static int logits_check(int64_t n_rows, const void *dev_logits, int logits_dtype, int64_t row_stride, int64_t vocab) {
     if (n_rows && !dev_logits) return fail(ACB_EINVAL, "null argument");
     if (logits_dtype != ACB_LOGITS_F32 && logits_dtype != ACB_LOGITS_F16 && logits_dtype != ACB_LOGITS_BF16)
         return fail(ACB_EINVAL, "logits_dtype must be ACB_LOGITS_F32, ACB_LOGITS_F16 or ACB_LOGITS_BF16");
     if (vocab < 1 || vocab >= (1ll << 62)) return fail(ACB_EINVAL, "vocab out of range (1 .. 2^62 - 1)");
     if (row_stride < 0 || row_stride >= (1ll << 62)) return fail(ACB_EINVAL, "row_stride out of range (0 .. 2^62 - 1)");
+    return ACB_OK;
+}
+
+// the logits checks of the mask and bias modes: logits_check, and V > max_last
+static int completions_logits_check(const ComplHeader &h, int64_t n_rows, const void *dev_logits, int logits_dtype, int64_t row_stride,
+                                    int64_t vocab) {
+    if (int rc = logits_check(n_rows, dev_logits, logits_dtype, row_stride, vocab)) return rc;
     if (h.n_entries && (int64_t)h.max_last >= vocab)
         return fail(ACB_EINVAL, "vocab " + std::to_string(vocab) + " does not hold the largest completing id " + std::to_string(h.max_last));
     return ACB_OK;
@@ -4126,6 +4133,132 @@ int acb_completions_bias(const acb_automaton *a, const void *dev_image, const vo
         completions_bias_dispatch<__nv_bfloat16>(token_bytes, filt, V, dev_tokens, n_tokens, dev_offsets, n_rows, F, dev_bias, dev_logits,
                                                  row_stride, vocab, d.sms, st);
     g_launches++;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+}  // extern "C"
+
+// ===========================================================================
+// Vocabulary masks (vocab.h, vocab.cuh)
+// ===========================================================================
+// the Standard DFA a vocabulary image of `a` copies: the automaton's own when its kind is Standard, otherwise a Standard
+// build of its patterns, made once and kept (extra = its image bytes)
+static int vocab_dfa(acb_automaton *a, const Automaton *&dfa, uint64_t &extra) {
+    Automaton &A = *a->impl;
+    if (A.hdr.match_kind == ACB_STANDARD) {
+        dfa = &A;
+        extra = 0;
+        return ACB_OK;
+    }
+    std::lock_guard<std::mutex> lock(A.sieve_mutex);
+    if (!A.vocab_dfa) {
+        try {
+            A.vocab_dfa.reset(build_automaton(A.pat_blob.data(), A.pat_offs.data(), A.hdr.n_patterns, ACB_STANDARD, A.implementation));
+        } catch (const std::exception &e) {
+            return fail(ACB_EBUILD, e.what());
+        }
+    }
+    dfa = A.vocab_dfa.get();
+    extra = dfa->image.size();
+    return ACB_OK;
+}
+
+// the checks of acb_vocab_build / _write, before anything is built
+static int vocab_args(const acb_automaton *a, const uint8_t *blob, const uint64_t *offsets, uint64_t n_vocab) {
+    if (!a || !offsets) return fail(ACB_EINVAL, "null argument");
+    if (n_vocab > kVocabMaxIds) return fail(ACB_EINVAL, "n_vocab " + std::to_string(n_vocab) + " exceeds ACB_VOCAB_MAX_IDS");
+    const std::string why = vocab_check(offsets, n_vocab);
+    if (!why.empty()) return fail(ACB_EINVAL, why);
+    if (offsets[n_vocab] && !blob) return fail(ACB_EINVAL, "null argument");
+    return ACB_OK;
+}
+
+template <typename T>
+static void vocab_state_launch(const void *img, const void *tokens, uint64_t n_tokens, const int64_t *offsets, int64_t n_rows,
+                               uint32_t *state, int sms, cudaStream_t st) {
+    constexpr int64_t kWarps = kVocabThreads / 32;
+    int64_t blocks = (n_rows + kWarps - 1) / kWarps;
+    if (blocks > 32ll * sms) blocks = 32ll * sms;   // grid-stride beyond that
+    vocab_state_kernel<T><<<(unsigned)blocks, kVocabThreads, 0, st>>>(static_cast<const uint8_t *>(img), static_cast<const T *>(tokens),
+                                                                      n_tokens, offsets, n_rows, state);
+}
+
+template <typename L>
+static void vocab_mask_launch(bool filt, const void *img, const uint32_t *state, int64_t n_rows, const SieveFilter &F, void *logits,
+                              int64_t row_stride, int64_t vocab, float value, cudaStream_t st) {
+    // x strides over the candidate ids (at most V; the kernel stops at n_vocab), y over the row tiles
+    const int64_t x = (vocab + kVocabThreads - 1) / kVocabThreads;
+    const int64_t y = (n_rows + kVocabRows - 1) / kVocabRows;
+    const dim3 grid((unsigned)(x < 4096 ? x : 4096), (unsigned)(y < 65535 ? y : 65535));
+    if (filt)
+        vocab_mask_kernel<L, true><<<grid, kVocabThreads, 0, st>>>(static_cast<const uint8_t *>(img), state, n_rows, F, static_cast<L *>(logits),
+                                                                   row_stride, vocab, value);
+    else
+        vocab_mask_kernel<L, false><<<grid, kVocabThreads, 0, st>>>(static_cast<const uint8_t *>(img), state, n_rows, F,
+                                                                    static_cast<L *>(logits), row_stride, vocab, value);
+}
+
+extern "C" {
+
+int acb_vocab_build(acb_automaton *a, const uint8_t *blob, const uint64_t *offsets, uint64_t n_vocab, uint64_t *image_bytes) {
+    if (!image_bytes) return fail(ACB_EINVAL, "null argument");
+    if (int rc = vocab_args(a, blob, offsets, n_vocab)) return rc;
+    const Automaton *dfa;
+    uint64_t extra;
+    if (int rc = vocab_dfa(a, dfa, extra)) return rc;
+    *image_bytes = vocab_image_bytes(dfa->image.size(), dfa->hdr.n_states, n_vocab, offsets[n_vocab]);
+    return ACB_OK;
+}
+
+int acb_vocab_write(acb_automaton *a, const uint8_t *blob, const uint64_t *offsets, uint64_t n_vocab, void *host_dst, uint64_t dst_bytes) {
+    if (!host_dst) return fail(ACB_EINVAL, "null argument");
+    if (int rc = vocab_args(a, blob, offsets, n_vocab)) return rc;
+    const Automaton *dfa;
+    uint64_t extra;
+    if (int rc = vocab_dfa(a, dfa, extra)) return rc;
+    if (dst_bytes < vocab_image_bytes(dfa->image.size(), dfa->hdr.n_states, n_vocab, offsets[n_vocab]))
+        return fail(ACB_ECAPACITY, "vocabulary image buffer too small");
+    vocab_image_build(*dfa, extra, blob, offsets, n_vocab, static_cast<uint8_t *>(host_dst));
+    return ACB_OK;
+}
+
+int acb_vocab_describe(const void *host_image, acb_vocab_desc *d) {
+    const VocabHeader *h = static_cast<const VocabHeader *>(host_image);
+    if (!h || !d || h->magic != kVocabMagic) return fail(ACB_EINVAL, "not a vocabulary image");
+    d->n_vocab = h->n_vocab;
+    d->states = h->n_states;
+    d->columns = h->n_cols;
+    d->max_pattern_len = h->max_pat_len;
+    d->extra_dfa_bytes = h->extra_dfa_bytes;
+    d->tail_hit_ids = h->n_tail_hits;
+    d->reserved = 0;
+    return ACB_OK;
+}
+
+int acb_vocab_mask(const acb_automaton *a, const void *dev_image, const void *dev_tokens, int token_bytes, uint64_t n_tokens,
+                   const int64_t *dev_offsets, int64_t n_rows, uint32_t *dev_state, void *dev_logits, int logits_dtype, int64_t row_stride,
+                   int64_t vocab, float value, const acb_pattern_filter *filter, void *stream) {
+    if (!a || !dev_image || (n_tokens && !dev_tokens) || (n_rows && (!dev_offsets || !dev_state))) return fail(ACB_EINVAL, "null argument");
+    if (token_bytes != 2 && token_bytes != 4 && token_bytes != 8) return fail(ACB_EINVAL, "token_bytes must be 2, 4 or 8");
+    if (n_tokens >= (1ull << 60)) return fail(ACB_EINVAL, "n_tokens must be below 2^60");
+    if (n_rows < 0 || n_rows > 0xfffffffell) return fail(ACB_EINVAL, "n_rows out of range (0 .. 2^32 - 2)");
+    SieveFilter F{};
+    bool filt = false;
+    if (int rc = filter_view(a, filter, n_rows, F, filt)) return rc;
+    if (filt && F.n_sets >= kVocabNoSet) return fail(ACB_EINVAL, "pattern filter: n_sets must be below 2^32 - 1");
+    if (int rc = logits_check(n_rows, dev_logits, logits_dtype, row_stride, vocab)) return rc;
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    if (n_rows == 0) return ACB_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (token_bytes == 2) vocab_state_launch<uint16_t>(dev_image, dev_tokens, n_tokens, dev_offsets, n_rows, dev_state, d.sms, st);
+    else if (token_bytes == 4) vocab_state_launch<int32_t>(dev_image, dev_tokens, n_tokens, dev_offsets, n_rows, dev_state, d.sms, st);
+    else vocab_state_launch<int64_t>(dev_image, dev_tokens, n_tokens, dev_offsets, n_rows, dev_state, d.sms, st);
+    if (logits_dtype == ACB_LOGITS_F32) vocab_mask_launch<float>(filt, dev_image, dev_state, n_rows, F, dev_logits, row_stride, vocab, value, st);
+    else if (logits_dtype == ACB_LOGITS_F16) vocab_mask_launch<__half>(filt, dev_image, dev_state, n_rows, F, dev_logits, row_stride, vocab, value, st);
+    else vocab_mask_launch<__nv_bfloat16>(filt, dev_image, dev_state, n_rows, F, dev_logits, row_stride, vocab, value, st);
+    g_launches += 2;
     CUDA_OK(cudaGetLastError());
     return ACB_OK;
 }

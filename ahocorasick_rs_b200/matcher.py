@@ -22,6 +22,10 @@ self-synchronising 3-byte format (include/acb200.h) and searched as bytes, posit
 ``completing_tokens`` / ``completing_tokens_batch`` / ``completing_tokens_device`` and ``mask_completing_tokens_`` give
 the next ids that would complete a pattern (a bad-words logits processor) from a token-level kernel of their own, and
 ``bias_completing_tokens_`` adds a bias per pattern to them (a sequence-bias logits processor).
+
+``vocabulary(entries)`` of ``AhoCorasick`` / ``BytesAhoCorasick`` binds a tokenizer's byte strings to the patterns: its
+``mask_completing_tokens_`` bans every next token whose bytes would complete a string pattern, however the model spells
+it (``TokenVocabulary``).
 """
 from __future__ import annotations
 
@@ -2272,6 +2276,243 @@ class _PatternSetMethods:
         return _filter_args(self._ac, pattern_sets, set_index, offsets.numel() - 1, data.device)
 
 
+_LOGITS_DTYPES = {"float32": _capi.ACB_LOGITS_F32, "float16": _capi.ACB_LOGITS_F16, "bfloat16": _capi.ACB_LOGITS_BF16}
+
+
+def _history_args(ac: "_Automaton", tokens, offsets, pattern_sets, set_index):
+    """The checks of a logits processor's histories, none of which reads the device: -> (tokens, offsets, n, filter)."""
+    torch = _torch()
+    if (not torch.is_tensor(tokens) or tokens.dim() != 1 or tokens.device.type != "cuda" or
+            tokens.dtype not in (torch.uint16, torch.int32, torch.int64)):
+        raise TypeError("tokens must be a 1-D CUDA tensor of uint16, int32 or int64 token ids")
+    if not torch.is_tensor(offsets) or offsets.dtype != torch.int64 or offsets.dim() != 1 or offsets.numel() < 1:
+        raise TypeError("offsets must be a 1-D int64 tensor of n + 1 token offsets")
+    if offsets.device != tokens.device:
+        raise ValueError(f"offsets live on {offsets.device}, the tokens on {tokens.device}")
+    n = offsets.numel() - 1
+    flt = _filter_shape_args(ac, pattern_sets, set_index, n, tokens.device)
+    _require_cuda()
+    return tokens.contiguous(), offsets.contiguous(), n, flt
+
+
+def _logits_shape(logits, tokens, n: int):
+    """The logits checks of a logits processor, none of which reads the device: -> (dtype code, V)."""
+    torch = _torch()
+    code = _LOGITS_DTYPES.get(str(logits.dtype).replace("torch.", "")) if torch.is_tensor(logits) else None
+    if code is None or logits.dim() != 2:
+        raise TypeError("logits must be a 2-D float32, float16 or bfloat16 tensor (n, V)")
+    if logits.device != tokens.device:
+        raise ValueError(f"logits live on {logits.device}, the tokens on {tokens.device}")
+    V = int(logits.shape[1])
+    if logits.shape[0] != n:
+        raise ValueError(f"logits have {logits.shape[0]} rows, offsets describe {n} histories")
+    if V < 1:
+        raise ValueError("logits need at least one column")
+    if logits.stride(1) != 1 and V > 1:
+        raise ValueError("logits rows must be contiguous (stride(1) == 1); any row stride is fine")
+    return code, V
+
+
+def _history_ids(seq, what: str) -> np.ndarray:
+    """One 1-D integer sequence (list, tuple, numpy array, CPU tensor) -> int64 numpy array.  Any value is kept: the
+    vocabulary forms read an id outside [0, n_vocab) as a break."""
+    torch = __import__("sys").modules.get("torch")
+    if torch is not None and torch.is_tensor(seq):
+        if seq.device.type != "cpu":
+            raise TypeError(f"{what}: a CUDA tensor goes to mask_completing_tokens_; this form takes host sequences")
+        seq = seq.detach().numpy()
+    try:
+        a = np.asarray(seq)
+    except ValueError as e:   # ragged nesting
+        raise TypeError(f"{what} must be a one-dimensional sequence of token ids") from e
+    if a.ndim != 1:
+        raise TypeError(f"{what} must be a one-dimensional sequence of token ids")
+    if a.size == 0:
+        return np.zeros(0, dtype=np.int64)
+    if a.dtype.kind == "O" and all(isinstance(x, (int, np.integer)) and not isinstance(x, bool) for x in a):
+        # ids beyond int64 are breaks like any other id outside [0, n_vocab)
+        a = np.array([int(x) if -(1 << 63) <= int(x) < (1 << 63) else -1 for x in a], dtype=np.int64)
+    if a.dtype.kind not in "iu":
+        raise TypeError(f"{what} must hold integer token ids, not {a.dtype}")
+    return a.astype(np.int64)
+
+
+class TokenVocabulary:
+    """The byte strings of a tokenizer's ids, bound to one AhoCorasick or BytesAhoCorasick: made by their
+    ``vocabulary(entries)``.  A logits processor that bans every next token whose bytes would complete a string
+    pattern, however the model spells it.
+
+    ``entries[t]`` holds the bytes of id t (bytes-like; it may be empty).  A row's history is a run of ids; an id
+    outside [0, n_vocab) (a negative pad, say) is a break: it decodes to nothing and no occurrence may span it, and an
+    empty entry adds nothing.  With T the history's bytes after its last break, id t COMPLETES a pattern when some
+    admitted pattern occurs in T + entries[t] with its end inside entries[t]: a Standard overlapping search of
+    T + entries[t] has a match ending past len(T).  So a token that holds a pattern is banned after every history, an
+    empty entry never is, and the answer does not depend on the automaton's match kind.  ``AhoCorasick`` patterns are
+    matched as UTF-8 bytes, so a character split across two tokens is still found.  Masking before every sampling step
+    keeps every sampled token from ending a pattern in the decoded text after the prompt.
+
+        ac = BytesAhoCorasick([b"damn", b"\nUser:"])
+        v = ac.vocabulary([b"d", b"am", b"n", b"damn", b"\n", b"User", b":", b"hello"])
+        v.completing_tokens([0, 1])       # [2, 3]: "dam" + "n"; "damn" holds the string itself
+        v.completing_tokens([4, 5])       # [3, 6]: "\nUser" + ":"
+        v.completing_tokens([4, -1, 5])   # [3]: -1 is a break, so "\nUser:" cannot span it
+
+    The image (csrc/vocab.h: a Standard DFA, each id's bytes and the last byte at which its own bytes enter a match
+    state) is built on the first call on a device and kept there; so is each thread's per-row state buffer, which only
+    grows (include/acb200.h, acb_vocab_*)."""
+
+    def __init__(self, ac: "_Automaton", entries):
+        if isinstance(entries, (str, bytes, bytearray, memoryview)):
+            raise TypeError("entries must be a sequence of bytes-like objects, one per token id")
+        chunks = []
+        for t, e in enumerate(iter(entries)):
+            if isinstance(e, str):
+                raise TypeError(f"entry {t} is a str: a tokenizer's display form (such as 'Ġ') is not the token's bytes; "
+                                "map it to bytes first")
+            chunks.append(bytes(_as_buffer_bytes(e)))
+        n = len(chunks)
+        offs = np.zeros(n + 1, dtype=np.uint64)
+        if n:
+            np.cumsum(np.fromiter((len(c) for c in chunks), dtype=np.uint64, count=n), out=offs[1:])
+        self._ac = ac
+        self._offsets = offs
+        self._blob = np.frombuffer(b"".join(chunks) or b"\0", dtype=np.uint8)
+        self._lens = np.diff(offs).astype(np.int64)
+        self.n_vocab = n
+        nbytes = C.c_uint64(0)
+        rc = ac._L.acb_vocab_build(ac._h, self._blob.ctypes.data, offs.ctypes.data, n, C.byref(nbytes))
+        if rc == _capi.ACB_EINVAL:
+            raise ValueError(_capi.last_error())
+        _check(rc)
+        self.image_bytes = int(nbytes.value)
+        self._images = {}    # device index -> (uint8 tensor, VocabDesc)
+        self._lock = threading.Lock()
+        self._tls = threading.local()   # .states: device index -> the calling thread's u32 state buffer
+
+    @property
+    def last_stats(self):
+        return self._ac.last_stats
+
+    def image(self, device):
+        """(device tensor, VocabDesc) of the vocabulary image on `device`, built and uploaded once."""
+        torch = _require_cuda()
+        idx = device.index if device.index is not None else torch.cuda.current_device()
+        with self._lock:
+            ent = self._images.get(idx)
+            if ent is None:
+                host = np.zeros(self.image_bytes, dtype=np.uint8)
+                _check(self._ac._L.acb_vocab_write(self._ac._h, self._blob.ctypes.data, self._offsets.ctypes.data, self.n_vocab,
+                                                   host.ctypes.data, self.image_bytes))
+                desc = _capi.VocabDesc()
+                _check(self._ac._L.acb_vocab_describe(host.ctypes.data, C.byref(desc)))
+                ent = (torch.from_numpy(host).to(torch.device("cuda", idx)), desc)
+                self._images[idx] = ent
+        return ent
+
+    def _state(self, device, n: int):
+        """The calling thread's per-row state buffer on `device`, at least n entries: grown, never shrunk, so after the
+        first call of a given row count nothing is allocated (the call can be captured in a CUDA graph).  A buffer that
+        a larger call replaces is kept, not freed: a graph captured with it goes on writing there on replay, so its
+        memory must never pass to another tensor (4 bytes per row, at most a doubling chain per thread)."""
+        torch = _torch()
+        states = getattr(self._tls, "states", None)
+        if states is None:
+            states = self._tls.states = {}
+            self._tls.retired = []
+        buf = states.get(device.index)
+        if buf is None or buf.numel() < n:
+            if buf is not None:
+                self._tls.retired.append(buf)
+            buf = states[device.index] = torch.empty(max(n, 1), dtype=torch.int32, device=device)
+        return buf
+
+    def _stats(self, desc):
+        self._ac.last_stats = {"mode": "vocab_completions", "n_vocab": int(desc.n_vocab), "states": int(desc.states),
+                               "columns": int(desc.columns), "max_pattern_len": int(desc.max_pattern_len),
+                               "extra_dfa_bytes": int(desc.extra_dfa_bytes), "tail_hit_ids": int(desc.tail_hit_ids)}
+
+    def mask_completing_tokens_(self, logits, tokens, offsets, pattern_sets=None, set_index=None, value: float = float("-inf")):
+        """In place: logits[i, t] = value for every id t < min(V, n_vocab) whose bytes complete a pattern for row i;
+        every other element (columns at or above n_vocab included) is untouched.  Returns `logits`.
+
+        ``logits``: float32 / float16 / bfloat16 CUDA tensor (n, V) with stride(1) == 1 and any row stride (so
+        ``scores[:, -1, :]`` works); any V >= 1.  ``tokens``: 1-D uint16 / int32 / int64 CUDA tensor; ``offsets``: int64
+        (n + 1,) in tokens -- an (n, L) ``input_ids`` tensor is ``ids.reshape(-1)`` with ``offsets = arange(n + 1) * L``.
+        Offsets are clamped to [0, len(tokens)], not validated, and b < a is an empty history.  ``pattern_sets`` /
+        ``set_index`` (n,): each row's own set, from the automaton's ``pattern_sets()``; an index outside [0, n_sets)
+        bans nothing.  Nothing is read back, and after the first call of a given row count (which builds and uploads the
+        image) nothing is allocated for contiguous inputs: the call can be captured in a CUDA graph.  Graphs captured
+        for several batch sizes on one thread stay valid: the per-row state buffer each one writes is never freed while
+        this object lives."""
+        tokens, offsets, n, flt = _history_args(self._ac, tokens, offsets, pattern_sets, set_index)
+        code, V = _logits_shape(logits, tokens, n)
+        torch = _torch()
+        dev = tokens.device
+        img, desc = self.image(dev)
+        state = self._state(torch.device("cuda", dev.index if dev.index is not None else torch.cuda.current_device()), n)
+        with torch.cuda.device(dev):
+            rc = self._ac._L.acb_vocab_mask(self._ac._h, img.data_ptr(), tokens.data_ptr(), tokens.element_size(), tokens.numel(),
+                                            offsets.data_ptr(), n, state.data_ptr(), logits.data_ptr(), code,
+                                            logits.stride(0) if n > 1 else V, V, float(value), _filter_struct(flt),
+                                            torch.cuda.current_stream(dev).cuda_stream)
+        _check(rc)
+        self._stats(desc)
+        return logits
+
+    def completing_tokens(self, history, patterns=None) -> list:
+        """-> the sorted distinct ids whose bytes complete a pattern (of `patterns`, when given) after `history`, a
+        1-D sequence of ids (any integers: those outside [0, n_vocab) are breaks)."""
+        return self.completing_tokens_batch([history], _one_set(patterns))[0]
+
+    ROWS_ELEMENTS = 1 << 26   # completing_tokens_batch: rows per device batch x n_vocab stays below this
+
+    def completing_tokens_batch(self, histories: Sequence, patterns=None) -> list:
+        """One sorted list of completing ids per history (``completing_tokens`` of each); `patterns`: one iterable of
+        pattern ids per history.  The bytes of each history that can matter (after its last break, the last
+        max_pattern_len - 1) go to the device in one batch, the mask is applied to a zero float32 (n, n_vocab) tensor,
+        and its nonzero entries are the ids."""
+        hists = [_history_ids(h, f"history {i}") for i, h in enumerate(histories)]
+        n = len(hists)
+        sets = _batch_sets(patterns, n)
+        if n == 0:
+            return []
+        torch = _require_cuda()
+        dev = torch.device("cuda", torch.cuda.current_device())
+        if self.n_vocab == 0:
+            if sets is not None:
+                _host_sets(self._ac, sets, n, dev)   # the same checks of patterns=
+            self._stats(self.image(dev)[1])
+            return [[] for _ in range(n)]
+        need = max(self._ac.max_pattern_len - 1, 0)
+        tails = []
+        for ids in hists:
+            brk = np.flatnonzero((ids < 0) | (ids >= self.n_vocab))
+            t = ids[brk[-1] + 1:] if brk.size else ids
+            if need == 0:
+                t = t[:0]
+            elif t.size:
+                cum = np.cumsum(self._lens[t[::-1]])
+                k = int(np.searchsorted(cum, need))   # the last k + 1 ids hold `need` bytes
+                t = t[t.size - 1 - k:] if k < t.size else t
+            tails.append(t)
+        out = []
+        step = max(1, self.ROWS_ELEMENTS // self.n_vocab)
+        for a in range(0, n, step):
+            b = min(n, a + step)
+            offs = np.zeros(b - a + 1, dtype=np.int64)
+            np.cumsum([t.size for t in tails[a:b]], out=offs[1:])
+            with torch.cuda.device(dev):
+                tokens = torch.from_numpy(np.concatenate(tails[a:b])).to(dev)
+                flt = None if sets is None else _host_sets(self._ac, sets[a:b], b - a, dev)
+                mask = torch.zeros((b - a, self.n_vocab), dtype=torch.float32, device=dev)
+                ps, idx = (None, None) if flt is None else flt
+                self.mask_completing_tokens_(mask, tokens, torch.from_numpy(offs).to(dev), ps, idx, 1.0)
+                hit = torch.nonzero(mask).cpu().numpy()
+            rows = np.searchsorted(hit[:, 0], np.arange(b - a + 1))
+            out += [hit[rows[i]:rows[i + 1], 1].tolist() for i in range(b - a)]
+        return out
+
+
 class AhoCorasick(_PatternSetMethods):
     """Search for multiple pattern strings against a haystack string
     (reference: src/lib.rs:15-33, 134-273).
@@ -2314,6 +2555,11 @@ class AhoCorasick(_PatternSetMethods):
             encoded.append(b)
         self._patterns = strs if store else None
         self._ac = _Automaton(encoded, matchkind, implementation)
+
+    def vocabulary(self, entries) -> TokenVocabulary:
+        """A TokenVocabulary over this automaton's patterns, matched as UTF-8 bytes: ``entries[t]`` is the bytes of
+        token id t (bytes-like; a str is a TypeError, as a tokenizer's display form is not the token's bytes)."""
+        return TokenVocabulary(self._ac, entries)
 
     def find_matches_as_indexes(self, haystack: str, overlapping: bool = False, patterns=None):
         """-> list of (pattern index, start, end) in code points (src/lib.rs:229-249).  `patterns`: search only for
@@ -2566,6 +2812,11 @@ class BytesAhoCorasick(_PatternSetMethods):
                 raise ValueError("You passed in an empty pattern")
             encoded.append(b)
         self._ac = _Automaton(encoded, matchkind, implementation)
+
+    def vocabulary(self, entries) -> TokenVocabulary:
+        """A TokenVocabulary over this automaton's patterns: ``entries[t]`` is the bytes of token id t (bytes-like; a
+        str is a TypeError, as a tokenizer's display form is not the token's bytes)."""
+        return TokenVocabulary(self._ac, entries)
 
     def find_matches_as_indexes(self, haystack, overlapping: bool = False, patterns=None):
         """-> list of (pattern index, start, end) in byte offsets (src/lib.rs:422-434).  `patterns`: search only for
@@ -3173,18 +3424,7 @@ class TokenAhoCorasick(_PatternSetMethods):
     # the completions image (csrc/completions.h) backwards over those ids (include/acb200.h, acb_completions_*).
     def _completions_args(self, tokens, offsets, pattern_sets, set_index):
         """The device forms' checks, none of which reads the device: -> (tokens, offsets, n, filter)."""
-        torch = _torch()
-        if (not torch.is_tensor(tokens) or tokens.dim() != 1 or tokens.device.type != "cuda" or
-                tokens.dtype not in (torch.uint16, torch.int32, torch.int64)):
-            raise TypeError("tokens must be a 1-D CUDA tensor of uint16, int32 or int64 token ids")
-        if not torch.is_tensor(offsets) or offsets.dtype != torch.int64 or offsets.dim() != 1 or offsets.numel() < 1:
-            raise TypeError("offsets must be a 1-D int64 tensor of n + 1 token offsets")
-        if offsets.device != tokens.device:
-            raise ValueError(f"offsets live on {offsets.device}, the tokens on {tokens.device}")
-        n = offsets.numel() - 1
-        flt = _filter_shape_args(self._ac, pattern_sets, set_index, n, tokens.device)
-        _require_cuda()
-        return tokens.contiguous(), offsets.contiguous(), n, flt
+        return _history_args(self._ac, tokens, offsets, pattern_sets, set_index)
 
     def _completions_stats(self, desc):
         self._ac.last_stats = {"mode": "completions", "nodes": int(desc.nodes), "entries": int(desc.entries)}
@@ -3251,7 +3491,7 @@ class TokenAhoCorasick(_PatternSetMethods):
         self._completions_stats(desc)
         return ids, row_offsets
 
-    _LOGITS_DTYPES = {"float32": _capi.ACB_LOGITS_F32, "float16": _capi.ACB_LOGITS_F16, "bfloat16": _capi.ACB_LOGITS_BF16}
+    _LOGITS_DTYPES = _LOGITS_DTYPES
 
     def mask_completing_tokens_(self, logits, tokens, offsets, pattern_sets=None, set_index=None, value: float = float("-inf")):
         """In place: logits[i, t] = value for every id t that completes a pattern for row i (the bad-words logits
@@ -3279,19 +3519,7 @@ class TokenAhoCorasick(_PatternSetMethods):
     def _logits_args(self, logits, tokens, n: int):
         """The logits checks of the mask and the bias, none of which reads the device, and the vocabulary check against
         the image's largest last id (on the host): -> (dtype code, V, image, desc)."""
-        torch = _torch()
-        code = self._LOGITS_DTYPES.get(str(logits.dtype).replace("torch.", "")) if torch.is_tensor(logits) else None
-        if code is None or logits.dim() != 2:
-            raise TypeError("logits must be a 2-D float32, float16 or bfloat16 tensor (n, V)")
-        if logits.device != tokens.device:
-            raise ValueError(f"logits live on {logits.device}, the tokens on {tokens.device}")
-        V = int(logits.shape[1])
-        if logits.shape[0] != n:
-            raise ValueError(f"logits have {logits.shape[0]} rows, offsets describe {n} histories")
-        if V < 1:
-            raise ValueError("logits need at least one column")
-        if logits.stride(1) != 1 and V > 1:
-            raise ValueError("logits rows must be contiguous (stride(1) == 1); any row stride is fine")
+        code, V = _logits_shape(logits, tokens, n)
         img, desc = self._ac.completions(tokens.device)
         if desc.entries and desc.max_last >= V:
             raise ValueError(f"logits have {V} columns, but id {desc.max_last} ends a pattern: V must exceed every pattern's last id")

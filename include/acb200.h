@@ -764,6 +764,59 @@ int acb_completions_bias(const acb_automaton *a, const void *dev_image, const vo
                          int64_t row_stride, int64_t vocab, const acb_pattern_filter *filter, void *stream);
 
 /*
+ * Vocabulary masks: for each row of token-id histories, the next ids whose BYTES would complete a pattern of a byte
+ * (or UTF-8 string) automaton.  A vocabulary is n_vocab byte strings: vocab[t] holds the bytes of id t (an entry may
+ * be empty).  Row i's history C is dev_tokens[a, b), clamped exactly as for acb_completions_mask.  An id outside
+ * [0, n_vocab) (a negative pad, say) is a BREAK: it decodes to nothing and no occurrence may span it.  An empty entry
+ * neither breaks nor adds bytes.  T = the bytes of C after its last break (only its last max_pattern_len - 1 bytes can
+ * matter).  Id t COMPLETES a pattern for the row when some admitted pattern (all, or with a filter the row's set)
+ * occurs in T || vocab[t] with its end inside vocab[t]: a Standard overlapping search of T || vocab[t] by an automaton
+ * of the admitted patterns has a match ending past len(T).  So a token that holds a pattern is banned after every
+ * history, an empty entry never is, and the answer does not depend on the automaton's match kind.  The candidates are
+ * t < min(vocab, n_vocab): columns at or above n_vocab are never written; ids at or above vocab still decode in
+ * histories.  Masking before every sampling step keeps every sampled token from ending a pattern in the decoded text.
+ *
+ * The vocabulary image (csrc/vocab.h) holds a Standard dense DFA (a copy of the automaton's own when its kind is
+ * Standard; otherwise one built once from its patterns and kept with the automaton), the depth of every state, each
+ * id's offset and length, each id's tail_hit (the last byte at which the walk from the root over vocab[t] enters a
+ * match state, -1 for none) and the entry bytes.  blob holds the entries back to back, entry t at
+ * blob[offsets[t], offsets[t + 1]); offsets = u64[n_vocab + 1] with offsets[0] = 0, non-decreasing.  The format's 32-bit
+ * index widths hold at most ACB_VOCAB_MAX_IDS ids and ACB_VOCAB_MAX_BYTES entry bytes.  acb_vocab_build checks the
+ * vocabulary and writes the image's size to *image_bytes (it reads the offsets, not the bytes); acb_vocab_write writes
+ * the image (ACB_ECAPACITY when dst_bytes is short); the caller uploads it and passes the device pointer as dev_image.
+ * acb_vocab_describe reads a host copy: n_vocab, the DFA's states and columns, max_pattern_len, the bytes of a DFA
+ * built for the vocabulary (0 when it copies the automaton's own) and the ids with tail_hit >= 0.  ACB_EINVAL for a
+ * null pointer (blob may be null when the entries hold no bytes), n_vocab above ACB_VOCAB_MAX_IDS, offsets[0] != 0,
+ * decreasing offsets or more than ACB_VOCAB_MAX_BYTES bytes; ACB_EBUILD when the Standard DFA cannot be built.
+ *
+ * acb_vocab_mask writes logits[i * row_stride + t] = value (rounded to the logits dtype) for every completing id t of
+ * row i; every other element is untouched.  dev_image must be the upload of acb_vocab_write(a, ...) for this `a`.
+ * dev_state = u32[n_rows], the caller's scratch (the rows' DFA states between the two launches).  Logits as for
+ * acb_completions_mask; any vocab >= 1 is valid.  Two launches (the rows' states, then the mask), no synchronisation,
+ * no allocation.  ACB_EINVAL, before any CUDA call: a null pointer (dev_tokens may be null when n_tokens == 0, the
+ * per-row pointers when n_rows == 0), token_bytes not 2, 4 or 8, n_tokens >= 2^60, n_rows outside [0, 2^32 - 2], a
+ * malformed filter or one of 2^32 - 1 sets or more, a logits_dtype not listed, vocab outside [1, 2^62) or row_stride
+ * outside [0, 2^62).  n_rows == 0 launches nothing.
+ */
+#define ACB_VOCAB_MAX_IDS 0x7fffffffull
+#define ACB_VOCAB_MAX_BYTES 0x7fffffffull
+typedef struct acb_vocab_desc {
+    uint32_t n_vocab;
+    uint32_t states;            /* of the Standard DFA */
+    uint32_t columns;
+    uint32_t max_pattern_len;   /* bytes; 0 without patterns */
+    uint64_t extra_dfa_bytes;   /* a DFA built for the vocabulary (the automaton's kind is not Standard); 0 otherwise */
+    uint32_t tail_hit_ids;      /* ids whose own bytes enter a match state from the root */
+    uint32_t reserved;
+} acb_vocab_desc;
+int acb_vocab_build(acb_automaton *a, const uint8_t *blob, const uint64_t *offsets, uint64_t n_vocab, uint64_t *image_bytes);
+int acb_vocab_write(acb_automaton *a, const uint8_t *blob, const uint64_t *offsets, uint64_t n_vocab, void *host_dst, uint64_t dst_bytes);
+int acb_vocab_describe(const void *host_image, acb_vocab_desc *desc);
+int acb_vocab_mask(const acb_automaton *a, const void *dev_image, const void *dev_tokens, int token_bytes, uint64_t n_tokens,
+                   const int64_t *dev_offsets, int64_t n_rows, uint32_t *dev_state, void *dev_logits, int logits_dtype, int64_t row_stride,
+                   int64_t vocab, float value, const acb_pattern_filter *filter, void *stream);
+
+/*
  * Multi-GPU: the fixed-size block a rank contributes to the gather of the per-shard match lists (the only exchange
  * of the sharded path; NCCL all-gather over NVLink).  dev_block holds (cap + 1) records of 16 bytes: record 0 =
  * (match count, hay_base, complete flag, 0), then the first `cap` matches of a finished scan (dev_total / dev_out of
