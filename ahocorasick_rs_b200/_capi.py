@@ -171,6 +171,7 @@ def lib():
         L.acb_vocab_write.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]
         L.acb_vocab_describe.argtypes = [C.c_void_p, C.POINTER(VocabDesc)]
         L.acb_vocab_mask.argtypes = compl + [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_float, F, C.c_void_p]
+        L.acb_vocab_stop.argtypes = compl + [C.c_int64, C.c_void_p, C.c_void_p, F, C.c_void_p]
         _lib = L
     return _lib
 
@@ -213,4 +214,5 @@ EXPORTS = [
     "acb_match_mask_non_overlapping_filtered", "acb_mask_rows", "acb_mask_unpack", "acb_stream_mask_rows", "acb_stream_mask_emit",
     "acb_completions_build", "acb_completions_write", "acb_completions_describe", "acb_completions_count", "acb_completions_emit",
     "acb_completions_mask", "acb_completions_bias", "acb_vocab_build", "acb_vocab_write", "acb_vocab_describe", "acb_vocab_mask",
+    "acb_vocab_stop",
 ]

@@ -4174,6 +4174,16 @@ static int vocab_args(const acb_automaton *a, const uint8_t *blob, const uint64_
     return ACB_OK;
 }
 
+// the checks every vocabulary entry point over rows of ids makes, before any CUDA call; the filter view
+static int vocab_rows_check(const acb_automaton *a, const void *dev_image, const void *dev_tokens, int token_bytes, uint64_t n_tokens,
+                            const int64_t *dev_offsets, int64_t n_rows, const acb_pattern_filter *filter, SieveFilter &F, bool &filt) {
+    if (!a || !dev_image || (n_tokens && !dev_tokens) || (n_rows && !dev_offsets)) return fail(ACB_EINVAL, "null argument");
+    if (token_bytes != 2 && token_bytes != 4 && token_bytes != 8) return fail(ACB_EINVAL, "token_bytes must be 2, 4 or 8");
+    if (n_tokens >= (1ull << 60)) return fail(ACB_EINVAL, "n_tokens must be below 2^60");
+    if (n_rows < 0 || n_rows > 0xfffffffell) return fail(ACB_EINVAL, "n_rows out of range (0 .. 2^32 - 2)");
+    return filter_view(a, filter, n_rows, F, filt);
+}
+
 template <typename T>
 static void vocab_state_launch(const void *img, const void *tokens, uint64_t n_tokens, const int64_t *offsets, int64_t n_rows,
                                uint32_t *state, int sms, cudaStream_t st) {
@@ -4197,6 +4207,18 @@ static void vocab_mask_launch(bool filt, const void *img, const uint32_t *state,
     else
         vocab_mask_kernel<L, false><<<grid, kVocabThreads, 0, st>>>(static_cast<const uint8_t *>(img), state, n_rows, F,
                                                                     static_cast<L *>(logits), row_stride, vocab, value);
+}
+
+template <typename T>
+static void vocab_stop_launch(bool filt, const void *img, const void *tokens, uint64_t n_tokens, const int64_t *offsets, int64_t n_rows,
+                              int64_t n_new, const int64_t *news, const SieveFilter &F, int64_t *out, int sms, cudaStream_t st) {
+    constexpr int64_t kWarps = kVocabThreads / 32;
+    int64_t blocks = (n_rows + kWarps - 1) / kWarps;
+    if (blocks > 32ll * sms) blocks = 32ll * sms;   // grid-stride beyond that
+    const uint8_t *i = static_cast<const uint8_t *>(img);
+    const T *t = static_cast<const T *>(tokens);
+    if (filt) vocab_stop_kernel<T, true><<<(unsigned)blocks, kVocabThreads, 0, st>>>(i, t, n_tokens, offsets, n_rows, n_new, news, F, out);
+    else vocab_stop_kernel<T, false><<<(unsigned)blocks, kVocabThreads, 0, st>>>(i, t, n_tokens, offsets, n_rows, n_new, news, F, out);
 }
 
 extern "C" {
@@ -4239,13 +4261,10 @@ int acb_vocab_describe(const void *host_image, acb_vocab_desc *d) {
 int acb_vocab_mask(const acb_automaton *a, const void *dev_image, const void *dev_tokens, int token_bytes, uint64_t n_tokens,
                    const int64_t *dev_offsets, int64_t n_rows, uint32_t *dev_state, void *dev_logits, int logits_dtype, int64_t row_stride,
                    int64_t vocab, float value, const acb_pattern_filter *filter, void *stream) {
-    if (!a || !dev_image || (n_tokens && !dev_tokens) || (n_rows && (!dev_offsets || !dev_state))) return fail(ACB_EINVAL, "null argument");
-    if (token_bytes != 2 && token_bytes != 4 && token_bytes != 8) return fail(ACB_EINVAL, "token_bytes must be 2, 4 or 8");
-    if (n_tokens >= (1ull << 60)) return fail(ACB_EINVAL, "n_tokens must be below 2^60");
-    if (n_rows < 0 || n_rows > 0xfffffffell) return fail(ACB_EINVAL, "n_rows out of range (0 .. 2^32 - 2)");
     SieveFilter F{};
     bool filt = false;
-    if (int rc = filter_view(a, filter, n_rows, F, filt)) return rc;
+    if (int rc = vocab_rows_check(a, dev_image, dev_tokens, token_bytes, n_tokens, dev_offsets, n_rows, filter, F, filt)) return rc;
+    if (n_rows && !dev_state) return fail(ACB_EINVAL, "null argument");
     if (filt && F.n_sets >= kVocabNoSet) return fail(ACB_EINVAL, "pattern filter: n_sets must be below 2^32 - 1");
     if (int rc = logits_check(n_rows, dev_logits, logits_dtype, row_stride, vocab)) return rc;
     DeviceInfo d;
@@ -4259,6 +4278,26 @@ int acb_vocab_mask(const acb_automaton *a, const void *dev_image, const void *de
     else if (logits_dtype == ACB_LOGITS_F16) vocab_mask_launch<__half>(filt, dev_image, dev_state, n_rows, F, dev_logits, row_stride, vocab, value, st);
     else vocab_mask_launch<__nv_bfloat16>(filt, dev_image, dev_state, n_rows, F, dev_logits, row_stride, vocab, value, st);
     g_launches += 2;
+    CUDA_OK(cudaGetLastError());
+    return ACB_OK;
+}
+
+int acb_vocab_stop(const acb_automaton *a, const void *dev_image, const void *dev_tokens, int token_bytes, uint64_t n_tokens,
+                   const int64_t *dev_offsets, int64_t n_rows, int64_t n_new, const int64_t *dev_new, int64_t *dev_out,
+                   const acb_pattern_filter *filter, void *stream) {
+    SieveFilter F{};
+    bool filt = false;
+    if (int rc = vocab_rows_check(a, dev_image, dev_tokens, token_bytes, n_tokens, dev_offsets, n_rows, filter, F, filt)) return rc;
+    if (n_rows && !dev_out) return fail(ACB_EINVAL, "null argument");
+    if (!dev_new && n_new < 0) return fail(ACB_EINVAL, "n_new must be >= 0 when dev_new is null");
+    DeviceInfo d;
+    if (int rc = device_info(d)) return rc;
+    if (n_rows == 0) return ACB_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (token_bytes == 2) vocab_stop_launch<uint16_t>(filt, dev_image, dev_tokens, n_tokens, dev_offsets, n_rows, n_new, dev_new, F, dev_out, d.sms, st);
+    else if (token_bytes == 4) vocab_stop_launch<int32_t>(filt, dev_image, dev_tokens, n_tokens, dev_offsets, n_rows, n_new, dev_new, F, dev_out, d.sms, st);
+    else vocab_stop_launch<int64_t>(filt, dev_image, dev_tokens, n_tokens, dev_offsets, n_rows, n_new, dev_new, F, dev_out, d.sms, st);
+    g_launches++;
     CUDA_OK(cudaGetLastError());
     return ACB_OK;
 }

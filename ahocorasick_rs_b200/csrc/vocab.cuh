@@ -19,6 +19,9 @@
 // step can hit, and otherwise the walk goes on to byte tail_hit[t] checking the admitted outputs.  A row whose set index
 // lies outside [0, n_sets) bans nothing.  Banned pairs get `value` (compl_value rounding); nothing else is written.  A
 // thread decides its candidate for all the tile's rows first, into one bit per row, and then stores.
+//
+// vocab_stop_kernel (acb_vocab_stop): each row's first new id whose bytes end an admitted pattern, by the same
+// backwards decode (vocab_tail) and a forward walk over the new ids (below).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -69,6 +72,63 @@ __device__ __forceinline__ VocabView vocab_view(const uint8_t *img) {
     return v;
 }
 
+// The bytes before index `end` of a row whose ids before `end` number `cnt` that can matter: the warp reads the ids
+// backwards from end - 1 in lane-sized pieces, summing entry lengths (a warp prefix sum) until it holds need =
+// max_pattern_len - 1 bytes, meets a break or has read all `cnt`.  On return every lane holds `start`, the first id a
+// forward walk reads, and `skip`, the bytes of that id it skips; start == end when need is 0.
+template <typename T>
+__device__ __forceinline__ void vocab_tail(const VocabView &V, const T *__restrict__ tokens, uint64_t end, uint64_t cnt, int lane,
+                                           uint64_t &start, uint32_t &skip) {
+    start = end;
+    skip = 0;
+    if (!V.need) return;
+    uint64_t have = 0;   // bytes of the ids after this piece
+    for (uint64_t base = 0;; base += 32) {
+        const uint64_t k = base + (uint64_t)lane;   // lane k: the id at end - 1 - k
+        const bool valid = k < cnt;
+        bool brk = false;
+        uint32_t len = 0;
+        if (valid) {
+            const long long id = token_value(tokens[end - 1 - k]);
+            if (id >= 0 && id < (long long)V.n_vocab) len = __ldg(V.recs + id).y;
+            else brk = true;
+        }
+        uint64_t cum = len;   // inclusive prefix sum over the lanes, then the bytes after the piece
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint64_t x = __shfl_up_sync(0xffffffffu, cum, o);
+            if (lane >= o) cum += x;
+        }
+        cum += have;
+        const bool reach = valid && !brk && cum >= V.need;
+        const unsigned stop = __ballot_sync(0xffffffffu, !valid || brk || reach);
+        if (stop) {
+            const int f = __ffs(stop) - 1;
+            const uint64_t cf = __shfl_sync(0xffffffffu, cum, f);
+            const bool rf = (__ballot_sync(0xffffffffu, reach) >> f) & 1u;
+            // reached: the id at lane f is the first, minus the bytes beyond `need`; otherwise the walk
+            // starts after lane f (a break, or the row start)
+            start = end - 1 - (base + (uint64_t)f) + (rf ? 0 : 1);
+            skip = rf ? (uint32_t)(cf - V.need) : 0u;
+            return;
+        }
+        have = __shfl_sync(0xffffffffu, cum, 31);
+    }
+}
+
+// the state the walk from the root reaches over ids [start, end), from byte `skip` of the first (none is a break)
+template <typename T>
+__device__ __forceinline__ uint32_t vocab_walk(const VocabView &V, const T *__restrict__ tokens, uint64_t start, uint32_t skip,
+                                               uint64_t end) {
+    uint32_t s = kRoot;
+    for (uint64_t i = start; i < end; ++i) {
+        const uint2 rc = __ldg(V.recs + token_value(tokens[i]));   // not a break: the scan stopped before any
+        for (uint32_t j = i == start ? skip : 0u; j < rc.y; ++j)
+            s = __ldg(V.trans + (uint64_t)s * V.n_cols + V.colmap[__ldg(V.bytes + rc.x + j)]) & kStateMask;
+    }
+    return s;
+}
+
 template <typename T>
 __global__ void __launch_bounds__(kVocabThreads) vocab_state_kernel(const uint8_t *__restrict__ img, const T *__restrict__ tokens,
                                                                     uint64_t n_tokens, const int64_t *__restrict__ offsets, int64_t n_rows,
@@ -82,52 +142,10 @@ __global__ void __launch_bounds__(kVocabThreads) vocab_state_kernel(const uint8_
         const uint64_t a = o0 < 0 ? 0 : ((uint64_t)o0 > n_tokens ? n_tokens : (uint64_t)o0);
         uint64_t b = o1 < 0 ? 0 : ((uint64_t)o1 > n_tokens ? n_tokens : (uint64_t)o1);
         if (b < a) b = a;
-        const uint64_t cnt = b - a;
-        uint64_t start = b;   // the first id the walk reads
-        uint32_t skip = 0;    // ... from its byte `skip` on
-        if (V.need) {
-            uint64_t have = 0;   // bytes of the ids after this piece
-            for (uint64_t base = 0;; base += 32) {
-                const uint64_t k = base + (uint64_t)lane;   // lane k: the id at b - 1 - k
-                const bool valid = k < cnt;
-                bool brk = false;
-                uint32_t len = 0;
-                if (valid) {
-                    const long long id = token_value(tokens[b - 1 - k]);
-                    if (id >= 0 && id < (long long)V.n_vocab) len = __ldg(V.recs + id).y;
-                    else brk = true;
-                }
-                uint64_t cum = len;   // inclusive prefix sum over the lanes, then the bytes after the piece
-#pragma unroll
-                for (int o = 1; o < 32; o <<= 1) {
-                    const uint64_t x = __shfl_up_sync(0xffffffffu, cum, o);
-                    if (lane >= o) cum += x;
-                }
-                cum += have;
-                const bool reach = valid && !brk && cum >= V.need;
-                const unsigned stop = __ballot_sync(0xffffffffu, !valid || brk || reach);
-                if (stop) {
-                    const int f = __ffs(stop) - 1;
-                    const uint64_t cf = __shfl_sync(0xffffffffu, cum, f);
-                    const bool rf = (__ballot_sync(0xffffffffu, reach) >> f) & 1u;
-                    // reached: the id at lane f is the first, minus the bytes beyond `need`; otherwise the walk
-                    // starts after lane f (a break, or the row start)
-                    start = b - 1 - (base + (uint64_t)f) + (rf ? 0 : 1);
-                    skip = rf ? (uint32_t)(cf - V.need) : 0u;
-                    break;
-                }
-                have = __shfl_sync(0xffffffffu, cum, 31);
-            }
-        }
-        if (lane == 0) {
-            uint32_t s = kRoot;
-            for (uint64_t i = start; i < b; ++i) {
-                const uint2 rc = __ldg(V.recs + token_value(tokens[i]));   // not a break: the scan stopped before any
-                for (uint32_t j = i == start ? skip : 0u; j < rc.y; ++j)
-                    s = __ldg(V.trans + (uint64_t)s * V.n_cols + V.colmap[__ldg(V.bytes + rc.x + j)]) & kStateMask;
-            }
-            state[r] = s;
-        }
+        uint64_t start;   // the first id the walk reads
+        uint32_t skip;    // ... from its byte `skip` on
+        vocab_tail(V, tokens, b, b - a, lane, start, skip);
+        if (lane == 0) state[r] = vocab_walk(V, tokens, start, skip, b);
     }
 }
 
@@ -220,6 +238,79 @@ __global__ void __launch_bounds__(kVocabThreads) vocab_mask_kernel(const uint8_t
             // row of the store address was taken from a uniform register (R2UR of the loop counter) while the lanes of
             // a warp were at different rows of their walks, so some bans went to another row of the tile (DESIGN §4.18).
             for (L *col = logits + t; hit; hit &= hit - 1) col[(r0 + (__ffs(hit) - 1)) * row_stride] = fill;
+        }
+    }
+}
+
+// vocab_stop_kernel: one warp per row, grid-stride.  Row i is clamped as for vocab_state_kernel; its last
+// min(max(new_i, 0), b - a) ids are new (new_i = news[i], or n_new when news is null), the first of them at f.  The warp
+// decodes backwards from f (vocab_tail), then lane 0 walks the DFA from the root over those bytes and on over the new
+// ids' bytes: a break resets the walk to the root, an empty entry adds nothing.  The first entered state with an
+// admitted output ends the walk: the first admitted pid of its output list (own patterns, then suffixes, longest first,
+// ties by ascending pid) is the row's stop, the occurrence with the earliest last byte inside a new id, the longest of
+// those.  out[4i .. 4i + 3] = (pid, token index from a, bytes of that id up to the match's last byte, pattern length),
+// or -1 four times.  The walk over the new ids is serial: meant for a decoding step's few ids, not a whole document.
+// The walk from state s over ids [i, b): a break resets it to the root, an empty entry adds nothing.  True when it
+// enters a state with an admitted output; then i, j and s are that id, its byte and the state.
+template <typename T, bool FILT>
+__device__ __forceinline__ bool vocab_stop_walk(const VocabView &V, const T *__restrict__ tokens, uint32_t s0, uint64_t b,
+                                                const uint32_t *set, uint64_t &i, uint32_t &j, uint32_t &s) {
+    s = s0;
+    for (; i < b; ++i) {
+        const long long id = token_value(tokens[i]);
+        if (id < 0 || id >= (long long)V.n_vocab) {   // a break: no occurrence spans it
+            s = kRoot;
+            continue;
+        }
+        const uint2 rc = __ldg(V.recs + id);
+        for (j = 0; j < rc.y; ++j) {
+            const uint32_t e = __ldg(V.trans + (uint64_t)s * V.n_cols + V.colmap[__ldg(V.bytes + rc.x + j)]);
+            s = e & kStateMask;
+            if (vocab_hit<FILT>(V, e, set)) return true;
+        }
+    }
+    return false;
+}
+
+template <typename T, bool FILT>
+__global__ void __launch_bounds__(kVocabThreads) vocab_stop_kernel(const uint8_t *__restrict__ img, const T *__restrict__ tokens,
+                                                                   uint64_t n_tokens, const int64_t *__restrict__ offsets, int64_t n_rows,
+                                                                   int64_t n_new, const int64_t *__restrict__ news, SieveFilter F,
+                                                                   int64_t *__restrict__ out) {
+    const VocabView V = vocab_view(img);
+    if (!V.ok) return;
+    const uint8_t *dfa = img + __ldg(&reinterpret_cast<const VocabHeader *>(img)->off_dfa);
+    const uint32_t *pat_len = reinterpret_cast<const uint32_t *>(dfa + __ldg(&reinterpret_cast<const ImageHeader *>(dfa)->off_pat_len));
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = (int64_t)gridDim.x * (kVocabThreads / 32);
+    for (int64_t r = (int64_t)blockIdx.x * (kVocabThreads / 32) + (threadIdx.x >> 5); r < n_rows; r += warps) {
+        const int64_t o0 = __ldg(offsets + r), o1 = __ldg(offsets + r + 1);
+        const uint64_t a = o0 < 0 ? 0 : ((uint64_t)o0 > n_tokens ? n_tokens : (uint64_t)o0);
+        uint64_t b = o1 < 0 ? 0 : ((uint64_t)o1 > n_tokens ? n_tokens : (uint64_t)o1);
+        if (b < a) b = a;
+        const int64_t nw = news ? __ldg(news + r) : n_new;
+        const uint64_t f = b - (nw <= 0 ? 0 : ((uint64_t)nw > b - a ? b - a : (uint64_t)nw));   // the first new id
+        uint64_t start;
+        uint32_t skip;
+        vocab_tail(V, tokens, f, f - a, lane, start, skip);
+        if (lane == 0) {
+            const uint32_t *set = FILT ? filter_row(F, r) : nullptr;
+            uint64_t i = f;   // the id, and its byte j, where the walk enters a state with an admitted output
+            uint32_t j = 0, s = kRoot;
+            const bool hit = (!FILT || set) && vocab_stop_walk<T, FILT>(V, tokens, vocab_walk(V, tokens, start, skip, f), b, set, i, j, s);
+            int64_t *o = out + 4 * r;
+            if (hit) {
+                uint32_t k = __ldg(V.match_off + s);   // the first admitted pid of s's output list
+                if (FILT)
+                    while (!filter_admits(set, __ldg(V.match_pid + k))) ++k;
+                const uint32_t pid = __ldg(V.match_pid + k);
+                o[0] = pid;
+                o[1] = (int64_t)(i - a);
+                o[2] = (int64_t)j + 1;
+                o[3] = __ldg(pat_len + pid);
+            } else {
+                o[0] = o[1] = o[2] = o[3] = -1;
+            }
         }
     }
 }

@@ -2349,7 +2349,8 @@ class TokenVocabulary:
     T + entries[t] has a match ending past len(T).  So a token that holds a pattern is banned after every history, an
     empty entry never is, and the answer does not depend on the automaton's match kind.  ``AhoCorasick`` patterns are
     matched as UTF-8 bytes, so a character split across two tokens is still found.  Masking before every sampling step
-    keeps every sampled token from ending a pattern in the decoded text after the prompt.
+    keeps every sampled token from ending a pattern in the decoded text after the prompt.  ``find_stop_device`` is the
+    stop-strings side: each row's first new id whose bytes end a pattern.
 
         ac = BytesAhoCorasick([b"damn", b"\nUser:"])
         v = ac.vocabulary([b"d", b"am", b"n", b"damn", b"\n", b"User", b":", b"hello"])
@@ -2426,8 +2427,8 @@ class TokenVocabulary:
             buf = states[device.index] = torch.empty(max(n, 1), dtype=torch.int32, device=device)
         return buf
 
-    def _stats(self, desc):
-        self._ac.last_stats = {"mode": "vocab_completions", "n_vocab": int(desc.n_vocab), "states": int(desc.states),
+    def _stats(self, desc, mode="vocab_completions"):
+        self._ac.last_stats = {"mode": mode, "n_vocab": int(desc.n_vocab), "states": int(desc.states),
                                "columns": int(desc.columns), "max_pattern_len": int(desc.max_pattern_len),
                                "extra_dfa_bytes": int(desc.extra_dfa_bytes), "tail_hit_ids": int(desc.tail_hit_ids)}
 
@@ -2459,6 +2460,21 @@ class TokenVocabulary:
         self._stats(desc)
         return logits
 
+    def _tail_start(self, ids) -> int:
+        """The index of the first id of `ids` (a host history) whose bytes can matter to what follows it: after its last
+        break, the ids that hold its last max_pattern_len - 1 bytes (len(ids) when that is 0 bytes)."""
+        need = max(self._ac.max_pattern_len - 1, 0)
+        if need == 0:
+            return int(ids.size)
+        brk = np.flatnonzero((ids < 0) | (ids >= self.n_vocab))
+        s = int(brk[-1]) + 1 if brk.size else 0
+        if s < ids.size:
+            cum = np.cumsum(self._lens[ids[s:][::-1]])
+            k = int(np.searchsorted(cum, need))   # the last k + 1 ids hold `need` bytes
+            if k < ids.size - s:
+                s = int(ids.size) - 1 - k
+        return s
+
     def completing_tokens(self, history, patterns=None) -> list:
         """-> the sorted distinct ids whose bytes complete a pattern (of `patterns`, when given) after `history`, a
         1-D sequence of ids (any integers: those outside [0, n_vocab) are breaks)."""
@@ -2483,18 +2499,7 @@ class TokenVocabulary:
                 _host_sets(self._ac, sets, n, dev)   # the same checks of patterns=
             self._stats(self.image(dev)[1])
             return [[] for _ in range(n)]
-        need = max(self._ac.max_pattern_len - 1, 0)
-        tails = []
-        for ids in hists:
-            brk = np.flatnonzero((ids < 0) | (ids >= self.n_vocab))
-            t = ids[brk[-1] + 1:] if brk.size else ids
-            if need == 0:
-                t = t[:0]
-            elif t.size:
-                cum = np.cumsum(self._lens[t[::-1]])
-                k = int(np.searchsorted(cum, need))   # the last k + 1 ids hold `need` bytes
-                t = t[t.size - 1 - k:] if k < t.size else t
-            tails.append(t)
+        tails = [ids[self._tail_start(ids):] for ids in hists]
         out = []
         step = max(1, self.ROWS_ELEMENTS // self.n_vocab)
         for a in range(0, n, step):
@@ -2511,6 +2516,128 @@ class TokenVocabulary:
             rows = np.searchsorted(hit[:, 0], np.arange(b - a + 1))
             out += [hit[rows[i]:rows[i + 1], 1].tolist() for i in range(b - a)]
         return out
+
+    def find_stop_device(self, tokens, offsets, new=1, pattern_sets=None, set_index=None, out=None):
+        """Stop strings: each row's first new id whose bytes end a pattern -> int64 CUDA tensor (n, 4) of
+        (pattern, token, end, length), -1 four times for a row without one.
+
+        Row i is tokens[offsets[i], offsets[i + 1]) (clamped as for ``mask_completing_tokens_``); its last ``new`` ids
+        are new (clamped to [0, the row's length]).  Decoding the row, with each break starting a fresh text, an
+        occurrence of an admitted pattern counts when a Standard overlapping search finds it and its last byte lies in
+        a new id's bytes; it may start in older ids.  The stop is the one with the earliest last byte, then the
+        longest, then the lowest pid.  ``token`` is the index, from the row's start, of the id holding its last byte,
+        ``end`` that id's bytes up to and including it, ``length`` the pattern's bytes.  The answer does not depend on
+        the match kind.  With new = 1, row h + [t] has a stop exactly when ``mask_completing_tokens_`` bans t after h
+        under the same sets.
+
+        ``new``: an int >= 0 for every row, or an int64 CUDA tensor (n,) on the tokens' device (a negative entry is 0).
+        ``pattern_sets`` / ``set_index``: each row's own set; an index outside [0, n_sets) admits nothing.  ``out``: an
+        optional contiguous int64 (n, 4) tensor on that device, written in place.  Nothing is read back, and with
+        ``out=`` and contiguous inputs nothing is allocated after the first call (which uploads the image): the call can
+        be captured in a CUDA graph."""
+        tokens, offsets, n, flt = _history_args(self._ac, tokens, offsets, pattern_sets, set_index)
+        torch = _torch()
+        dev = tokens.device
+        n_new, news = _new_arg(new, n, dev)
+        if out is None:
+            out = torch.empty((n, 4), dtype=torch.int64, device=dev)
+        elif (not torch.is_tensor(out) or out.dtype != torch.int64 or out.dim() != 2 or out.shape[1] != 4 or
+              not out.is_contiguous()):
+            raise TypeError("out must be a contiguous int64 tensor (n, 4)")
+        elif out.device != dev:
+            raise ValueError(f"out lives on {out.device}, the tokens on {dev}")
+        elif out.shape[0] != n:
+            raise ValueError(f"out has {out.shape[0]} rows, offsets describe {n} histories")
+        img, desc = self.image(dev)
+        with torch.cuda.device(dev):
+            rc = self._ac._L.acb_vocab_stop(self._ac._h, img.data_ptr(), tokens.data_ptr(), tokens.element_size(), tokens.numel(),
+                                            offsets.data_ptr(), n, n_new, None if news is None else news.data_ptr(), out.data_ptr(),
+                                            _filter_struct(flt), torch.cuda.current_stream(dev).cuda_stream)
+        _check(rc)
+        self._stats(desc, "vocab_stop")
+        return out
+
+    def find_stop(self, history, new=1, patterns=None):
+        """-> (pattern, token, end, length) of the stop among the last `new` ids of `history` (a 1-D sequence of ids;
+        those outside [0, n_vocab) are breaks), ``token`` an index into `history`; None when there is none.  `patterns`:
+        only these pattern ids count.  As ``find_stop_device``."""
+        return self.find_stop_batch([history], new, _one_set(patterns))[0]
+
+    def find_stop_batch(self, histories: Sequence, new=1, patterns=None) -> list:
+        """``find_stop`` of each history: `new` is an int >= 0 for all of them or one int per history (a negative one
+        is 0), `patterns` one iterable of pattern ids per history.  Each history sends only what can matter to the
+        device: its new ids, and before them the ids holding the last max_pattern_len - 1 bytes after the last break."""
+        hists = [_history_ids(h, f"history {i}") for i, h in enumerate(histories)]
+        n = len(hists)
+        sets = _batch_sets(patterns, n)
+        news = _host_news(new, n)
+        if n == 0:
+            return []
+        torch = _require_cuda()
+        dev = torch.device("cuda", torch.cuda.current_device())
+        if self.n_vocab == 0 or self._ac.max_pattern_len == 0:   # nothing can match: no launch
+            if sets is not None:
+                _host_sets(self._ac, sets, n, dev)   # the same checks of patterns=
+            self._stats(self.image(dev)[1], "vocab_stop")
+            return [None] * n
+        rows, starts, counts = [], [], []
+        for ids, k in zip(hists, news):
+            k = min(max(int(k), 0), int(ids.size))
+            s = self._tail_start(ids[:ids.size - k])
+            rows.append(ids[s:])
+            starts.append(s)
+            counts.append(k)
+        offs = np.zeros(n + 1, dtype=np.int64)
+        np.cumsum([r.size for r in rows], out=offs[1:])
+        with torch.cuda.device(dev):
+            tokens = torch.from_numpy(np.concatenate(rows)).to(dev)
+            flt = None if sets is None else _host_sets(self._ac, sets, n, dev)
+            ps, idx = (None, None) if flt is None else flt
+            res = self.find_stop_device(tokens, torch.from_numpy(offs).to(dev), torch.tensor(counts, dtype=torch.int64, device=dev),
+                                        ps, idx).cpu().numpy()
+        return [None if r[0] < 0 else (int(r[0]), int(r[1]) + s, int(r[2]), int(r[3])) for r, s in zip(res, starts)]
+
+
+def _host_news(new, n: int) -> list:
+    """find_stop_batch's new= -> one Python int per history: an int >= 0 for all of them, or one int per history (a
+    list, tuple, numpy array or CPU tensor; any value, clamped later to [0, the history's length])."""
+    torch = __import__("sys").modules.get("torch")
+    if torch is not None and torch.is_tensor(new):
+        if new.device.type != "cpu":
+            raise TypeError("new: a CUDA tensor of per-row counts goes to find_stop_device; this form takes host counts")
+        new = new.tolist()
+    if isinstance(new, (int, np.integer)) and not isinstance(new, bool):
+        if new < 0:
+            raise ValueError(f"new must be >= 0, not {new}")
+        return [int(new)] * n
+    what = "new must be an int >= 0 or one int per history"
+    if isinstance(new, (str, bytes, bytearray)) or not hasattr(new, "__iter__"):
+        raise TypeError(what)
+    news = list(new)
+    if not all(isinstance(k, (int, np.integer)) and not isinstance(k, bool) for k in news):
+        raise TypeError(what)
+    if len(news) != n:
+        raise ValueError(f"new needs one count per history: {n} histories, {len(news)} counts")
+    return [int(k) for k in news]
+
+
+def _new_arg(new, n: int, dev):
+    """find_stop_device's new= -> (n_new, None) for an int, (0, contiguous tensor) for a per-row tensor; reads nothing
+    from the device."""
+    torch = _torch()
+    if torch.is_tensor(new):
+        if new.dtype != torch.int64 or new.dim() != 1 or new.device.type != "cuda":
+            raise TypeError("new must be an int >= 0 or a 1-D int64 CUDA tensor of n new-id counts")
+        if new.device != dev:
+            raise ValueError(f"new lives on {new.device}, the tokens on {dev}")
+        if new.numel() != n:
+            raise ValueError(f"new has {new.numel()} counts, offsets describe {n} histories")
+        return 0, new.contiguous()
+    if not isinstance(new, (int, np.integer)) or isinstance(new, bool):
+        raise TypeError("new must be an int >= 0 or a 1-D int64 CUDA tensor of n new-id counts")
+    if not 0 <= new < (1 << 63):
+        raise ValueError(f"new must be >= 0 (and below 2^63), not {new}")
+    return int(new), None
 
 
 class AhoCorasick(_PatternSetMethods):

@@ -797,6 +797,19 @@ int acb_completions_bias(const acb_automaton *a, const void *dev_image, const vo
  * per-row pointers when n_rows == 0), token_bytes not 2, 4 or 8, n_tokens >= 2^60, n_rows outside [0, 2^32 - 2], a
  * malformed filter or one of 2^32 - 1 sets or more, a logits_dtype not listed, vocab outside [1, 2^62) or row_stride
  * outside [0, 2^62).  n_rows == 0 launches nothing.
+ *
+ * acb_vocab_stop finds each row's stop string: the first of its new ids whose bytes end an admitted pattern.  Row i is
+ * clamped as for acb_vocab_mask; its last n = min(max(new_i, 0), b - a) ids are new, new_i = dev_new[i] (int64[n_rows])
+ * or n_new when dev_new is null, the first at f = (b - a) - n.  Decoding the row (each break starts a fresh text), an
+ * occurrence of an admitted pattern counts when a Standard overlapping search of its break-free text finds it and its
+ * last byte lies in a new id's bytes; it may start in older ids.  The stop is the counted occurrence with the earliest
+ * last byte, then the longest, then the lowest pid.  dev_out = int64[n_rows * 4]: row i gets (pattern, token, end,
+ * length): `token` the index from a of the id holding the match's last byte (>= f), `end` that id's bytes up to and
+ * including it (1 .. its length), `length` the pattern's bytes; -1 four times for none.  The answer does not depend on
+ * the automaton's match kind.  For n = 1, row h || [t] has a stop exactly when acb_vocab_mask bans t after h under the
+ * same filter.  One launch, no synchronisation, no allocation.  ACB_EINVAL, before any CUDA call: a null pointer (as
+ * for acb_vocab_mask; dev_new may be null), token_bytes not 2, 4 or 8, n_tokens >= 2^60, n_rows outside
+ * [0, 2^32 - 2], a malformed filter, or n_new < 0 when dev_new is null.  n_rows == 0 launches nothing.
  */
 #define ACB_VOCAB_MAX_IDS 0x7fffffffull
 #define ACB_VOCAB_MAX_BYTES 0x7fffffffull
@@ -815,6 +828,9 @@ int acb_vocab_describe(const void *host_image, acb_vocab_desc *desc);
 int acb_vocab_mask(const acb_automaton *a, const void *dev_image, const void *dev_tokens, int token_bytes, uint64_t n_tokens,
                    const int64_t *dev_offsets, int64_t n_rows, uint32_t *dev_state, void *dev_logits, int logits_dtype, int64_t row_stride,
                    int64_t vocab, float value, const acb_pattern_filter *filter, void *stream);
+int acb_vocab_stop(const acb_automaton *a, const void *dev_image, const void *dev_tokens, int token_bytes, uint64_t n_tokens,
+                   const int64_t *dev_offsets, int64_t n_rows, int64_t n_new, const int64_t *dev_new, int64_t *dev_out,
+                   const acb_pattern_filter *filter, void *stream);
 
 /*
  * Multi-GPU: the fixed-size block a rank contributes to the gather of the per-shard match lists (the only exchange
